@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — images/sec of the MQ-GLIP-T multi-modal query forward on B200 (BASELINE.json metric).
+"""bench.py — images/sec of the MQ-GLIP-T multi-modal query forward on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl mqdet|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl mqdet|reference] [--dump-outputs DIR]
 
 A step = one forward of ``GeneralizedVLRCNN_New`` (Swin-T -> FPN -> QuerySelector/PreSelect/GCP-BERT -> 6x[BiAttention,
 BERT layer, DyConv] -> dot-product token head -> ATSS post-processing + ml_nms) over one batch of synthetic 800x1333
@@ -13,6 +13,9 @@ random-init weights of the real architecture (no checkpoints offline).
           memory, runs the forward and reads the fixed-shape detections back.
   N > 1 : one process per GPU (torchrun), images sharded over ranks (weak scaling, B per GPU fixed), ONE NCCL all-gather
           of the fixed-shape per-image detections per step.
+  --dump-outputs DIR : after the timed steps, the outputs of the last timed step (every floating / integer tensor the forward
+          returns, as float32 / float64 .npy; a fixed seeded sample of the larger ones, 64 MB in all) -> DIR/<name>.npy.  The
+          inputs are seeded, so two builds run with the same arguments can be compared output for output.
   --impl reference : the CPU oracle (oracle/restate.py — the reference's algorithm restated; its own modules cannot run
           the full forward on CPU, SURVEY.md §8c) on the host cores, one image per step (bounded sample), rank 0 only.
 """
@@ -38,7 +41,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured (MEASURED_PEAKS.json, sustained)"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "src": "H100 SXM data sheet (dense fp16, 700 W)"}
 
 
 def cpu_threads():
@@ -89,12 +92,8 @@ class ClockSampler:
 
 
 def traffic_note():
-    """(dram bytes per launch of the dominant kernel from the committed ncu --set full capture, its source) or (None, why)."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("dram_bytes_per_launch"), d.get("source")
-    return None, "no ncu --set full capture summarised in profiles/r02_traffic.json"
+    """(dram bytes per launch of the dominant kernel, its source) or (None, why): no DRAM-counter capture is committed."""
+    return None, "not measured (no DRAM-counter capture)"
 
 
 # Algorithmic work per IMAGE and stage (SURVEY.md §8d, 80-class prompt, fp16 storage): (GFLOP, activation MB per image that
@@ -450,6 +449,51 @@ def run_reference(args):
         "e2e": {"value": v, "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
 
 
+DUMP_BYTES = 64 << 20     # total size of --dump-outputs
+DUMP_SAMPLE = 1 << 20     # elements kept of a tensor larger than that (fixed seeded sample)
+
+
+def dump_outputs(raw, out_dir):
+    """Writes every tensor of the forward's output dict (nested keys joined by '.') as DIR/<name>.npy: floating tensors as
+    float32, integer / bool ones as float64.  Tensors above DUMP_SAMPLE elements keep a fixed sample (seeded generator over the
+    flattened index; the indices go to <name>.index.npy).  Stops before DUMP_BYTES would be exceeded."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    flat = []
+
+    def walk(prefix, v):
+        if isinstance(v, torch.Tensor):
+            flat.append((prefix, v))
+        elif isinstance(v, dict):
+            for k in sorted(v, key=str):
+                walk(f"{prefix}.{k}" if prefix else str(k), v[k])
+        elif isinstance(v, (list, tuple)):
+            for i, x in enumerate(v):
+                walk(f"{prefix}.{i}", x)
+    walk("", raw)
+    used, written = 0, []
+    for name, t in flat:
+        a = t.detach()
+        a = a.float() if a.is_floating_point() else a.double()
+        a = a.reshape(-1) if a.numel() > DUMP_SAMPLE else a
+        idx = None
+        if a.dim() == 1 and a.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            a = a[idx.to(a.device)]
+        arr = a.cpu().numpy()
+        size = arr.nbytes + (idx.numel() * 8 if idx is not None else 0)
+        if used + size > DUMP_BYTES:
+            continue
+        np.save(os.path.join(out_dir, f"{name}.npy"), arr)
+        if idx is not None:
+            np.save(os.path.join(out_dir, f"{name}.index.npy"), idx.numpy())
+        used += size
+        written.append(name)
+    return written
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -470,7 +514,11 @@ def main():
                     help="coco: BASELINE config 2 (the headline metric); lvis: BASELINE config 3 (MQ-GLIP-L, chunked 1203-class prompt); "
                          "gdino: BASELINE config 4 (MQ-GroundingDINO-T, 2 images / GPU, 13-class prompt)")
     ap.add_argument("--chunks-per-pass", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (coco config)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "mqdet" or args.config != "coco"):
+        ap.error("--dump-outputs applies to the default workload (--impl mqdet --config coco)")
     if args.impl == "reference":
         return run_reference(args)
     if args.config == "lvis":
@@ -511,7 +559,7 @@ def main():
     img_host = img.pin_memory()
     img_dev = img.to(dev)
     from mqdet_b200.engine.inference import InferenceEngine
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -550,10 +598,11 @@ def main():
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
     barrier()
     main_stream = torch.cuda.current_stream()
+    last = None
     for i in range(args.steps):
         flush.zero_()  # L2 flush between timed iterations (outside the per-step events)
         ev[i][0].record()
-        engine.device_step(k=i & 1)
+        last = engine.device_step(k=i & 1)
         ev[i][1].record()
     # the exchange ring (one all-gather per `gather_every` steps) runs on the engine's result stream behind the forward; a
     # step's bracket holds the wait for the result work issued two steps earlier, and this last bracket the flush of the ring
@@ -576,6 +625,9 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
     value = world * B / (ms / 1e3)
+    if args.dump_outputs and rank == 0 and last is not None:
+        # before anything else runs on the engine: the graph's output buffers are reused by the next replay
+        dump_outputs(last["raw"], args.dump_outputs)
 
     # ---- end to end through the public API with host buffers ----------------------------------------------------------
     # `for boxlists in engine.run(batches)`: every batch starts in pinned HOST memory and ends as list[BoxList] built from the
@@ -606,7 +658,7 @@ def main():
           "pre_nms_boxes_per_image_after_topk": float(o["cand_totals"].float().mean().item()),
           "detections_per_image": float(o["num"].float().mean().item())}
 
-    # ---- roofline of the dominant kernel family (the tcgen05 GEMM): every launch timed with CUDA events on its stream ----
+    # ---- roofline of the dominant kernel family (the tensor-core kernels): every launch timed with CUDA events on its stream ----
     def eager_step():
         return model.forward_device(ImageList(img_dev, sizes), caps, pmap)
 
@@ -669,11 +721,11 @@ def main():
                        "launch": graph_note + ("; tower text branch on a second stream" if model.rpn.head.overlap_text_stream else ""),
                        "l2": "256 MiB buffer written between timed steps", "postprocess": pp,
                        "tokenisation": "pre-tokenised ids (no bert-base-uncased vocabulary offline); prompt state cached per prompt"},
-            # the dominant kernel family = the tcgen05 kernels: every matrix product of the step (the set round 1 ran through
-            # the one GEMM kernel; since round 2 the attention products and the DCNv2 convolutions have kernels of their own)
+            # the dominant kernel family = the tensor-core (wgmma) kernels: every matrix product of the step (the GEMM, the
+            # attention products and the DCNv2 convolutions)
             "roofline": {"bound": "tensor", "achieved": tc_achieved, "peak": pk["tflops"], "unit": "TFLOP/s",
                          "frac": tc_achieved / pk["tflops"], "traffic": traffic_note()[0], "peak_source": pk["src"],
-                         "kernel": "tcgen05 kernels: gemm_tcp_kernel (all shapes), dcn_conv_kernel, biattn_image_kernel, "
+                         "kernel": "wgmma kernels: gemm_wg_kernel (all shapes), dcn_conv_kernel, biattn_image_kernel, "
                                    "biattn_text_kernel — every matrix product of one step", "launches": len(kprof),
                          "kernel_ms_per_step": tc_ms, "kernel_share_of_step": tc_ms / stages["eager_step_ms"] if stages else None,
                          "algorithmic_tflop_per_step": tc_flops / 1e12, "executed_tflop_per_step": tc_executed / 1e12,

@@ -1,4 +1,4 @@
-/* mqdet_b200 — C ABI of the B200-native MQ-Det hot path.
+/* mqdet_b200 — C ABI of the H100-native MQ-Det hot path.
  *
  * Every entry point takes DEVICE pointers + explicit sizes/strides + a cudaStream_t (passed as
  * void*), allocates nothing, never synchronises the device, and returns 0 on success or a
@@ -39,9 +39,9 @@ extern "C" {
 #define MQDET_VEC_PER_COL 2 /* length N */
 #define MQDET_VEC_PER_ROW 3 /* length M */
 
-#define MQDET_GEMM_IMPL_TCGEN05 0 /* TMA + tcgen05.mma + TMEM, persistent tile loop, double-buffered TMEM (product path) */
+#define MQDET_GEMM_IMPL_TC 0      /* TMA + wgmma, warp-specialised, one tile per CTA (product path) */
 #define MQDET_GEMM_IMPL_SIMT 1    /* plain shared-memory tiled fp32-FMA kernel (validation only) */
-#define MQDET_GEMM_IMPL_TCGEN05_ONESHOT 2 /* tcgen05, one tile per CTA (non-persistent variant, A/B measurements) */
+#define MQDET_GEMM_IMPL_TC_ONESHOT 2 /* the same tensor-core kernel (value kept so that callers selecting it stay valid) */
 
 const char* mqdet_last_error(void);
 int mqdet_version(void);
@@ -151,9 +151,9 @@ int mqdet_colstats_rowsoftmax(void* A, int64_t Z, int64_t N, int64_t T, const fl
                               float mask_value, float keep_add, float* workspace, void* stream);
 
 /* Text -> image side of BiMultiHeadAttention (maskrcnn_benchmark/utils/fuse_helper.py:257-275,289-291) fused into one
- * tcgen05 kernel per (image, head, 128 text tokens): out[z][t][:] = sum_n softmax_n(clamp(k_t . q_n))[n] * Vv[n][:], without
- * materialising the transposed probabilities: S^T = K Q^T (tcgen05, 64 image tokens per step) -> exp(fp16-rounded score
- * - column max) -> fp16 P tile in shared memory -> O += P Vv (tcgen05) -> O / column sum.  stat[z][2][T] as produced by
+ * wgmma kernel per (image, head, 64 text tokens): out[z][t][:] = sum_n softmax_n(clamp(k_t . q_n))[n] * Vv[n][:], without
+ * materialising the transposed probabilities: S^T = K Q^T (wgmma, 64 image tokens per step) -> exp(fp16-rounded score
+ * - column max) -> fp16 P (register operand) -> O += P Vv (wgmma) -> O / column sum.  stat[z][2][T] as produced by
  * mqdet_colsoftmax_stats from the SAME scores (q already carries the 1/sqrt(d) scale).  z = z2 * nb1 + z1.
  *   k [z][T][d], q [z][N][d], vvT [z][d][Np] f16 (Np >= N, zero padded), out [z][T][d] f16; *_ld = row stride, *_b1 / *_b2 =
  *   batch strides in elements (multiples of 8); d == 256, T <= 256. */
@@ -175,9 +175,9 @@ int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2
                          int64_t nb1, int64_t nb2, int64_t T, int64_t N, void* stream);
 
 /* Image -> text side of BiMultiHeadAttention fused with the query, value and output projections, layer scale and residual
- * (maskrcnn_benchmark/utils/fuse_helper.py:240-256,277-302,420-425) in ONE persistent tcgen05 kernel: per 128 image tokens and
- * head, S = vn gT_h^T + gbias_h stays in TMEM (fp32) -> clamp -> masked softmax over the T tokens in registers -> P (fp16,
- * shared memory) -> acc += P mT_h^T in a second TMEM accumulator summed over the heads -> out = res + gamma * (acc + bias).
+ * (maskrcnn_benchmark/utils/fuse_helper.py:240-256,277-302,420-425) in ONE wgmma kernel: per 64 image tokens and
+ * head, S = vn gT_h^T + gbias_h stays in registers (fp32) -> clamp -> masked softmax over the T tokens in registers -> P (fp16,
+ * registers) -> acc += P mT_h^T summed over the heads -> out = res + gamma * (acc + bias).
  * Neither q, the score matrix nor a per-head context reaches HBM.  mask [B][T] f32 (0 = padding token: probability exactly 0,
  * like the reference's -9e15; an all-masked image gets the uniform distribution the reference's fp32 sum produces) or NULL;
  * gamma / bias [256] f32 (16-byte aligned) and res may be NULL.

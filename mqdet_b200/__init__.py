@@ -1,4 +1,4 @@
-"""mqdet_b200 — B200-native (sm_100a) implementation of MQ-Det's multi-modal query forward pass.
+"""mqdet_b200 — H100-native (sm_90a) implementation of MQ-Det's multi-modal query forward pass.
 
 Host code is Python/PyTorch plumbing over hand-written CUDA kernels behind a C ABI (include/mqdet_b200.h,
 mqdet_b200/csrc).  The module tree mirrors the slice of ``maskrcnn_benchmark.modeling`` on the hot path

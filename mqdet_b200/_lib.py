@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libmqdet_b200.so")
 F16, F32 = 0, 1
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
 VEC_NONE, VEC_SCALAR, VEC_PER_COL, VEC_PER_ROW = 0, 1, 2, 3
-IMPL_TCGEN05, IMPL_SIMT, IMPL_TCGEN05_ONESHOT = 0, 1, 2
+IMPL_TC, IMPL_SIMT, IMPL_TC_ONESHOT = 0, 1, 2
 
 
 class GemmArgs(ctypes.Structure):

@@ -1,48 +1,62 @@
 // mqdet_b200 — the bi-directional image <-> text attention of the VL fusion tower (BiMultiHeadAttention,
-// maskrcnn_benchmark/utils/fuse_helper.py:218-303) as two tcgen05 kernels that never materialise the score matrix:
+// maskrcnn_benchmark/utils/fuse_helper.py:218-303) as two wgmma kernels that never materialise the score matrix:
 //
-//   biattn_image_kernel : image -> text side.  Per 128 image tokens and head: S = Q K^T (fp32 in TMEM) -> +-5e4 clamp ->
-//                         column-max partials (for the text side) -> masked row softmax over the T tokens in registers ->
-//                         P (fp16, shared memory) -> O = P V_l -> fp16 -> out-projection accumulated over the heads in a second
-//                         TMEM accumulator -> v' = residual + gamma * (acc + bias) -> TMA store.  Neither the scores A nor the
-//                         per-head context reach HBM; the softmax statistics are taken from the fp32 accumulator.
-//   biattn_text_kernel  : text -> image side (one CTA per (image, head, 128 text tokens), streams all image tokens):
-//                         S^T recomputed on the tensor cores, exp(S^T - column max), P . V accumulated in TMEM.
+//   biattn_image_kernel : image -> text side.  Per 64 image tokens and head: S = Q K^T (fp32, registers) -> +-5e4 clamp ->
+//                         column-max partials (for the text side) -> masked row softmax over the T tokens in the accumulator
+//                         fragments -> P (fp16, registers: the A operand of the next wgmma) -> P . mT_h, summed over the heads
+//                         -> v' = residual + gamma * (acc + bias).  Neither the scores nor the per-head context reach HBM.
+//   biattn_text_kernel  : text -> image side (one CTA per (image, head, 64 text tokens), streams all image tokens):
+//                         S^T recomputed on the tensor cores, exp(S^T - column max), P . V accumulated in registers.
 //                         VN variant: V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile),
 //                         the value projection is applied AFTER the token reduction (sum_n p[n] = 1), and the column sums are
 //                         accumulated in-kernel, so the [B, E, N] value tensor of the image side is never built.
+// Each CTA is one warpgroup; a 64-row tile keeps a 64 x 256 fp32 accumulator in its registers (128 per thread).  Operands arrive
+// by TMA (128B swizzle) through a two-stage ring; accumulator fragment: row / column of element i of thread t = wg_row / wg_col.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/mqdet_b200.h"
 
 namespace mqdet {
 
-constexpr int BM = 128;
+constexpr int BM = 64;  // rows (text tokens / image tokens) per CTA
 constexpr int BK = 64;  // 64 fp16 = 128 B = one swizzle row
+constexpr int KB_BYTES = 64 * BK * 2;  // one [64 x 64] k-block
+
+// A-operand fragment of k-step kk (16 columns) from a 64 x N accumulator fragment: the register layouts coincide
+template <int R>
+__device__ __forceinline__ void acc_to_a(const float (&e)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_half2(e[8 * kk + 0], e[8 * kk + 1]);
+  a[1] = pack_half2(e[8 * kk + 2], e[8 * kk + 3]);
+  a[2] = pack_half2(e[8 * kk + 4], e[8 * kk + 5]);
+  a[3] = pack_half2(e[8 * kk + 6], e[8 * kk + 7]);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 // =====================================================================================================================
 // Fused text -> image side of the bi-directional attention (BiMultiHeadAttention, fuse_helper.py:257-275, 289-291):
 //     out[t, :] = sum_n softmax_n(clamp(k_t . q_n)) * Vv[n, :]        per (image, head), t = text token, n = image token
-// One CTA per (z, 128 text tokens).  The transposed probabilities [T, N] never reach HBM.  Per step of 256 image tokens:
-//     S^T   = K_tile (128 x 256, resident) . Q_step^T      16 tcgen05 MMAs 128x256x16, Q streamed as four [256 x 64] k-blocks
-//     P_j   = exp(fp16(clamp(S^T[:, 64j..])) - colmax_t)   -> fp16, 128B-swizzled A-operand tile in shared memory (j = 0..3)
-//     O    += P_j . Vv_j                                    4 MMAs 128x256x16 per 64-token sub-block, O (128 x 256) in TMEM
-//     out   = O / colsum_t  -> fp16 -> TMA store
-// Every MMA is 256 wide: narrower ones (the first version used 64-token steps) pay ~the same ~130-160 cycles per
-// instruction for a fraction of the work.  colmax / colsum come from mqdet_colsoftmax_stats / mqdet_colstats_rowsoftmax over
-// the SAME fp16 scores the image -> text side uses, so no online rescaling is needed.
-// Roles: warp 0 = Q producer, warp 3 = V producer (separate rings: a Q k-block is free as soon as its MMAs retire),
-// warp 1 = MMA issuer, warp 2 = TMEM allocator, warps 4-19 = exponentials + epilogue (thread == text token == TMEM lane,
-// four warps per lane quarter, 16 of the 64 sub-block columns each).  TMEM: S^T 256 columns + O 256 columns.
+// One CTA per (z, 64 text tokens).  The transposed probabilities [T, N] never reach HBM.  Per step of 64 image tokens:
+//     S^T   = K_tile (64 x 256, resident) . Q_step^T           16 wgmma 64x64x16
+//     P     = exp(fp16(clamp(S^T)) - colmax_t)                  in the accumulator fragments -> fp16 A operand (registers)
+//     O    += P . Vv_step                                        4 wgmma 64x256x16, O (64 x 256) in registers
+//     out   = O / colsum_t  -> fp16
+// colmax / colsum come from mqdet_colsoftmax_stats / mqdet_colstats_rowsoftmax over the SAME fp16 scores the image -> text
+// side uses, so no online rescaling is needed.
 // =====================================================================================================================
-constexpr int BT_STEP = 256;  // image tokens per S^T accumulator
-constexpr int BT_SUB = 64;    // image tokens per P / V tile
-constexpr int BT_PF = 2;      // L2 prefetch distance in steps
+constexpr int BT_STEP = 64;  // image tokens per step
 struct BtCfg {
-  static constexpr int KT_BYTES = 4 * BM * BK * 2;    // resident K tile: 4 k-blocks of [128 x 64]
-  static constexpr int Q_BYTES = BT_STEP * BK * 2;    // one k-block [256 n x 64 d]
-  static constexpr int V_BYTES = 256 * BT_SUB * 2;    // Vv^T tile [256 d x 64 n]  /  VN: image-token tile [64 n x 256 c]
-  static constexpr int P_BYTES = BM * BT_SUB * 2;     // P tile [128 t x 64 n]
-  static constexpr int SMEM_BYTES = KT_BYTES + 2 * Q_BYTES + 2 * V_BYTES + 2 * P_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int KT_BYTES = 4 * KB_BYTES;       // resident K tile: 4 k-blocks of [64 x 64]
+  static constexpr int Q_BYTES = 4 * KB_BYTES;        // Q step [64 n x 256 d]
+  static constexpr int V_BYTES = 256 * BT_STEP * 2;   // Vv^T tile [256 d x 64 n]  /  VN: image-token tile [64 n x 256 c]
+  static constexpr int STAGE_BYTES = Q_BYTES + V_BYTES;
+  static constexpr int SMEM_BYTES = KT_BYTES + 2 * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 static_assert(BtCfg::SMEM_BYTES <= 232448, "biattn_text: dynamic shared memory above the 227 KB per-CTA limit");
 struct BtP {
@@ -50,247 +64,143 @@ struct BtP {
   float clamp;
   int nb1, T, N, n_steps;
   int k_bc1, k_bc2, q_bc1, q_bc2, v_bc1, v_bc2;  // 1 -> batch coordinate pinned to 0
-  uint32_t vn_lbo, vn_sbo;                        // VN: MN-major descriptor strides of the image-token tile
   const float* rowbias;                           // VN: optional [Z][T * rb_ld] additive score bias per text token (folded q bias)
   int rb_ld;
+  __half* out;                                    // [nb2][nb1][T][256]
+  long o_ld, o_b1, o_b2;
 };
 
 template <bool VN>
-__global__ void __launch_bounds__(640, 1) biattn_text_kernel(const __grid_constant__ CUtensorMap tma_k,
+__global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_constant__ CUtensorMap tma_k,
                                                              const __grid_constant__ CUtensorMap tma_q,
-                                                             const __grid_constant__ CUtensorMap tma_v,
-                                                             const __grid_constant__ CUtensorMap tma_o, const BtP p) {
+                                                             const __grid_constant__ CUtensorMap tma_v, const BtP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* kt = smem;
-  uint8_t* qring = kt + BtCfg::KT_BYTES;           // 2 x 32 KB
-  uint8_t* vring = qring + 2 * BtCfg::Q_BYTES;     // 2 x 32 KB
-  uint8_t* pring = vring + 2 * BtCfg::V_BYTES;     // 2 x 16 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(pring + 2 * BtCfg::P_BYTES);
+  uint8_t* ring = kt + BtCfg::KT_BYTES;  // 2 x [Q step | V step]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + 2 * BtCfg::STAGE_BYTES);
   uint64_t* kt_full = bars;
-  uint64_t* q_full = bars + 1;    // [2] Q k-block landed
-  uint64_t* q_empty = bars + 3;   // [2] its four MMAs retired
-  uint64_t* v_full = bars + 5;    // [2] Vv sub-block landed
-  uint64_t* pv_done = bars + 7;   // [2] P_j . Vv_j retired: V slot and P slot may be overwritten
-  uint64_t* p_full = bars + 9;    // [2] P tile written by the 16 exp warps
-  uint64_t* s_full = bars + 11;   // S^T accumulator complete
-  uint64_t* s_empty = bars + 12;  // S^T accumulator copied to registers by the 16 exp warps
-  uint64_t* o_full = bars + 13;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 14);
-  // VN: [4 parts][128 rows] partial column sums, exchanged after the last S^T product has retired -> the K tile is free
-  float* lsum_sm = reinterpret_cast<float*>(kt);
+  uint64_t* full = bars + 1;  // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x;
   const int mt = blockIdx.x, z = blockIdx.y;
   const int z1 = z % p.nb1, z2 = z / p.nb1;
   const int NS = p.n_steps;
+  const int qz1 = p.q_bc1 ? 0 : z1, qz2 = p.q_bc2 ? 0 : z2, vz1 = p.v_bc1 ? 0 : z1, vz2 = p.v_bc2 ? 0 : z2;
 
-  if (threadIdx.x == 0) {
+  auto issue = [&](int i) {  // Q and V of step i into stage i & 1
+    uint8_t* st = ring + (i & 1) * BtCfg::STAGE_BYTES;
+    uint64_t* bar = &full[i & 1];
+    mbar_expect_tx(bar, BtCfg::STAGE_BYTES);
+    for (int kb = 0; kb < 4; ++kb) tma_load_4d(st + kb * KB_BYTES, &tma_q, bar, kb * BK, i * BT_STEP, qz1, qz2);
+    if (VN)  // image tokens themselves, [64 n x 256 c] as four [64 n x 64 c] blocks: the B operand of P.vn is read MN-major
+      for (int cb = 0; cb < 4; ++cb) tma_load_4d(st + BtCfg::Q_BYTES + cb * KB_BYTES, &tma_v, bar, cb * BK, i * BT_STEP, vz1, vz2);
+    else
+      tma_load_4d(st + BtCfg::Q_BYTES, &tma_v, bar, i * BT_STEP, 0, vz1, vz2);
+  };
+  if (tid == 0) {
     tma_prefetch_desc(&tma_k);
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_v);
-    tma_prefetch_desc(&tma_o);
     mbar_init(kt_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&q_full[s], 1);
-      mbar_init(&q_empty[s], 1);
-      mbar_init(&v_full[s], 1);
-      mbar_init(&pv_done[s], 1);
-      mbar_init(&p_full[s], 16);  // one arrival per exp warp
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 16);
-    mbar_init(o_full, 1);
+    mbar_init(&full[0], 1);
+    mbar_init(&full[1], 1);
     fence_mbar_init();
+    mbar_expect_tx(kt_full, BtCfg::KT_BYTES);
+    for (int kb = 0; kb < 4; ++kb)
+      tma_load_4d(kt + kb * KB_BYTES, &tma_k, kt_full, kb * BK, mt * BM, p.k_bc1 ? 0 : z1, p.k_bc2 ? 0 : z2);
+    issue(0);
+    if (NS > 1) issue(1);
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = *tmem_base_slot;
-  const uint32_t tmem_o = tmem_s + 256;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(kt_full, BtCfg::KT_BYTES);
-      for (int kb = 0; kb < 4; ++kb)
-        tma_load_4d(kt + kb * (BM * BK * 2), &tma_k, kt_full, kb * BK, mt * BM, p.k_bc1 ? 0 : z1, p.k_bc2 ? 0 : z2);
-      const int qz1 = p.q_bc1 ? 0 : z1, qz2 = p.q_bc2 ? 0 : z2;
-      for (int qc = 0; qc < 4 * NS; ++qc) {
-        const int i = qc >> 2, kb = qc & 3, s = qc & 1;
-        if (i + BT_PF < NS) tma_prefetch_l2_4d(&tma_q, kb * BK, (i + BT_PF) * BT_STEP, qz1, qz2);
-        if (qc >= 2) mbar_wait(&q_empty[s], ((qc >> 1) - 1) & 1);
-        mbar_expect_tx(&q_full[s], BtCfg::Q_BYTES);
-        tma_load_4d(qring + s * BtCfg::Q_BYTES, &tma_q, &q_full[s], kb * BK, i * BT_STEP, qz1, qz2);
-      }
-    }
-  } else if (warp == 3) {
-    if (lane == 0) {
-      const int vz1 = p.v_bc1 ? 0 : z1, vz2 = p.v_bc2 ? 0 : z2;
-      for (int sc = 0; sc < 4 * NS; ++sc) {
-        const int s = sc & 1;
-        if (VN) {
-          // image tokens themselves, [64 n x 256 c] as four [64 n x 64 c] blocks: the B operand of P.vn is read MN-major
-          if (sc + 4 * BT_PF < 4 * NS)
-            for (int cb = 0; cb < 4; ++cb) tma_prefetch_l2_4d(&tma_v, cb * BK, (sc + 4 * BT_PF) * BT_SUB, vz1, vz2);
-          if (sc >= 2) mbar_wait(&pv_done[s], ((sc >> 1) - 1) & 1);
-          mbar_expect_tx(&v_full[s], BtCfg::V_BYTES);
-          for (int cb = 0; cb < 4; ++cb)
-            tma_load_4d(vring + s * BtCfg::V_BYTES + cb * (BT_SUB * 128), &tma_v, &v_full[s], cb * BK, sc * BT_SUB, vz1, vz2);
-          continue;
-        }
-        if (sc + 4 * BT_PF < 4 * NS) tma_prefetch_l2_4d(&tma_v, (sc + 4 * BT_PF) * BT_SUB, 0, vz1, vz2);
-        if (sc >= 2) mbar_wait(&pv_done[s], ((sc >> 1) - 1) & 1);
-        mbar_expect_tx(&v_full[s], BtCfg::V_BYTES);
-        tma_load_4d(vring + s * BtCfg::V_BYTES, &tma_v, &v_full[s], sc * BT_SUB, 0, vz1, vz2);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, 256, 0);
-      mbar_wait(kt_full, 0);
-      tc_fence_after();
-      const uint32_t kt_addr = smem_u32(kt);
-      auto issue_s = [&](int i) {  // S^T of step i: 4 k-blocks x 4 MMAs
-        for (int kb = 0; kb < 4; ++kb) {
-          const int qc = 4 * i + kb, s = qc & 1;
-          mbar_wait(&q_full[s], (qc >> 1) & 1);
-          tc_fence_after();
-          const uint32_t b0 = smem_u32(qring + s * BtCfg::Q_BYTES);
+  // the two text tokens (rows) of this thread
+  constexpr float L2E = 1.4426950408889634f;
+  float m_l2[2] = {0.f, 0.f}, inv[2] = {0.f, 0.f}, gb[2] = {0.f, 0.f}, lsum[2] = {0.f, 0.f};
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_f16(tmem_s, umma_desc_k_sw128(kt_addr + kb * (BM * BK * 2) + k * 32), umma_desc_k_sw128(b0 + k * 32), idesc,
-                       (kb | k) != 0 ? 1u : 0u);
-          tc_commit(&q_empty[s]);
-        }
-        tc_commit(s_full);
-      };
-      issue_s(0);
-      for (int i = 0; i < NS; ++i) {
-        // S^T of the NEXT step goes first: the exp warps hold step i's scores in registers (s_empty), so the tensor pipe
-        // computes S^T(i+1) while they turn S^T(i) into the four P tiles, and P(i).Vv follows back to back
-        if (i + 1 < NS) {
-          mbar_wait(s_empty, i & 1);
-          tc_fence_after();
-          issue_s(i + 1);
-        }
-        for (int j = 0; j < 4; ++j) {
-          const int sc = 4 * i + j, s = sc & 1;
-          mbar_wait(&v_full[s], (sc >> 1) & 1);
-          mbar_wait(&p_full[s], (sc >> 1) & 1);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(pring + s * BtCfg::P_BYTES), b0 = smem_u32(vring + s * BtCfg::V_BYTES);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            // VN: B = vn tile read MN-major (N = channel contiguous): 16 image tokens per MMA = 2 KB further down the block,
-            // next 8 tokens (SBO) 1 KB apart, next 64 channels (LBO) one [64 n x 64 c] block = 8 KB apart
-            const uint64_t db = VN ? umma_desc_mn_sw128(b0 + k * 2048, p.vn_lbo, p.vn_sbo) : umma_desc_k_sw128(b0 + k * 32);
-            tc_mma_f16(tmem_o, umma_desc_k_sw128(a0 + k * 32), db, VN ? (idesc | UMMA_B_MN_MAJOR) : idesc, (sc | k) != 0 ? 1u : 0u);
-          }
-          tc_commit(&pv_done[s]);
-        }
-      }
-      tc_commit(o_full);
-    }
-  } else if (warp >= 4) {
-    const int ew = (warp - 4) & 3, part = (warp - 4) >> 2;
-    const int row = ew * 32 + lane;
-    const int t = mt * BM + row;
-    constexpr float L2E = 1.4426950408889634f;
-    float m_l2 = 0.f, inv = 0.f, lsum = 0.f, gb = 0.f;
+  for (int h = 0; h < 2; ++h) {
+    const int t = mt * BM + wg_row(tid, 2 * h);
     if (t < p.T) {
       if (VN) {
-        m_l2 = -p.stat[(long)z * p.T + t] * L2E;
-        if (p.rowbias) gb = p.rowbias[((long)z * p.T + t) * p.rb_ld];
+        m_l2[h] = -p.stat[(long)z * p.T + t] * L2E;
+        if (p.rowbias) gb[h] = p.rowbias[((long)z * p.T + t) * p.rb_ld];
       } else {
-        m_l2 = -p.stat[((long)z * 2) * p.T + t] * L2E;
-        inv = p.stat[((long)z * 2 + 1) * p.T + t];
+        m_l2[h] = -p.stat[((long)z * 2) * p.T + t] * L2E;
+        inv[h] = p.stat[((long)z * 2 + 1) * p.T + t];
       }
-    }
-    const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
-    const int sw = row & 7;
-    const uint32_t lane_addr = (uint32_t)(ew * 32) << 16;
-    const int j0 = part * 2;  // 16-byte chunks of this thread's 16 columns inside the 128-byte P row
-    for (int i = 0; i < NS; ++i) {
-      mbar_wait(s_full, i & 1);
-      tc_fence_after();
-      // this thread's 16 columns of each of the four 64-token sub-blocks
-      uint32_t r[4][16];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) tmem_ld_32x16(tmem_s + lane_addr + (uint32_t)(j * BT_SUB + part * 16), r[j]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty);  // the accumulator may be overwritten by the next step's S^T
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int sc = 4 * i + j, s = sc & 1;
-        if (sc >= 2) mbar_wait(&pv_done[s], ((sc >> 1) - 1) & 1);  // the product that read this P slot has retired
-        const int nrem = p.N - sc * BT_SUB - part * 16;  // valid columns of this thread's 16 (< 16 only at the very end)
-        uint32_t h[8];
-#pragma unroll
-        for (int q2 = 0; q2 < 8; ++q2) {
-          const float a = fminf(fmaxf(__uint_as_float(r[j][2 * q2]) + gb, -clampv), clampv);
-          const float b = fminf(fmaxf(__uint_as_float(r[j][2 * q2 + 1]) + gb, -clampv), clampv);
-          // !VN: the score as the fp16 matrix A holds it (the statistics were taken from those values);
-          //  VN: the fp32 score itself (the column maxima come from the fp32 scores of the image-side kernel)
-          const float2 f = VN ? make_float2(a, b) : __half22float2(__floats2half2_rn(a, b));
-          float e0 = ex2_approx(fmaf(f.x, L2E, m_l2)), e1 = ex2_approx(fmaf(f.y, L2E, m_l2));
-          if (nrem < 16) {  // image tokens beyond N (zero-filled q rows) must not contribute exp(-max)
-            if (2 * q2 >= nrem) e0 = 0.f;
-            if (2 * q2 + 1 >= nrem) e1 = 0.f;
-          }
-          if (VN) lsum += e0 + e1;  // the column sum of the softmax is accumulated here, no separate pass over the scores
-          h[q2] = pack_half2(e0, e1);
-        }
-        const uint32_t prow = smem_u32(pring + s * BtCfg::P_BYTES) + row * 128;
-        sts128(prow + (((j0) ^ sw) << 4), h[0], h[1], h[2], h[3]);
-        sts128(prow + (((j0 + 1) ^ sw) << 4), h[4], h[5], h[6], h[7]);
-        fence_proxy_async();  // generic-proxy writes of P -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[s]);
-      }
-    }
-    // ---- epilogue: O / colsum -> fp16 -> swizzled staging (the Q and V rings are idle by now) -> TMA store ----
-    if (VN) {  // total column sum = the four column-quarter partials of this text token
-      lsum_sm[part * BM + row] = lsum;
-      asm volatile("bar.sync 1, 512;" ::: "memory");
-      const float tot = lsum_sm[row] + lsum_sm[BM + row] + lsum_sm[2 * BM + row] + lsum_sm[3 * BM + row];
-      inv = tot > 0.f ? 1.f / tot : 0.f;
-    }
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const uint32_t blk = smem_u32(qring) + part * (BM * 128) + row * 128;  // this warp's 64-column block (4 x 16 KB)
-    uint32_t ra[16], rb[16];
-    tmem_ld_32x16(tmem_o + lane_addr + (uint32_t)(part * 64), ra);
-#pragma unroll
-    for (int c0 = 0; c0 < 64; c0 += 32) {
-      tmem_ld_wait_dep(ra);
-      tmem_ld_32x16(tmem_o + lane_addr + (uint32_t)(part * 64 + c0 + 16), rb);
-      uint32_t h[8];
-#pragma unroll
-      for (int q2 = 0; q2 < 8; ++q2) h[q2] = pack_half2(__uint_as_float(ra[2 * q2]) * inv, __uint_as_float(ra[2 * q2 + 1]) * inv);
-      sts128(blk + ((((c0 >> 3)) ^ sw) << 4), h[0], h[1], h[2], h[3]);
-      sts128(blk + ((((c0 >> 3) + 1) ^ sw) << 4), h[4], h[5], h[6], h[7]);
-      tmem_ld_wait_dep(rb);
-      if (c0 + 32 < 64) tmem_ld_32x16(tmem_o + lane_addr + (uint32_t)(part * 64 + c0 + 32), ra);
-#pragma unroll
-      for (int q2 = 0; q2 < 8; ++q2) h[q2] = pack_half2(__uint_as_float(rb[2 * q2]) * inv, __uint_as_float(rb[2 * q2 + 1]) * inv);
-      sts128(blk + ((((c0 >> 3) + 2) ^ sw) << 4), h[0], h[1], h[2], h[3]);
-      sts128(blk + ((((c0 >> 3) + 3) ^ sw) << 4), h[4], h[5], h[6], h[7]);
-    }
-    tc_fence_before();
-    fence_proxy_async();
-    asm volatile("bar.sync 1, 512;" ::: "memory");
-    if (warp == 4 && lane == 0) {
-      for (int cb = 0; cb < 4; ++cb) tma_store_4d(&tma_o, qring + cb * (BM * 128), cb * 64, mt * BM, z1, z2);
-      tma_store_commit_and_wait_read();
     }
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_s, 512);
+  const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
+  const uint32_t kt_addr = smem_u32(kt);
+  float o[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) o[i] = 0.f;
+  mbar_wait(kt_full, 0);
+  for (int i = 0; i < NS; ++i) {
+    const int s = i & 1;
+    mbar_wait(&full[s], (i >> 1) & 1);
+    const uint32_t q0 = smem_u32(ring + s * BtCfg::STAGE_BYTES), v0 = q0 + BtCfg::Q_BYTES;
+    float sc[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) sc[j] = 0.f;
+    wgmma_fence_acc(sc);
+    wgmma_fence();
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss_m64n64_kk(sc, wg_desc_k_sw128(kt_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(q0 + kb * KB_BYTES + k * 32), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(sc);
+    const int nrem = p.N - i * BT_STEP;  // valid image tokens of this step
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int h = (j >> 1) & 1;
+      const float a = fminf(fmaxf(sc[j] + gb[h], -clampv), clampv);
+      // !VN: the score as the fp16 matrix A holds it (the statistics were taken from those values);
+      //  VN: the fp32 score itself (the column maxima come from the fp32 scores of the image-side kernel)
+      const float f = VN ? a : __half2float(__float2half_rn(a));
+      float e = ex2_approx(fmaf(f, L2E, m_l2[h]));
+      if (wg_col(tid, j) >= nrem) e = 0.f;  // image tokens beyond N (zero-filled q rows) must not contribute exp(-max)
+      if (VN) lsum[h] += e;
+      sc[j] = e;
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) acc_to_a(sc, kk, pa[kk]);
+    wgmma_fence_acc(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      // VN: B = vn tile read MN-major (N = channel contiguous): 16 image tokens per MMA = 2 KB further down the block,
+      // next 8 tokens (SBO) 1 KB apart, next 64 channels (LBO) one [64 n x 64 c] block = 8 KB apart
+      if (VN)
+        wgmma_rs_m64n256_kmn(o, pa[kk], wg_desc_mn_sw128(v0 + kk * 2048, KB_BYTES, 1024), 1);
+      else
+        wgmma_rs_m64n256_kk(o, pa[kk], wg_desc_k_sw128(v0 + kk * 32), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
+    __syncthreads();  // every wgmma of the warpgroup has read stage s
+    if (tid == 0 && i + 2 < NS) issue(i + 2);
+  }
+  if (VN) {  // total column sum of this text token: the four threads of a quad hold its columns
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float tot = quad_sum(lsum[h]);
+      inv[h] = tot > 0.f ? 1.f / tot : 0.f;
+    }
+  }
+  // ---- epilogue: O / colsum -> fp16 ----
+  __half* out = p.out + z1 * p.o_b1 + z2 * p.o_b2;
+#pragma unroll
+  for (int j = 0; j < 128; j += 2) {
+    const int h = (j >> 1) & 1;
+    const int t = mt * BM + wg_row(tid, j);
+    if (t < p.T)
+      *reinterpret_cast<__half2*>(out + (long)t * p.o_ld + wg_col(tid, j)) = __floats2half2_rn(o[j] * inv[h], o[j + 1] * inv[h]);
   }
 }
 
@@ -304,31 +214,21 @@ __global__ void __launch_bounds__(640, 1) biattn_text_kernel(const __grid_consta
 //                              (image, head) by a tiny GEMM — (P V_l,h) W_h^T == P (V_l,h W_h^T), so the per-head context O never
 //                              exists and a head costs two tensor-core products instead of three
 //   out[B][N][256] fp16
-// Persistent: one CTA per SM walks (image, 128-token tile) items; per item the eight heads run back to back:
-//   S (128 x 256 t)   = vn . gT_h^T (+ gbias_h)   16 MMAs 128x256x16, the operands streamed as [.. x 64] k-blocks through a 3-stage ring
-//   P                 = softmax_t(clamp(S) + mask): thread == image token == TMEM lane, 4 warps per lane quarter, 64 tokens each;
-//                       pass 1 over the TMEM columns = column maxima (for the text side) + partial row maxima, pass 2 = exp into
-//                       registers + partial row sums; both statistics are exchanged through shared memory; P = e / rowsum -> fp16
-//                       -> shared memory (A operand)
-//   D (128 x 256 o)  += P . mT_h^T           second TMEM accumulator, summed over the heads
-//   out               = res + gamma * (D + bias)
-// The scratch columns are free as soon as pass 2 has read them, so the issuer runs S of head h+1 while the warps normalise and
-// store P of head h, and D of head h while they exponentiate S of head h+1.
-// TMEM: columns 0..255 S, 256..511 D.  Shared memory: one 64 KB tile PX (P, finally the output staging), 3 x 48 KB ring stages
-// ([128 x 64] A slot + [256 x 64] B slot), exchange arrays.
-// Column maxima of the clamped scores over the tile's valid rows go to colmax_part[b][h][tile][t] (reduced by
-// colmax_reduce_kernel); the text side needs them as the softmax shift.
-// Roles: warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator, warps 4-19 = softmax / epilogue.
+// One CTA per (image, 64-token tile); per tile the heads run back to back:
+//   S (64 x 256 t)   = vn . gT_h^T (+ gbias_h)   16 wgmma 64x256x16, gT_h streamed as [256 x 64] k-blocks
+//   P                = softmax_t(clamp(S) + mask) in the fragments (a row lives in one quad of threads); the column maxima of
+//                      the clamped scores over the tile's valid rows go to colmax_part[b][h][tile][t] (reduced by
+//                      colmax_reduce_kernel) — the text side needs them as the softmax shift
+//   D (64 x 256 o)  += P . mT_h^T                 P from registers; the head sum is kept in thread-private shared memory
+//   out              = res + gamma * (D + bias)
 // =====================================================================================================================
-constexpr int BI_STAGES = 3;
 struct BiCfg {
-  static constexpr int PX_BYTES = 4 * BM * BK * 2;           // 64 KB: four k-blocks [128 x 64]
-  static constexpr int A_BYTES = BM * BK * 2;                // 16 KB
-  static constexpr int B_BYTES = 256 * BK * 2;               // 32 KB
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;      // 48 KB
+  static constexpr int VN_BYTES = 4 * KB_BYTES;     // image-token tile [64 x 256 c]
+  static constexpr int STAGE_BYTES = 256 * BK * 2;  // one [256 x 64] k-block of gT_h or mT_h
   static constexpr int MAX_HEADS = 8;
-  static constexpr int EXTRA_BYTES = (4 * BM * 2 + 4 * 256 + MAX_HEADS * 256) * 4;  // rx | rsum, cmx, gk
-  static constexpr int SMEM_BYTES = PX_BYTES + BI_STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + EXTRA_BYTES;
+  static constexpr int D_BYTES = 128 * 128 * 4;     // head sum: [128 fragment elements][128 threads] fp32
+  static constexpr int EXTRA_BYTES = (4 * 256 + MAX_HEADS * 256) * 4;  // cmx, gk
+  static constexpr int SMEM_BYTES = VN_BYTES + 2 * STAGE_BYTES + D_BYTES + EXTRA_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 static_assert(BiCfg::SMEM_BYTES <= 232448, "biattn_image: dynamic shared memory above the 227 KB per-CTA limit");
 struct BiP {
@@ -337,353 +237,177 @@ struct BiP {
   const float* gamma;  // [256] layer scale, or nullptr (1)
   const __half* res;   // residual [B][N][256] (row stride res_ld, batch stride res_b) or nullptr
   long res_ld, res_b;
+  __half* out;         // [B][N][256] (row stride o_ld, batch stride o_b)
+  long o_ld, o_b;
   float* colmax_part;  // [B][H][tiles_per_img][T]
   const float* gbias;  // [B*H][T * gb_ld] additive score bias per (head, token): the folded query-projection bias, or nullptr
   int gb_ld;
   float clamp;
-  int B, H, T, N, tiles_per_img, total_tiles;
+  int B, H, T, N, tiles_per_img;
 };
 
-__device__ __forceinline__ float lds32f(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
-  return v;
-}
-
-__global__ void __launch_bounds__(640, 1) biattn_image_kernel(const __grid_constant__ CUtensorMap tma_q,
+__global__ void __launch_bounds__(128, 1) biattn_image_kernel(const __grid_constant__ CUtensorMap tma_q,
                                                               const __grid_constant__ CUtensorMap tma_k,
-                                                              const __grid_constant__ CUtensorMap tma_m,
-                                                              const __grid_constant__ CUtensorMap tma_o, const BiP p) {
+                                                              const __grid_constant__ CUtensorMap tma_m, const BiP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* px = smem;
-  uint8_t* ring = px + BiCfg::PX_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + BI_STAGES * BiCfg::STAGE_BYTES);
-  uint64_t* full_bar = bars;                     // [3] ring stage landed
-  uint64_t* empty_bar = bars + BI_STAGES;        // [3] its MMAs retired
-  uint64_t* s_full = bars + 6;                   // S complete
-  uint64_t* scratch_free = bars + 7;             // S has been read (16 warps): the scratch columns may take the next head's S
-  uint64_t* p_ready = bars + 8;                  // P written (16 warps)
-  uint64_t* op_done = bars + 9;                  // the head's P . mT MMAs retired: PX may be rewritten; last head: D complete
-  uint64_t* dv_free = bars + 10;                 // D has been read (16 warps)
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 13);
-  float* rx = reinterpret_cast<float*>(bars + 32);  // [4 parts][128 rows] partial row maxima
-  float* rsum = rx + 4 * BM;                         // [4 parts][128 rows] partial row sums
-  float* cmx = rsum + 4 * BM;                        // [4 lane quarters][256 tokens] column maxima
-  float* gk = cmx + 4 * 256;                         // [H][256] additive row-softmax term per (head, token): folded query bias
-                                                     // + token mask (0 keep / -inf masked)
+  uint8_t* vnt = smem;
+  uint8_t* ring = vnt + BiCfg::VN_BYTES;
+  float* dsum = reinterpret_cast<float*>(ring + 2 * BiCfg::STAGE_BYTES);
+  float* cmx = dsum + 128 * 128;  // [4 warps][256 tokens] column maxima
+  float* gk = cmx + 4 * 256;      // [H][256] additive row-softmax term per (head, token): folded query bias + mask (0 / -inf)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(gk + BiCfg::MAX_HEADS * 256);
+  uint64_t* vn_full = bars;
+  uint64_t* full = bars + 1;  // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.H;
-
-  if (threadIdx.x == 0) {
+  const int b = blockIdx.x / p.tiles_per_img, ti = blockIdx.x - b * p.tiles_per_img, m0 = ti * BM;
+  const int nq = 8 * H;  // ring sequence: per head 4 k-blocks of gT_h, then 4 of mT_h
+  auto issue = [&](int q) {
+    const int h = q >> 3, kb = q & 3;
+    uint64_t* bar = &full[q & 1];
+    mbar_expect_tx(bar, BiCfg::STAGE_BYTES);
+    tma_load_4d(ring + (q & 1) * BiCfg::STAGE_BYTES, (q & 4) ? &tma_m : &tma_k, bar, kb * BK, 0, h, b);
+  };
+  if (tid == 0) {
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_k);
     tma_prefetch_desc(&tma_m);
-    tma_prefetch_desc(&tma_o);
-    for (int s = 0; s < BI_STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(scratch_free, 16);
-    mbar_init(p_ready, 16);
-    mbar_init(op_done, 1);
-    mbar_init(dv_free, 16);
+    mbar_init(vn_full, 1);
+    mbar_init(&full[0], 1);
+    mbar_init(&full[1], 1);
     fence_mbar_init();
+    mbar_expect_tx(vn_full, BiCfg::VN_BYTES);
+    for (int kb = 0; kb < 4; ++kb) tma_load_4d(vnt + kb * KB_BYTES, &tma_q, vn_full, kb * BK, m0, b, 0);
+    issue(0);
+    issue(1);
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = *tmem_base_slot;
-  const uint32_t tmem_d = tmem_s + 256;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int b = tile / p.tiles_per_img, m0 = (tile - b * p.tiles_per_img) * BM;
-        // consumption order of the MMA issuer: S(0); then per head  S(h+1), D(h)
-        auto load = [&](int ph, int h) {
-          for (int kb = 0; kb < 4; ++kb, ++it) {
-            const int s = it % BI_STAGES;
-            mbar_wait(&empty_bar[s], ((it / BI_STAGES) & 1) ^ 1);
-            uint8_t* st = ring + s * BiCfg::STAGE_BYTES;
-            if (ph == 0) {  // S: A = image-token k-block (the same for every head: L2 hit), B = gT_h k-block
-              mbar_expect_tx(&full_bar[s], BiCfg::STAGE_BYTES);
-              tma_load_4d(st, &tma_q, &full_bar[s], kb * BK, m0, b, 0);
-              tma_load_4d(st + BiCfg::A_BYTES, &tma_k, &full_bar[s], kb * BK, 0, h, b);
-            } else {  // D: B = mT_h [256 o x 64 t]
-              mbar_expect_tx(&full_bar[s], BiCfg::B_BYTES);
-              tma_load_4d(st + BiCfg::A_BYTES, &tma_m, &full_bar[s], kb * BK, 0, h, b);
-            }
-          }
-        };
-        load(0, 0);
-        for (int h = 0; h < H; ++h) {
-          if (h + 1 < H) load(0, h + 1);
-          load(1, h);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, 256, 0);
-      int it = 0, hc = 0, tcnt = 0;
-      const uint32_t px_addr = smem_u32(px);
-      auto issue = [&](int ph, int h) {
-        // ph 0: S = Q_h K_h^T -> scratch columns;  1: D += P mT_h^T
-        for (int kb = 0; kb < 4; ++kb, ++it) {
-          const int s = it % BI_STAGES;
-          mbar_wait(&full_bar[s], (it / BI_STAGES) & 1);
-          tc_fence_after();
-          const uint32_t st = smem_u32(ring + s * BiCfg::STAGE_BYTES);
-          const uint32_t a0 = ph == 0 ? st : px_addr + kb * BiCfg::A_BYTES, b0 = st + BiCfg::A_BYTES;
-          const uint32_t acc = ph == 0 ? tmem_s : tmem_d;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_f16(acc, umma_desc_k_sw128(a0 + k * 32), umma_desc_k_sw128(b0 + k * 32), idesc,
-                       ((ph == 1 ? h : 0) | kb | k) != 0 ? 1u : 0u);
-          tc_commit(&empty_bar[s]);
-        }
-        tc_commit(ph == 0 ? s_full : op_done);
-      };
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcnt) {
-        // S of the item's first head (the previous item's last S must have been read out of the scratch columns)
-        if (hc > 0) {
-          mbar_wait(scratch_free, (hc - 1) & 1);
-          tc_fence_after();
-        }
-        issue(0, 0);
-        for (int h = 0; h < H; ++h, ++hc) {
-          if (h + 1 < H) {  // the next head's S only needs the scratch columns: it runs while P of this head is written
-            mbar_wait(scratch_free, hc & 1);
-            tc_fence_after();
-            issue(0, h + 1);
-          }
-          mbar_wait(p_ready, hc & 1);
-          tc_fence_after();
-          if (h == 0 && tcnt > 0) {  // the previous item's D must have been read by the epilogue
-            mbar_wait(dv_free, (tcnt - 1) & 1);
-            tc_fence_after();
-          }
-          issue(1, h);
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    const int ew = (warp - 4) & 3, part = (warp - 4) >> 2;
-    const int row = ew * 32 + lane, tid_e = threadIdx.x - 128;
-    const int sw = row & 7;
-    const uint32_t lane_addr = (uint32_t)(ew * 32) << 16;
-    const uint32_t px_row = smem_u32(px) + part * BiCfg::A_BYTES + row * 128;  // this thread's 128-byte row of k-block `part`
-    const uint32_t gk_addr0 = smem_u32(gk) + part * 64 * 4, rx_addr = smem_u32(rx) + row * 4, rsum_addr = smem_u32(rsum) + row * 4;
-    constexpr float L2E = 1.4426950408889634f;
-    const float NEG_INF = __int_as_float(0xff800000);
-    const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
-    const bool issuer = (tid_e == 0);
-    int hc = 0, tcnt = 0, cur_b = -1;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tcnt) {
-      const int b = tile / p.tiles_per_img, ti = tile - b * p.tiles_per_img, m0 = ti * BM;
-      const bool valid_row = m0 + row < p.N;
-      const bool full_tile = m0 + BM <= p.N;
-      if (b != cur_b) {  // token mask of this image (warp-uniform branch: every thread walks the same items)
-        asm volatile("bar.sync 1, 512;" ::: "memory");  // nobody still reads the previous image's flags
-        if (tid_e < 256) {
-          const bool kept = tid_e < p.T && (!p.mask || p.mask[(long)b * p.T + tid_e] != 0.f);
-          for (int hh = 0; hh < H; ++hh)
-            gk[hh * 256 + tid_e] = !kept ? NEG_INF : (p.gbias ? p.gbias[(((long)b * H + hh) * p.T + tid_e) * p.gb_ld] : 0.f);
-        }
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        cur_b = b;
-      }
-      for (int h = 0; h < H; ++h, ++hc) {
-        // ================= S -> P = softmax_t(clamp(S) + mask) =================
-        mbar_wait(s_full, hc & 1);
-        tc_fence_after();
-        const uint32_t t_s = tmem_s + lane_addr + (uint32_t)(part * 64);
-        const uint32_t kl_addr = gk_addr0 + (uint32_t)(h * 256 * 4);  // this head's additive term (query bias + token mask)
-        // ---- pass 1 over this thread's 64 tokens: column maxima (for the text side) and the partial row maximum ----
-        // The +-5e4 clamp of the scores (fuse_helper.py:245-252) is applied to the REDUCED values (clamp is monotonic:
-        // max(clamp(s)) == clamp(max(s))), not per element; `kl` carries the token mask as an additive 0 / -inf.
-        float mpart = NEG_INF;
-        {
-          uint32_t ra[16], rb[16];
-          tmem_ld_32x16(t_s, ra);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint32_t (&r)[16] = (j & 1) ? rb : ra;
-            tmem_ld_wait_dep(r);
-            if (j + 1 < 4) tmem_ld_32x16(t_s + (uint32_t)((j + 1) * 16), (j & 1) ? ra : rb);
-            float cm[16];
-            if (full_tile) {  // warp-uniform: every row of the tile is a real image token
-#pragma unroll
-              for (int i = 0; i < 16; ++i) cm[i] = warp_redux_max(__uint_as_float(r[i]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) cm[i] = warp_redux_max(valid_row ? __uint_as_float(r[i]) : NEG_INF);
-            }
-            if (lane == 0) {  // the reduction result is warp-uniform: one lane stores the 16 column maxima of this warp's 32 rows
-              const uint32_t dst = smem_u32(cmx) + (uint32_t)((ew * 256 + part * 64 + j * 16) * 4);
-#pragma unroll
-              for (int i4 = 0; i4 < 4; ++i4)
-                sts128(dst + i4 * 16, __float_as_uint(cm[i4 * 4]), __float_as_uint(cm[i4 * 4 + 1]), __float_as_uint(cm[i4 * 4 + 2]),
-                       __float_as_uint(cm[i4 * 4 + 3]));
-            }
-#pragma unroll
-            for (int i4 = 0; i4 < 4; ++i4) {
-              const float4 kf = lds128f(kl_addr + (uint32_t)((j * 16 + i4 * 4) * 4));
-              mpart = fmaxf(mpart, __uint_as_float(r[i4 * 4 + 0]) + kf.x);
-              mpart = fmaxf(mpart, __uint_as_float(r[i4 * 4 + 1]) + kf.y);
-              mpart = fmaxf(mpart, __uint_as_float(r[i4 * 4 + 2]) + kf.z);
-              mpart = fmaxf(mpart, __uint_as_float(r[i4 * 4 + 3]) + kf.w);
-            }
-          }
-        }
-        rx[part * BM + row] = mpart;
-        // the previous item's output staging (PX) must have been read by the TMA store before P overwrites it
-        if (issuer && h == 0 && tcnt > 0) tma_store_wait_read_all();
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        if (tid_e < p.T) {  // column-max partial of this (image, head, tile), clamped like the scores
-          float c4 = fmaxf(fmaxf(cmx[tid_e], cmx[256 + tid_e]), fmaxf(cmx[512 + tid_e], cmx[768 + tid_e]));
-          if (p.gbias) c4 += p.gbias[(((long)b * H + h) * p.T + tid_e) * p.gb_ld];  // the text side sees the full score, no mask
-          c4 = fminf(fmaxf(c4, -clampv), clampv);
-          p.colmax_part[(((long)b * H + h) * p.tiles_per_img + ti) * p.T + tid_e] = c4;
-        }
-        const float m_raw = fmaxf(fmaxf(lds32f(rx_addr), lds32f(rx_addr + BM * 4)), fmaxf(lds32f(rx_addr + 2 * BM * 4), lds32f(rx_addr + 3 * BM * 4)));
-        // every token masked: the reference's fp32 sum A + (-9e15) swallows A and the softmax is uniform over the T tokens
-        const bool uniform = (m_raw == NEG_INF);
-        const float m = fminf(fmaxf(m_raw, -clampv), clampv);  // max over the kept tokens of the CLAMPED scores
-        const float ml2 = uniform ? 0.f : m * L2E;
-        // per-element clamping can only change exp(clamp(s) - m) when the row maximum itself exceeds the clamp (s > 5e4), or
-        // when m is so low that exp(-5e4 - m) does not underflow; otherwise exp(s - m) is bit-identical without it
-        const bool need_clamp = (m_raw > clampv) || (m_raw < -clampv + 256.f);
-        // ---- pass 2: e = exp(S - rowmax) kept in registers, partial row sum ----
-        float e[64];
-        float lpart = 0.f;
-        {
-          uint32_t ra[16], rb[16];
-          tmem_ld_32x16(t_s, ra);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint32_t (&r)[16] = (j & 1) ? rb : ra;
-            tmem_ld_wait_dep(r);
-            if (j + 1 < 4) tmem_ld_32x16(t_s + (uint32_t)((j + 1) * 16), (j & 1) ? ra : rb);
-            if (j == 3) {  // S has left the scratch columns: they may take the next head's S
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(scratch_free);
-            }
-            if (!need_clamp && !uniform) {  // the common path: 4 issue slots per score (FADD, FFMA, MUFU.EX2, FADD)
-#pragma unroll
-              for (int i4 = 0; i4 < 4; ++i4) {
-                const float4 kf = lds128f(kl_addr + (uint32_t)((j * 16 + i4 * 4) * 4));
-                const float kk[4] = {kf.x, kf.y, kf.z, kf.w};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  // kk = folded query bias of this (head, token), or -inf on a masked token: exp2(-inf) = 0, exactly what the
-                  // reference's -9e15 does in fp32
-                  const float ev = ex2_approx(fmaf(__uint_as_float(r[i4 * 4 + i]) + kk[i], L2E, -ml2));
-                  e[j * 16 + i4 * 4 + i] = ev;
-                  lpart += ev;
-                }
-              }
-            } else {
-#pragma unroll
-              for (int i4 = 0; i4 < 4; ++i4) {
-                const float4 kf = lds128f(kl_addr + (uint32_t)((j * 16 + i4 * 4) * 4));
-                const float kk[4] = {kf.x, kf.y, kf.z, kf.w};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const int c = j * 16 + i4 * 4 + i;
-                  const float sc = fminf(fmaxf(__uint_as_float(r[i4 * 4 + i]) + kk[i], -clampv), clampv);
-                  float ev = (kk[i] == NEG_INF) ? 0.f : ex2_approx(fmaf(sc, L2E, -ml2));
-                  if (uniform) ev = (part * 64 + c < p.T) ? 1.f : 0.f;
-                  e[c] = ev;
-                  lpart += ev;
-                }
-              }
-            }
-          }
-        }
-        rsum[part * BM + row] = lpart;
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        const float inv = 1.f / (lds32f(rsum_addr) + lds32f(rsum_addr + BM * 4) + lds32f(rsum_addr + 2 * BM * 4) + lds32f(rsum_addr + 3 * BM * 4));
-        if (hc > 0) mbar_wait(op_done, (hc - 1) & 1);  // the previous head's product no longer reads PX
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          sts128(px_row + ((j ^ sw) << 4), pack_half2(e[8 * j] * inv, e[8 * j + 1] * inv), pack_half2(e[8 * j + 2] * inv, e[8 * j + 3] * inv),
-                 pack_half2(e[8 * j + 4] * inv, e[8 * j + 5] * inv), pack_half2(e[8 * j + 6] * inv, e[8 * j + 7] * inv));
-        fence_proxy_async();  // generic-proxy writes of P -> visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_ready);
-      }
-      // ================= item epilogue: out = res + gamma * (D + bias) =================
-      mbar_wait(op_done, (hc - 1) & 1);  // the last head's product: D complete, PX free
-      tc_fence_after();
-      {
-        const bool has_res = p.res != nullptr && valid_row;
-        const uint4* src = reinterpret_cast<const uint4*>(p.res + (long)b * p.res_b + (long)(m0 + row) * p.res_ld + part * 64);
-        const uint32_t t_d = tmem_d + lane_addr + (uint32_t)(part * 64);
-        const float4* gam4 = reinterpret_cast<const float4*>(p.gamma) + part * 16;
-        const float4* bia4 = reinterpret_cast<const float4*>(p.bias) + part * 16;
-        uint32_t ra[16], rb[16];
-        tmem_ld_32x16(t_d, ra);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {  // 16 columns = two 16-byte chunks per step
-          uint32_t (&r)[16] = (j & 1) ? rb : ra;
-          uint4 rq0 = make_uint4(0, 0, 0, 0), rq1 = make_uint4(0, 0, 0, 0);
-          if (has_res) {
-            rq0 = __ldg(src + 2 * j);
-            rq1 = __ldg(src + 2 * j + 1);
-          }
-          tmem_ld_wait_dep(r);
-          if (j + 1 < 4) tmem_ld_32x16(t_d + (uint32_t)((j + 1) * 16), (j & 1) ? ra : rb);
-          if (j == 3) {  // D has been read: the next item's products may overwrite it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(dv_free);
-          }
-          float o[16];
-#pragma unroll
-          for (int i4 = 0; i4 < 4; ++i4) {
-            const float4 sv = p.gamma ? __ldg(gam4 + j * 4 + i4) : make_float4(1.f, 1.f, 1.f, 1.f);
-            const float4 bv = p.bias ? __ldg(bia4 + j * 4 + i4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            o[i4 * 4 + 0] = (__uint_as_float(r[i4 * 4 + 0]) + bv.x) * sv.x;  // gamma * (D + bias)
-            o[i4 * 4 + 1] = (__uint_as_float(r[i4 * 4 + 1]) + bv.y) * sv.y;
-            o[i4 * 4 + 2] = (__uint_as_float(r[i4 * 4 + 2]) + bv.z) * sv.z;
-            o[i4 * 4 + 3] = (__uint_as_float(r[i4 * 4 + 3]) + bv.w) * sv.w;
-          }
-          const __half2* h0 = reinterpret_cast<const __half2*>(&rq0);
-          const __half2* h1 = reinterpret_cast<const __half2*>(&rq1);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 f0 = __half22float2(h0[i]), f1 = __half22float2(h1[i]);
-            o[2 * i] += f0.x;
-            o[2 * i + 1] += f0.y;
-            o[8 + 2 * i] += f1.x;
-            o[8 + 2 * i + 1] += f1.y;
-          }
-          sts128(px_row + (((2 * j) ^ sw) << 4), pack_half2(o[0], o[1]), pack_half2(o[2], o[3]), pack_half2(o[4], o[5]),
-                 pack_half2(o[6], o[7]));
-          sts128(px_row + (((2 * j + 1) ^ sw) << 4), pack_half2(o[8], o[9]), pack_half2(o[10], o[11]), pack_half2(o[12], o[13]),
-                 pack_half2(o[14], o[15]));
-        }
-      }
-      fence_proxy_async();
-      asm volatile("bar.sync 1, 512;" ::: "memory");
-      if (issuer) {
-        for (int cb = 0; cb < 4; ++cb) tma_store_4d(&tma_o, px + cb * BiCfg::A_BYTES, cb * 64, m0, b, 0);
-        tma_store_commit();
-      }
-    }
-    if (issuer) tma_store_wait_read_all();
+  constexpr float L2E = 1.4426950408889634f;
+  const float NEG_INF = __int_as_float(0xff800000);
+  const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
+  for (int t = tid; t < 256; t += 128) {
+    const bool kept = t < p.T && (!p.mask || p.mask[(long)b * p.T + t] != 0.f);
+    for (int hh = 0; hh < H; ++hh)
+      gk[hh * 256 + t] = !kept ? NEG_INF : (p.gbias ? p.gbias[(((long)b * H + hh) * p.T + t) * p.gb_ld] : 0.f);
   }
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_s, 512);
+  bool valid[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) valid[h] = m0 + wg_row(tid, 2 * h) < p.N;
+  const uint32_t vn_addr = smem_u32(vnt);
+  int q = 0;
+  auto ring_wait = [&](int qq) { mbar_wait(&full[qq & 1], (qq >> 1) & 1); };
+  auto ring_release = [&](int qq) {  // every wgmma of the warpgroup has read stage qq & 1
+    __syncthreads();
+    if (tid == 0 && qq + 2 < nq) issue(qq + 2);
+  };
+  mbar_wait(vn_full, 0);
+  for (int h = 0; h < H; ++h) {
+    // ================= S = vn . gT_h^T =================
+    float sc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) sc[j] = 0.f;
+    for (int kb = 0; kb < 4; ++kb, ++q) {
+      ring_wait(q);
+      const uint32_t b0 = smem_u32(ring + (q & 1) * BiCfg::STAGE_BYTES);
+      wgmma_fence_acc(sc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss_m64n256_kk(sc, wg_desc_k_sw128(vn_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(b0 + k * 32), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(sc);
+      ring_release(q);
+    }
+    // ---- column maxima over the tile's valid rows (for the text side): two rows per thread, then the 8 row groups of the warp,
+    //      then the 4 warps through shared memory.  The +-5e4 clamp (fuse_helper.py:245-252) is applied to the REDUCED values
+    //      (clamp is monotonic) ----
+#pragma unroll
+    for (int j = 0; j < 128; j += 4) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        float m = fmaxf(valid[0] ? sc[j + c] : NEG_INF, valid[1] ? sc[j + 2 + c] : NEG_INF);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
+        if (lane < 4) cmx[warp * 256 + wg_col(tid, j + c)] = m;
+      }
+    }
+    __syncthreads();
+    for (int t = tid; t < p.T; t += 128) {
+      float c4 = fmaxf(fmaxf(cmx[t], cmx[256 + t]), fmaxf(cmx[512 + t], cmx[768 + t]));
+      if (p.gbias) c4 += p.gbias[(((long)b * H + h) * p.T + t) * p.gb_ld];  // the text side sees the full score, no mask
+      c4 = fminf(fmaxf(c4, -clampv), clampv);
+      p.colmax_part[(((long)b * H + h) * p.tiles_per_img + ti) * p.T + t] = c4;
+    }
+    // ---- row softmax over the T tokens; `kk` carries the folded query bias and the token mask as an additive 0 / -inf ----
+    const float* kl = gk + h * 256;
+    float mr[2] = {NEG_INF, NEG_INF};
+#pragma unroll
+    for (int j = 0; j < 128; ++j) mr[(j >> 1) & 1] = fmaxf(mr[(j >> 1) & 1], sc[j] + kl[wg_col(tid, j)]);
+    float ml2[2];
+    bool uniform[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float m_raw = quad_max(mr[r]);
+      // every token masked: the reference's fp32 sum A + (-9e15) swallows A and the softmax is uniform over the T tokens
+      uniform[r] = (m_raw == NEG_INF);
+      ml2[r] = uniform[r] ? 0.f : fminf(fmaxf(m_raw, -clampv), clampv) * L2E;  // max over the kept tokens of the CLAMPED scores
+    }
+    float ls[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 128; ++j) {
+      const int r = (j >> 1) & 1, c = wg_col(tid, j);
+      const float kk = kl[c];
+      float ev = (kk == NEG_INF) ? 0.f : ex2_approx(fmaf(fminf(fmaxf(sc[j] + kk, -clampv), clampv), L2E, -ml2[r]));
+      if (uniform[r]) ev = (c < p.T) ? 1.f : 0.f;
+      sc[j] = ev;
+      ls[r] += ev;
+    }
+    const float inv[2] = {1.f / quad_sum(ls[0]), 1.f / quad_sum(ls[1])};
+#pragma unroll
+    for (int j = 0; j < 128; ++j) sc[j] *= inv[(j >> 1) & 1];
+    uint32_t pa[16][4];
+#pragma unroll
+    for (int kk = 0; kk < 16; ++kk) acc_to_a(sc, kk, pa[kk]);
+    // ================= D_h = P . mT_h^T, added to the head sum =================
+    float d[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) d[j] = 0.f;
+    for (int kb = 0; kb < 4; ++kb, ++q) {
+      ring_wait(q);
+      const uint32_t b0 = smem_u32(ring + (q & 1) * BiCfg::STAGE_BYTES);
+      wgmma_fence_acc(d);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_rs_m64n256_kk(d, pa[kb * 4 + k], wg_desc_k_sw128(b0 + k * 32), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(d);
+      ring_release(q);
+    }
+#pragma unroll
+    for (int j = 0; j < 128; ++j) dsum[j * 128 + tid] = (h == 0 ? 0.f : dsum[j * 128 + tid]) + d[j];
+  }
+  // ================= epilogue: out = res + gamma * (D + bias) =================
+#pragma unroll 4
+  for (int j = 0; j < 128; j += 2) {
+    const long row = m0 + wg_row(tid, j);
+    const int c = wg_col(tid, j);
+    if (row >= p.N) continue;
+    float o0 = dsum[j * 128 + tid], o1 = dsum[(j + 1) * 128 + tid];
+    const float g0 = p.gamma ? p.gamma[c] : 1.f, g1 = p.gamma ? p.gamma[c + 1] : 1.f;
+    const float b0 = p.bias ? p.bias[c] : 0.f, b1 = p.bias ? p.bias[c + 1] : 0.f;
+    o0 = (o0 + b0) * g0;  // gamma * (D + bias)
+    o1 = (o1 + b1) * g1;
+    if (p.res) {
+      const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.res + (long)b * p.res_b + row * p.res_ld + c));
+      o0 += r.x;
+      o1 += r.y;
+    }
+    *reinterpret_cast<__half2*>(p.out + (long)b * p.o_b + row * p.o_ld + c) = __floats2half2_rn(o0, o1);
   }
 }
 
@@ -714,7 +438,7 @@ static int text_launch(bool vn, const float* rowbias, int64_t rb_ld, const void*
   for (int64_t x : lds) MQ_REQUIRE((x % 8) == 0, "biattn_text: strides must be multiples of 8 elements");
   MQ_REQUIRE(((uintptr_t)k % 16) == 0 && ((uintptr_t)q % 16) == 0 && ((uintptr_t)v % 16) == 0 && ((uintptr_t)out % 16) == 0,
              "biattn_text: operands must be 16-byte aligned");
-  CUtensorMap mk, mq, mv, mo;
+  CUtensorMap mk, mq, mv;
   BtP p;
   memset(&p, 0, sizeof(p));
   int rc = make_operand_map(&mk, k, T, d, k_ld, (int)nb1, k_b1, (int)nb2, k_b2, BM, &p.k_bc1, &p.k_bc2);
@@ -722,13 +446,15 @@ static int text_launch(bool vn, const float* rowbias, int64_t rb_ld, const void*
   rc = make_operand_map(&mq, q, N, d, q_ld, (int)nb1, q_b1, (int)nb2, q_b2, BT_STEP, &p.q_bc1, &p.q_bc2);
   if (rc) return rc;
   if (vn)  // image tokens [N][256 c]: box [64 n x 64 c]
-    rc = make_operand_map(&mv, v, N, 256, v_ld, (int)nb1, v_b1, (int)nb2, v_b2, BT_SUB, &p.v_bc1, &p.v_bc2);
+    rc = make_operand_map(&mv, v, N, 256, v_ld, (int)nb1, v_b1, (int)nb2, v_b2, BT_STEP, &p.v_bc1, &p.v_bc2);
   else     // Vv^T [256 d][Np]: box [256 d x 64 n]
     rc = make_operand_map(&mv, v, d, Np, v_ld, (int)nb1, v_b1, (int)nb2, v_b2, 256, &p.v_bc1, &p.v_bc2);
   if (rc) return rc;
   MQ_REQUIRE((nb1 == 1 || o_b1 != 0) && (nb2 == 1 || o_b2 != 0), "biattn_text: output batch strides must be non-zero");
-  rc = make_store_map(&mo, out, MQDET_F16, T, d, o_ld, (int)nb1, o_b1, (int)nb2, o_b2);
-  if (rc) return rc;
+  p.out = (__half*)out;
+  p.o_ld = o_ld;
+  p.o_b1 = o_b1;
+  p.o_b2 = o_b2;
   p.stat = stat;
   p.clamp = clamp;
   p.nb1 = (int)nb1;
@@ -737,20 +463,15 @@ static int text_launch(bool vn, const float* rowbias, int64_t rb_ld, const void*
   p.n_steps = (int)((N + BT_STEP - 1) / BT_STEP);
   p.rowbias = rowbias;
   p.rb_ld = (int)(rb_ld > 0 ? rb_ld : 1);
-  p.vn_lbo = BT_SUB * 128;  // next 64 channels: the next [64 n x 64 c] block
-  p.vn_sbo = 1024;          // next 8 image tokens
-  if (const char* dbg = getenv("MQDET_VN_DESC_SWAP")) {  // bring-up aid: swap the two strides
-    if (atoi(dbg)) { p.vn_lbo = 1024; p.vn_sbo = BT_SUB * 128; }
-  }
   dim3 grid((unsigned)((T + BM - 1) / BM), (unsigned)(nb1 * nb2));
   if (vn) {
     rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel<true>), BtCfg::SMEM_BYTES);
     if (rc) return rc;
-    biattn_text_kernel<true><<<grid, 640, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, mo, p);
+    biattn_text_kernel<true><<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
   } else {
     rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel<false>), BtCfg::SMEM_BYTES);
     if (rc) return rc;
-    biattn_text_kernel<false><<<grid, 640, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, mo, p);
+    biattn_text_kernel<false><<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
   }
   return check_launch("biattn_text_kernel");
 }
@@ -788,7 +509,7 @@ extern "C" int mqdet_biattn_image(const void* vn, int64_t vn_ld, int64_t vn_b, c
   MQ_REQUIRE(((uintptr_t)vn % 16) == 0 && ((uintptr_t)gT % 16) == 0 && ((uintptr_t)mT % 16) == 0 && ((uintptr_t)out % 16) == 0 &&
                  ((uintptr_t)res % 16) == 0 && ((uintptr_t)bias % 16) == 0 && ((uintptr_t)gamma % 16) == 0,
              "biattn_image: operands must be 16-byte aligned");
-  CUtensorMap mq, mk, mm, mo;
+  CUtensorMap mq, mk, mm;
   int bc1, bc2;
   int rc = make_operand_map(&mq, vn, N, 256, vn_ld, (int)B, vn_b, 1, 0, BM, &bc1, &bc2);
   if (rc) return rc;
@@ -798,8 +519,6 @@ extern "C" int mqdet_biattn_image(const void* vn, int64_t vn_ld, int64_t vn_b, c
   rc = make_operand_map(&mm, mT, 256, T, m_ld, (int)H, m_bh, (int)B, m_b, 256, &bc1, &bc2);  // [B][H][256 o][T]
   if (rc) return rc;
   MQ_REQUIRE(B == 1 || o_b != 0, "biattn_image: output batch stride must be non-zero");
-  rc = make_store_map(&mo, out, MQDET_F16, N, 256, o_ld, (int)B, o_b, 1, 0);
-  if (rc) return rc;
   BiP p;
   memset(&p, 0, sizeof(p));
   p.mask = mask;
@@ -808,17 +527,18 @@ extern "C" int mqdet_biattn_image(const void* vn, int64_t vn_ld, int64_t vn_b, c
   p.res = (const __half*)res;
   p.res_ld = res_ld;
   p.res_b = res_b;
+  p.out = (__half*)out;
+  p.o_ld = o_ld;
+  p.o_b = o_b;
   p.colmax_part = workspace;
   p.gbias = gbias;
   p.gb_ld = (int)(gb_ld > 0 ? gb_ld : 1);
   p.clamp = clamp;
   p.B = (int)B; p.H = (int)H; p.T = (int)T; p.N = (int)N;
   p.tiles_per_img = (int)((N + BM - 1) / BM);
-  p.total_tiles = p.tiles_per_img * (int)B;
   rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_image_kernel), BiCfg::SMEM_BYTES);
   if (rc) return rc;
-  const int grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-  biattn_image_kernel<<<grid, 640, BiCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mq, mk, mm, mo, p);
+  biattn_image_kernel<<<(unsigned)(p.tiles_per_img * B), 128, BiCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mq, mk, mm, p);
   rc = check_launch("biattn_image_kernel");
   if (rc) return rc;
   colmax_reduce_kernel<<<(unsigned)(B * H), 256, 0, (cudaStream_t)stream>>>(workspace, p.tiles_per_img, (int)T, colmax);

@@ -27,7 +27,7 @@ int check_launch(const char* what) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Host helpers shared by the tcgen05 kernels: TMA tensor maps (cached per thread: encoding one costs a driver call, and the
+// Host helpers shared by the TMA / wgmma kernels: TMA tensor maps (cached per thread: encoding one costs a driver call, and the
 // same (pointer, shape) tuples recur every step because the caller's allocator recycles its blocks), the SM count and the
 // dynamic shared-memory opt-in, both per device.
 // ---------------------------------------------------------------------------------------------------------------------
@@ -164,7 +164,7 @@ int num_sms() {
   int v = n[slot].load(std::memory_order_relaxed);
   if (!v) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    if (v <= 0) v = 148;
+    if (v <= 0) v = 132;
     n[slot].store(v, std::memory_order_relaxed);
   }
   const int r = g_reserved_sms.load(std::memory_order_relaxed);

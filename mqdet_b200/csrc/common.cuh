@@ -1,5 +1,5 @@
-// mqdet_b200 — shared device/host helpers for the sm_100a kernels.
-// PTX wrappers (mbarrier, TMA, tcgen05) are written out here so the kernels read as plain CUDA.
+// mqdet_b200 — shared device/host helpers for the sm_90a kernels.
+// PTX wrappers (mbarrier, TMA, wgmma) are written out here so the kernels read as plain CUDA.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -50,7 +50,7 @@ static inline int fill_levels(LevelTable* t, const int32_t* hw, int64_t nlev) {
   return off;
 }
 
-// host helpers of the tcgen05 kernels (capi.cu): cached TMA tensor maps, per-device SM count / shared-memory opt-in
+// host helpers of the TMA / wgmma kernels (capi.cu): cached TMA tensor maps, per-device SM count / shared-memory opt-in
 int make_operand_map(CUtensorMap* map, const void* ptr, long rows, long K, long ld, int nb1, long s1, int nb2, long s2,
                      int box_rows, int* bcast1, int* bcast2);
 int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2);
@@ -120,31 +120,15 @@ __device__ __forceinline__ uint32_t pack_half2(float x, float y) {
   const __half2 h = __floats2half2_rn(x, y);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-// packed fp32x2 FMA (sm_100): (d0, d1) = (a0, a1) * (s, s) + (b0, b1) in ONE issue slot
+// (d0, d1) = (a0, a1) * s + (b0, b1): two fused multiply-adds
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float s, float b0, float b1) {
-  asm("{\n"
-      ".reg .b64 va, vs, vb, vd;\n"
-      "mov.b64 va, {%2, %3};\n"
-      "mov.b64 vs, {%4, %4};\n"
-      "mov.b64 vb, {%5, %6};\n"
-      "fma.rn.f32x2 vd, va, vs, vb;\n"
-      "mov.b64 {%0, %1}, vd;\n"
-      "}\n"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(s), "f"(b0), "f"(b1));
+  d0 = fmaf(a0, s, b0);
+  d1 = fmaf(a1, s, b1);
 }
 // (d0, d1) = (a0, a1) * (s0, s1) + (b0, b1)
 __device__ __forceinline__ void ffma2v(float& d0, float& d1, float a0, float a1, float s0, float s1, float b0, float b1) {
-  asm("{\n"
-      ".reg .b64 va, vs, vb, vd;\n"
-      "mov.b64 va, {%2, %3};\n"
-      "mov.b64 vs, {%4, %5};\n"
-      "mov.b64 vb, {%6, %7};\n"
-      "fma.rn.f32x2 vd, va, vs, vb;\n"
-      "mov.b64 {%0, %1}, vd;\n"
-      "}\n"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(s0), "f"(s1), "f"(b0), "f"(b1));
+  d0 = fmaf(a0, s0, b0);
+  d1 = fmaf(a1, s1, b1);
 }
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -216,117 +200,46 @@ __device__ __forceinline__ void tma_store_commit_and_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-// ---- tcgen05 / TMEM ------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Whole warp. Writes the TMEM base address (lane<<16 | column) to *smem_out.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_out, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_out)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (fp16/bf16 operands, fp32 accumulate).
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                           uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <- lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread.
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// wait::ld that also "touches" the destination registers of an earlier tcgen05.ld, so that the compiler cannot schedule
-// their first use above the wait when the load was issued several statements earlier (software-pipelined epilogue)
-__device__ __forceinline__ void tmem_ld_wait_dep(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
+// ---- wgmma (sm_90a warpgroup MMA) -----------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, 128-byte-swizzled shared-memory matrix descriptor (8-row groups 1024 B apart).
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused: 1)
-//   bits [32,46) stride byte offset >> 4   bits [46,48) descriptor version = 1 (Blackwell)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// K-major, 128-byte-swizzled shared-memory matrix descriptor (8-row groups 1024 B apart; the tile base 1024-aligned).
+//   bits [0,14) start address >> 4   bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout: 1 = SWIZZLE_128B
+// Advancing the start address by 32 B steps 16 fp16 along K inside the swizzle row.
+__device__ __forceinline__ uint64_t wg_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-
-// MN-major (the M / N index is the contiguous one), 128-byte-swizzled descriptor: the swizzle atom is 64 MN elements (128 B)
-// x 8 K rows; `lbo` = byte distance between atoms along MN (next 64 elements), `sbo` = between atoms along K (next 8 rows).
-// Used with the matching major bit of the instruction descriptor (UMMA_A_MN_MAJOR / UMMA_B_MN_MAJOR).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+// MN-major (the M / N index is the contiguous one), 128-byte-swizzled: the swizzle atom is 64 MN elements (128 B) x 8 K rows;
+// `lbo` = byte distance between atoms along MN (next 64 elements), `sbo` = between atoms along K (next 8 rows).
+__device__ __forceinline__ uint64_t wg_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-constexpr uint32_t UMMA_A_MN_MAJOR = 1u << 15;
-constexpr uint32_t UMMA_B_MN_MAJOR = 1u << 16;
+// Accumulator fragment of a 64 x N wgmma: thread t of the warpgroup holds d[i] at
+//   row = 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),   col = 8 * (i / 4) + 2 * (t % 4) + (i % 2)
+__device__ __forceinline__ int wg_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int wg_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
 
-// warp-wide max of an fp32 value in one instruction (sm_100a CREDUX.MAX.F32); every lane receives the result
-__device__ __forceinline__ float warp_redux_max(float v) {
-  float r;
-  asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-  return r;
-}
-
-// erf-GELU of TWO values with the packed fp32x2 FMA pipe (sm_100): the same Abramowitz-Stegun 7.1.26 form as gelu_fast,
+// erf-GELU of TWO values: the same Abramowitz-Stegun 7.1.26 form as gelu_fast,
 //   gelu(x) = 0.5 (x + |x| (1 - erfc(|z|))),  z = x / sqrt(2),  erfc(|z|) = t P4(t) exp(-z^2),  t = 1 / (1 + 0.3275911 |z|),
 // with z pre-scaled by sqrt(log2 e) so that exp(-z^2) is one MUFU.EX2 of -(z')^2.  ~10 issue slots per value instead of ~17:
 // the GELU epilogues of the K <= 384 MLP GEMMs (Swin fc1, FFNs) are issue-bound on the eight epilogue warps.
@@ -353,12 +266,6 @@ __device__ __forceinline__ void gelu_fast2(float& x0, float& x1) {
   ffma2v(u0, u1, -a0, -a1, e0, e1, a0, a1);                   // |x| (1 - erfc)
   ffma2(h0, h1, x0, x1, 0.5f, 0.f, 0.f);
   ffma2(x0, x1, u0, u1, 0.5f, h0, h1);                        // 0.5 x + 0.5 |x| (1 - erfc)
-}
-
-// kind::f16 instruction descriptor: fp16 A/B (format 0) or bf16 (1), fp32 accumulate, K-major A/B.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int ab_format) {
-  return (1u << 4) | ((uint32_t)ab_format << 7) | ((uint32_t)ab_format << 10) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 }  // namespace mqdet

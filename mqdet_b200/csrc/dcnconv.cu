@@ -1,4 +1,4 @@
-// mqdet_b200 — DyConv's DCNv2 3x3 convolutions as ONE implicit GEMM on tcgen05 (no column matrix in HBM).
+// mqdet_b200 — DyConv's DCNv2 3x3 convolutions as ONE implicit GEMM on the sm_90a tensor cores (no column matrix in HBM).
 //
 // Reference: maskrcnn_benchmark/modeling/rpn/vldyhead.py DyConv.forward :205-247 (three ModulatedDeformConv per layer);
 //            maskrcnn_benchmark/csrc/cuda/deform_conv_kernel_cuda.cu :473-505 (bilinear), :578-641 (modulated im2col),
@@ -7,44 +7,37 @@
 //   y_j[rows_j, 256] = A_j[rows_j, 2304] * W_j[256, 2304]^T + bias_j        (k = tap*256 + c; j = one of the three branches)
 //
 // A_j is the bilinearly sampled, mask-modulated column matrix of dyhead.cu's dcn_cols_kernel — here it only ever exists as
-// 128x64 fp16 tiles in shared memory.  Persistent, one CTA (768 threads) per SM walks the 128-row tiles of ALL jobs of the
-// launch (1400 + 350 + 350 tiles for DyConv at the benchmark shape):
-//   * warps 8-23 (gather): per tile, every (pixel, tap) gets ONE sampling record in shared memory (four corner offsets, four
-//     corner weights with the modulation mask folded in; 36 KB); then, per k-block (tap, 64 channels), four threads per pixel
-//     fetch 32 contiguous bytes of each corner row (one 256-bit load: a warp's request covers eight full 128-byte lines), blend
-//     in fp32 (packed FFMA2), round once to fp16 and store straight into the 128B-swizzled K-major A stage; the loads of
-//     k-block kb+1 are issued before k-block kb is blended;
-//   * warp 0: the [256 x 64] weight tile of the k-block by TMA;  warp 1: four tcgen05.mma 128x256x16 per k-block, fp32
-//     accumulator in TMEM (two of them: the epilogue of tile i overlaps the mainloop of tile i+1);
-//   * warps 4-7 (epilogue): TMEM -> +bias -> fp16 -> swizzled staging window -> TMA store, 64 columns at a time.
-//
-// HBM traffic per DyConv layer at B=8, 800x1344 (ncu): 245 MB read + 113 MB written (algorithmic: 92 MB of x, 3.5 MB of weights,
-// 138 MB of y) — against 1.24 GB written + 1.24 GB read for the materialised column matrix.  What bounds it now is the L2 -> SM
-// rate: per k-block an SM takes in the 32 KB weight tile plus ~45 KB of corner rows (64 KB at the measured 31 % L1 hit rate):
-// 5.9 GB per layer (ncu lts__t_sectors) in 0.545 ms = 10.7 TB/s, against the ~12 TB/s the L2 delivers chip-wide; 600 TFLOP/s,
-// tensor pipe 31 % active.  Sharing the weight tile between the two CTAs of a cluster by TMA multicast was measured and changes
-// nothing (0.57 ms): the limit is what each SM can take in, not what the L2 slices read.
+// 64x64 fp16 tiles in shared memory.  Persistent, one CTA (384 threads) per SM walks the 64-row tiles of ALL jobs of the launch:
+//   * warps 8-11 (gather): per tile, every (pixel, tap) gets ONE sampling record in shared memory (four corner offsets, four
+//     corner weights with the modulation mask folded in; 18 KB); then, per k-block (tap, 64 channels), two threads per pixel
+//     fetch 64 contiguous bytes of each corner row (four 128-bit loads), blend in fp32, round once to fp16 and store straight
+//     into the 128B-swizzled K-major A stage; the loads of k-block kb+1 are issued before k-block kb is stored;
+//   * warp 0: the [256 x 64] weight tile of the k-block by TMA;
+//   * warps 4-7 (one warpgroup): four wgmma.m64n256k16 per k-block, fp32 accumulator in registers (128 per thread), then
+//     +bias -> fp16 -> global stores straight from the accumulator fragments.
+// 64-row tiles keep the 64 x 256 accumulator in one warpgroup's registers next to the gather warps.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/mqdet_b200.h"
 
 namespace mqdet {
 
-constexpr int DC_BM = 128, DC_BN = 256, DC_BK = 64, DC_C = 256, DC_TAPS = 9;
-constexpr int DC_STAGES = 3;
-constexpr int DC_A_BYTES = DC_BM * DC_BK * 2;  // 16 KB
+constexpr int DC_BM = 64, DC_BN = 256, DC_BK = 64, DC_C = 256, DC_TAPS = 9;
+constexpr int DC_STAGES = 4;
+constexpr int DC_A_BYTES = DC_BM * DC_BK * 2;  // 8 KB
 constexpr int DC_B_BYTES = DC_BN * DC_BK * 2;  // 32 KB
-constexpr int DC_STG_BYTES = DC_BM * 128;      // one 64-column fp16 window of the output tile
 constexpr int DC_KB = DC_TAPS * DC_C / DC_BK;  // 36 k-blocks: tap = kb / 4, channels (kb % 4) * 64 ..
-constexpr int DC_GATHER_WARPS = 16;
-constexpr int DC_THREADS = 256 + DC_GATHER_WARPS * 32;  // warps 0-3 control, 4-7 epilogue, 8-23 gather
+constexpr int DC_GATHER_WARPS = 4;
+constexpr int DC_GATHER_THREADS = DC_GATHER_WARPS * 32;  // two per pixel
+constexpr int DC_THREADS = 256 + DC_GATHER_THREADS;      // warp 0 TMA, warps 4-7 MMA + epilogue, warps 8-11 gather
 constexpr int DC_COORD_BYTES = DC_TAPS * DC_BM * 32;     // per (tap, row): 4 corner offsets + 4 corner weights
-constexpr int DC_SMEM_BYTES = DC_STAGES * (DC_A_BYTES + DC_B_BYTES) + 2 * DC_STG_BYTES + DC_COORD_BYTES + 1024 /*align*/ +
-                              256 /*barriers*/ + DC_BN * 4 /*bias row*/;
+constexpr int DC_SMEM_BYTES = DC_STAGES * (DC_A_BYTES + DC_B_BYTES) + DC_COORD_BYTES + 1024 /*align*/ + 256 /*barriers*/ +
+                              DC_BN * 4 /*bias row*/;
 static_assert(DC_SMEM_BYTES <= 232448, "dcn_conv: shared memory budget");
 
 struct DcnP {
   CUtensorMap map_w[MQDET_DCN_MAX_JOBS];  // weights  [256][2304] fp16, box 64 x 256
-  CUtensorMap map_y[MQDET_DCN_MAX_JOBS];  // outputs  [rows][256]  fp16, box 64 x 128
+  __half* y[MQDET_DCN_MAX_JOBS];          // outputs  [rows][256]  fp16
   const __half* x;
   const float* om;
   const float* bias[MQDET_DCN_MAX_JOBS];
@@ -56,22 +49,13 @@ struct DcnP {
   LevelTable lt;
 };
 
-// 32 contiguous bytes (16 fp16 channels) of a corner row in ONE request: a warp's load then covers 8 full 128-byte lines
-struct U8 { uint4 lo, hi; };
-__device__ __forceinline__ U8 ldg256(const __half* p) {
-  U8 v;
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v.lo.x), "=r"(v.lo.y), "=r"(v.lo.z), "=r"(v.lo.w), "=r"(v.hi.x), "=r"(v.hi.y), "=r"(v.hi.z), "=r"(v.hi.w)
-               : "l"(p));
-  return v;
-}
 __device__ __forceinline__ uint4 lds128u(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
 
-// (w1 v1 + w2 v2 + w3 v3 + w4 v4) of 8 fp16 channels, fp32 math (packed FFMA2), rounded once to fp16.
+// (w1 v1 + w2 v2 + w3 v3 + w4 v4) of 8 fp16 channels, fp32 math, rounded once to fp16.
 __device__ __forceinline__ uint4 blend8(const uint4& v1, const uint4& v2, const uint4& v3, const uint4& v4, float w1, float w2,
                                         float w3, float w4) {
   const __half2* h1 = reinterpret_cast<const __half2*>(&v1);
@@ -96,41 +80,26 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + DC_STAGES * DC_A_BYTES;
-  uint8_t* stg = smem_b + DC_STAGES * DC_B_BYTES;
-  uint8_t* coords = stg + 2 * DC_STG_BYTES;
+  uint8_t* coords = smem_b + DC_STAGES * DC_B_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(coords + DC_COORD_BYTES);
   uint64_t* a_full = bars;                       // [S] one arrival per gather warp
   uint64_t* b_full = bars + DC_STAGES;           // [S] TMA bytes of the weight tile
-  uint64_t* empty = bars + 2 * DC_STAGES;        // [S] tcgen05.commit: the stage's MMAs have read it
-  uint64_t* tmem_full = bars + 3 * DC_STAGES;    // [2]
-  uint64_t* tmem_empty = tmem_full + 2;          // [2] one arrival per epilogue warp
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* empty = bars + 2 * DC_STAGES;        // [S] every MMA thread: the stage's wgmma group has read it
   float* s_bias = reinterpret_cast<float*>(bars + 32);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_tiles = p.tile_begin[p.njobs];
 
   if (threadIdx.x == 0) {
-    for (int j = 0; j < p.njobs; ++j) {
-      tma_prefetch_desc(&p.map_w[j]);
-      tma_prefetch_desc(&p.map_y[j]);
-    }
+    for (int j = 0; j < p.njobs; ++j) tma_prefetch_desc(&p.map_w[j]);
     for (int s = 0; s < DC_STAGES; ++s) {
       mbar_init(&a_full[s], DC_GATHER_WARPS);
       mbar_init(&b_full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], 4);
+      mbar_init(&empty[s], 128);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 2 * DC_BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto job_of = [&](int tile) {
     int j = 0;
@@ -152,116 +121,66 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
         }
       }
     }
-  } else if (warp == 1) {
-    // ---- MMA issue ----------------------------------------------------------------------------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(DC_BM, DC_BN, 0);
-      uint32_t it = 0;
-      int lt = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-        const int buf = lt & 1;
-        mbar_wait(&tmem_empty[buf], ((lt >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(buf * DC_BN);
-        for (int kb = 0; kb < DC_KB; ++kb, ++it) {
-          const int s = it % DC_STAGES;
-          const uint32_t ph = (it / DC_STAGES) & 1;
-          mbar_wait(&b_full[s], ph);
-          mbar_wait(&a_full[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + s * DC_A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + s * DC_B_BYTES);
-#pragma unroll
-          for (int k = 0; k < DC_BK / 16; ++k)
-            tc_mma_f16(acc, umma_desc_k_sw128(a_addr + k * 32), umma_desc_k_sw128(b_addr + k * 32), idesc,
-                       (kb | k) != 0 ? 1u : 0u);
-          tc_commit(&empty[s]);
-        }
-        tc_commit(&tmem_full[buf]);
-      }
-    }
   } else if (warp >= 4 && warp < 8) {
-    // ---- epilogue: TMEM -> (+bias) -> fp16 -> swizzled staging window -> TMA store -------------------------------------
-    const int ew = warp - 4, tid_e = threadIdx.x - 128;
-    const bool issuer = tid_e == 0;
-    const int r_local = ew * 32 + lane, sw = r_local & 7;
-    int lt = 0, wcount = 0, cur_job = -1;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+    // ---- MMA + epilogue: registers -> (+bias) -> fp16 -> global ---------------------------------------------------------
+    const int tid = threadIdx.x - 128;
+    uint32_t it = 0;
+    int cur_job = -1;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int j = job_of(tile);
-      if (j != cur_job) {  // uniform over the 128 epilogue threads
+      if (j != cur_job) {  // uniform over the 128 MMA threads
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        s_bias[tid_e] = p.bias[j] ? p.bias[j][tid_e] : 0.f;
-        s_bias[tid_e + 128] = p.bias[j] ? p.bias[j][tid_e + 128] : 0.f;
+        s_bias[tid] = p.bias[j] ? p.bias[j][tid] : 0.f;
+        s_bias[tid + 128] = p.bias[j] ? p.bias[j][tid + 128] : 0.f;
         cur_job = j;
         asm volatile("bar.sync 1, 128;" ::: "memory");
       }
-      const int buf = lt & 1;
-      const int row0 = (tile - p.tile_begin[j]) * DC_BM;
-      mbar_wait(&tmem_full[buf], (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (uint32_t)(buf * DC_BN) + ((uint32_t)(ew * 32) << 16);
-#pragma unroll 1
-      for (int w = 0; w < 4; ++w, ++wcount) {
-        uint8_t* const st_win = stg + (wcount & 1) * DC_STG_BYTES;
-        const uint32_t st_row = smem_u32(st_win) + r_local * 128;
-        uint32_t ra[16], rb[16];
-        tmem_ld_32x16(t_row + (uint32_t)(w * 64), ra);
-        // the store that read this window two windows ago has been awaited by the issuer (wait_read1 below)
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        auto emit = [&](uint32_t (&r)[16], int c0) {  // c0: column inside the window (0, 16, 32, 48)
-          const uint32_t baddr = smem_u32(s_bias) + (uint32_t)((w * 64 + c0) * 4);
-          uint32_t h[8];
+      float acc[128];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float4 bv = lds128f(baddr + k * 16);
-            h[2 * k] = pack_half2(__uint_as_float(r[4 * k]) + bv.x, __uint_as_float(r[4 * k + 1]) + bv.y);
-            h[2 * k + 1] = pack_half2(__uint_as_float(r[4 * k + 2]) + bv.z, __uint_as_float(r[4 * k + 3]) + bv.w);
-          }
-          const int j0 = c0 >> 3;
-          sts128(st_row + (((j0) ^ sw) << 4), h[0], h[1], h[2], h[3]);
-          sts128(st_row + (((j0 + 1) ^ sw) << 4), h[4], h[5], h[6], h[7]);
-        };
-        tmem_ld_wait_dep(ra);
-        tmem_ld_32x16(t_row + (uint32_t)(w * 64 + 16), rb);
-        emit(ra, 0);
-        tmem_ld_wait_dep(rb);
-        tmem_ld_32x16(t_row + (uint32_t)(w * 64 + 32), ra);
-        emit(rb, 16);
-        tmem_ld_wait_dep(ra);
-        tmem_ld_32x16(t_row + (uint32_t)(w * 64 + 48), rb);
-        emit(ra, 32);
-        tmem_ld_wait_dep(rb);
-        emit(rb, 48);
-        tc_fence_before();
-        if (w == 3) {  // the accumulator may be overwritten by the tile after next
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-        }
-        fence_proxy_async();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (issuer) {
-          tma_store_4d(&p.map_y[j], st_win, w * 64, row0, 0, 0);
-          tma_store_commit_and_wait_read1();  // the OTHER window's store has been read -> it may be rewritten next
-        }
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < DC_KB; ++kb, ++it) {
+        const int s = it % DC_STAGES;
+        const uint32_t ph = (it / DC_STAGES) & 1;
+        mbar_wait(&b_full[s], ph);
+        mbar_wait(&a_full[s], ph);
+        const uint32_t a_addr = smem_u32(smem_a + s * DC_A_BYTES);
+        const uint32_t b_addr = smem_u32(smem_b + s * DC_B_BYTES);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < DC_BK / 16; ++k)
+          wgmma_ss_m64n256_kk(acc, wg_desc_k_sw128(a_addr + k * 32), wg_desc_k_sw128(b_addr + k * 32), 1);
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_fence_acc(acc);
+        if (kb > 0) mbar_arrive(&empty[(it - 1) % DC_STAGES]);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      mbar_arrive(&empty[(it - 1) % DC_STAGES]);
+      const long row0 = (long)(tile - p.tile_begin[j]) * DC_BM;
+      __half* const y = p.y[j];
+#pragma unroll
+      for (int i = 0; i < 128; i += 2) {
+        const long row = row0 + wg_row(tid, i);
+        const int col = wg_col(tid, i);
+        if (row < p.rows[j])
+          *reinterpret_cast<__half2*>(y + row * DC_BN + col) = __floats2half2_rn(acc[i] + s_bias[col], acc[i + 1] + s_bias[col + 1]);
       }
     }
-    if (issuer) tma_store_wait_read_all();
   } else if (warp >= 8) {
-    // ---- gather: 4 threads per output pixel, 2 x 8 channels each per k-block -------------------------------------------
-    const int pt = threadIdx.x - 256, rl = pt >> 2, q = pt & 3;
+    // ---- gather: 2 threads per output pixel, 4 x 8 channels each per k-block -------------------------------------------
+    const int pt = threadIdx.x - 256, rl = pt >> 1, q = pt & 1;
     const int sw = rl & 7;
-    // thread q of a row owns the adjacent 16-byte chunks 2q, 2q+1; rows r and r+1 differ in swizzle bit 0, so the eight
-    // threads of a quarter-warp (two rows) store to eight distinct bank groups
-    const int jA = 2 * q, jB = 2 * q + 1;
+    // thread q of a row owns the adjacent 16-byte chunks 4q .. 4q+3 of the 128-byte swizzled row
     const uint32_t a_row = smem_u32(smem_a) + rl * 128;
-    const uint32_t offA = (uint32_t)((jA ^ sw) << 4), offB = (uint32_t)((jB ^ sw) << 4);
     const uint32_t my_coords = smem_u32(coords) + rl * 32;
     const LevelTable& L = p.lt;
-    const __half* const xa = p.x + q * 16;
+    const __half* const xa = p.x + q * 32;
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int j = job_of(tile);
-      // -- sampling records of the tile: thread pt works out (row pt % 128, taps pt / 128 + 4 i): four corner offsets
+      // -- sampling records of the tile: thread pt works out (row pt % 64, taps pt / 64 + 2 i): four corner offsets
       //    (elements from x) and four corner weights with the modulation mask folded in
       {
         const int branch = p.branch[j];
@@ -293,7 +212,7 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
         const int HWl = L.H[lo] * L.W[lo], HWo = Ho * Wo, pix = ho * Wo + wo;
         const float* omb = p.om ? p.om + ((long)b * p.N + L.off[lo]) * p.om_ld : nullptr;
         const int xrow0 = b * p.N + L.off[li];
-        for (int tap = pt >> 7; tap < DC_TAPS; tap += DC_GATHER_WARPS * 32 / DC_BM) {
+        for (int tap = pt / DC_BM; tap < DC_TAPS; tap += DC_GATHER_THREADS / DC_BM) {
           float off_h = 0.f, off_w = 0.f, m = 1.f;
           if (omb && valid) {
             // flat NCHW index c*HWo + pix re-read through the strides of the level the record was produced at
@@ -323,12 +242,20 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
           sts128(rec + 16, __float_as_uint(w1), __float_as_uint(w2), __float_as_uint(w3), __float_as_uint(w4));
         }
       }
-      asm volatile("bar.sync 2, 512;" ::: "memory");
+      asm volatile("bar.sync 2, %0;" ::"n"(DC_GATHER_THREADS) : "memory");
       // -- 36 k-blocks (tap = kb / 4, channels (kb % 4) * 64 ..): the corner rows of k-block kb+1 are in flight while
-      //    k-block kb is blended and stored
+      //    k-block kb is stored
       uint4 o = lds128u(my_coords);
       float4 w = lds128f(my_coords + 16);
-      U8 c1 = ldg256(xa + o.x), c2 = ldg256(xa + o.y), c3 = ldg256(xa + o.z), c4 = ldg256(xa + o.w);
+      uint4 c[4][4];
+      auto load = [&](int ch) {
+        const uint32_t off[4] = {o.x, o.y, o.z, o.w};
+#pragma unroll
+        for (int cr = 0; cr < 4; ++cr)
+#pragma unroll
+          for (int h = 0; h < 4; ++h) c[cr][h] = __ldg(reinterpret_cast<const uint4*>(xa + off[cr] + ch) + h);
+      };
+      load(0);
 #pragma unroll 1
       for (int kb = 0; kb < DC_KB; ++kb, ++it) {
         const int s = it % DC_STAGES;
@@ -339,27 +266,20 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
           o = lds128u(rec);
           w = lds128f(rec + 16);
         }
-        const int ch = (nk & 3) * DC_BK;
-        const uint4 oa = blend8(c1.lo, c2.lo, c3.lo, c4.lo, wc.x, wc.y, wc.z, wc.w);
-        const uint4 ob = blend8(c1.hi, c2.hi, c3.hi, c4.hi, wc.x, wc.y, wc.z, wc.w);
-        if (nk < DC_KB) {
-          c1 = ldg256(xa + o.x + ch); c2 = ldg256(xa + o.y + ch); c3 = ldg256(xa + o.z + ch); c4 = ldg256(xa + o.w + ch);
-        }
+        uint4 ob[4];
+#pragma unroll
+        for (int h = 0; h < 4; ++h) ob[h] = blend8(c[0][h], c[1][h], c[2][h], c[3][h], wc.x, wc.y, wc.z, wc.w);
+        if (nk < DC_KB) load((nk & 3) * DC_BK);
         mbar_wait(&empty[s], ((it / DC_STAGES) & 1) ^ 1);
         const uint32_t dst = a_row + s * DC_A_BYTES;
-        sts128(dst + offA, oa.x, oa.y, oa.z, oa.w);
-        sts128(dst + offB, ob.x, ob.y, ob.z, ob.w);
+#pragma unroll
+        for (int h = 0; h < 4; ++h) sts128(dst + (uint32_t)(((4 * q + h) ^ sw) << 4), ob[h].x, ob[h].y, ob[h].z, ob[h].w);
         fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_full[s]);
       }
-      asm volatile("bar.sync 2, 512;" ::: "memory");  // every record of this tile has been read
+      asm volatile("bar.sync 2, %0;" ::"n"(DC_GATHER_THREADS) : "memory");  // every record of this tile has been read
     }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * DC_BN);
   }
 }
 
@@ -374,7 +294,7 @@ extern "C" int mqdet_dcn_conv(const void* x, const float* om, int64_t om_ld, con
   MQ_REQUIRE(C == DC_C, "dcn_conv: C must be 256 (got %ld)", (long)C);
   MQ_REQUIRE(njobs >= 1 && njobs <= MQDET_DCN_MAX_JOBS, "dcn_conv: 1..%d jobs (got %ld)", MQDET_DCN_MAX_JOBS, (long)njobs);
   MQ_REQUIRE(B >= 1, "dcn_conv: empty batch");
-  MQ_REQUIRE(((uintptr_t)x & 31) == 0, "dcn_conv: x must be 32-byte aligned (256-bit loads)");
+  MQ_REQUIRE(((uintptr_t)x & 15) == 0, "dcn_conv: x must be 16-byte aligned (128-bit loads)");
   MQ_REQUIRE(om == nullptr || om_ld >= 27, "dcn_conv: om_ld must hold the 27 offset/mask channels");
   MQ_REQUIRE(nlev >= 1 && nlev <= MQDET_MAX_LEVELS, "dcn_conv: 1..%d levels", MQDET_MAX_LEVELS);
   DcnP q;
@@ -402,8 +322,7 @@ extern "C" int mqdet_dcn_conv(const void* x, const float* om, int64_t om_ld, con
     int bc1, bc2;
     int rc = make_operand_map(&q.map_w[j], weight[j], DC_BN, DC_TAPS * DC_C, DC_TAPS * DC_C, 1, 0, 1, 0, DC_BN, &bc1, &bc2);
     if (rc != MQDET_OK) return rc;
-    rc = make_store_map(&q.map_y[j], y[j], MQDET_F16, q.rows[j], DC_BN, DC_BN, 1, 0, 1, 0);
-    if (rc != MQDET_OK) return rc;
+    q.y[j] = (__half*)y[j];
   }
   q.tile_begin[njobs] = tiles;
   int rc = ensure_dyn_smem((const void*)dcn_conv_kernel, DC_SMEM_BYTES);

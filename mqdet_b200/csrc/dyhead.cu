@@ -6,7 +6,7 @@
 //
 // Layout: all FPN levels of an image live in one fp16 tensor x[B][N][C] (N = sum_l H_l*W_l, level l at row offset
 // off_l, row-major (h, w)); every kernel below walks ALL levels in one launch through a LevelTable.
-// The DCNv2 sampling stage writes an fp16 column matrix [rows][9*C] (k = tap*C + c) that feeds the tcgen05 GEMM.
+// The DCNv2 sampling stage writes an fp16 column matrix [rows][9*C] (k = tap*C + c) that feeds the wgmma GEMM.
 #include "common.cuh"
 #include "../../include/mqdet_b200.h"
 

@@ -203,7 +203,7 @@ extern "C" int mqdet_shift_clamp_f32(float* x, int64_t n, const float* shift, fl
   MQ_REQUIRE(x && shift && n > 0, "shift_clamp: null pointer / empty");
   MQ_REQUIRE(((uintptr_t)x & 15) == 0, "shift_clamp: x must be 16-byte aligned");
   const long blocks = (n / 4 + 255) / 256;
-  shift_clamp_kernel<<<(unsigned)(blocks < 1 ? 1 : (blocks > 148 * 16 ? 148 * 16 : blocks)), 256, 0, (cudaStream_t)stream>>>(x, n, shift, lo,
+  shift_clamp_kernel<<<(unsigned)(blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks)), 256, 0, (cudaStream_t)stream>>>(x, n, shift, lo,
                                                                                                                         hi);
   return check_launch("shift_clamp_kernel");
 }

@@ -252,7 +252,7 @@ extern "C" int mqdet_add_cast(const float* a, const float* b, const float* rowga
              "add_cast: pointers must be 16-byte aligned");
   const long n4 = rows * D / 4;
   long blocks = (n4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   add_cast_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const float4*)a, (const float4*)b, rowgate, n4, (int)(D / 4),
                                                                       (uint2*)out16, (float4*)out32);
   return check_launch("add_cast_kernel");

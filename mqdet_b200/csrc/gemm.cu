@@ -1,19 +1,18 @@
-// mqdet_b200 — fp16 x fp16 -> fp32-accumulate GEMM with fused epilogue, hand-written for sm_100a.
+// mqdet_b200 — fp16 x fp16 -> fp32-accumulate GEMM with fused epilogue, hand-written for sm_90a.
 //
 //   D[z][m,n] = epi( sum_k A[z][m,k] * B[z][n,k] )      (both operands K-contiguous: "TN")
 //
-// Product kernel (gemm_tc_kernel): warp-specialised, one 128 x BLOCK_N output tile per CTA.
-//   warp 0   : TMA producer  — cp.async.bulk.tensor (4-D maps, 128B swizzle) into a STAGES-deep ring
-//   warp 1   : MMA issuer    — one lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128,N=BLOCK_N,K=16),
-//                              tcgen05.commit releases ring slots / signals the epilogue
-//   warp 2   : TMEM allocator (BLOCK_N fp32 columns)
-//   warps 4-7: epilogue      — tcgen05.ld (lane == output row) -> bias/act/gate/residual -> 16B stores
-// Two CTAs fit per SM (<=~100 KB smem, <=256 TMEM columns each) so one CTA's epilogue overlaps the
-// other's main loop; the grid runs n-tiles fastest so the A row-panel is shared through L2.
+// Product kernel (gemm_wg_kernel): warp-specialised, one 128 x BN output tile per CTA (BN = 64 or 128).
+//   warpgroup 0    : TMA producer — one thread issues cp.async.bulk.tensor (4-D maps, 128B swizzle) into a STAGES-deep ring
+//   warpgroups 1-2 : consumers    — rows 0-63 / 64-127 of the tile: wgmma.m64nBNk16 from the swizzled ring (fp32
+//                                   accumulators in registers, one commit group per k-block, the previous k-block's slot
+//                                   released as soon as its group retires), then the epilogue straight from the fragments
+// The grid runs n-tiles fastest so the A row-panel is shared through L2.
 //
 // Validation kernel (gemm_simt_kernel): plain 64x64 shared-memory tiled FMA kernel with the same
 // epilogue, used by the tests to cross-check the tensor-core path (never by the product path).
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/mqdet_b200.h"
 
 namespace mqdet {
@@ -40,13 +39,10 @@ struct GemmP {
   int r_dtype;
   long ldr, r_b1, r_b2;
   int a_bcast1, a_bcast2, b_bcast1, b_bcast2;  // 1 -> TMA coordinate pinned to 0
-  int use_tma_store;
-  // epilogue variant (host decides from alignment / residual)
-  int fast_epi;                                // persistent kernel: the compact epilogue applies (fast_epilogue_ok)
-  int debug;                                   // MQDET_GEMM_DEBUG experiments: 1 = no epilogue, 2 = no TMA store, 4 = no A loads
+  int vec2;                                    // output pairs (col, col + 1) may be written with one aligned store
 };
 
-// One output element's epilogue, split so the tensor-core kernel can apply the residual in its coalesced phase:
+// One output element's epilogue:
 //   epi_pre : alpha / bias / activation / clamp / gate      epi_one = epi_pre + residual
 __device__ __forceinline__ float epi_pre(const GemmP& p, float acc, long row, long col, int z1, int z2,
                                          float gate_scalar) {
@@ -94,439 +90,41 @@ __device__ __forceinline__ void store_one(const GemmP& p, float v, long row, lon
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 kernel
+// wgmma kernel
 // ---------------------------------------------------------------------------------------------
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 fp16 = 128 B = one swizzle row
 
-// ---- epilogue of one 128 x BN tile (4 warps; thread == output row == TMEM lane) -------------------------------------
-// 16 accumulator columns at a time: tcgen05.ld -> alpha/bias/act/clamp/gate in registers -> staging tile `stg`.
-//   TMA-store variant (no residual, aligned C): values are converted to the output type and written in the
-//     128B-swizzled box layout (chunk ^ (row & 7): conflict-free), then ONE thread issues cp.async.bulk.tensor
-//     stores; the TMA unit clips the M/N edges.  ~350 instructions per thread for a 128x128 tile.
-//   fallback variant: fp32 staging rows padded by 16 B, then a coalesced row loop adds the residual and stores.
-// tmem_empty_bar != nullptr (persistent kernel): arrive on it as soon as the accumulator has been read, and end with a
-// barrier of the 4 epilogue warps so the staging tile can be rewritten for the next tile.
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const GemmP& p, const CUtensorMap* tma_c, uint32_t tmem_acc, uint8_t* stg,
-                                              int m_tile, int n_tile, int z1, int z2, int ew, int lane,
-                                              uint64_t* tmem_empty_bar, int pend = 0, int half = 0, int nhalf = 1,
-                                              int cw0 = 0, int cw = BN, bool release = true) {
-  // nhalf == 2: eight epilogue warps, two per TMEM lane quarter, each taking one half of the window's columns
-  // [cw0, cw0 + cw): the column window of the tile handled by this call (TMA-store variant only; default = whole tile);
-  //   `stg` holds just that window, and the accumulator is released (`release`) by the call that reads its last window
-  // ---- epilogue (4 warps; thread == output row == TMEM lane) -------------------------------------------------
-  // The operand ring is idle once tmem_full fires, so it doubles as the staging tile.  16 accumulator columns at
-  // a time: tcgen05.ld -> alpha/bias/act/clamp/gate in registers -> staging.
-  //   TMA-store variant (no residual, aligned C): values are converted to the output type and written in the
-  //     128B-swizzled box layout (chunk ^ (row & 7): conflict-free), then ONE thread issues cp.async.bulk.tensor
-  //     stores; the TMA unit clips the M/N edges.  ~350 instructions per thread for a 128x128 tile.
-  //   fallback variant: fp32 staging rows padded by 16 B, then a coalesced row loop adds the residual and stores.
-  const int r_local = ew * 32 + lane;
-  const long row = (long)m_tile * BM + r_local;
-  float gate_s = 1.f;
-  if (p.gate_mode == MQDET_VEC_SCALAR) gate_s = p.gate_tanh ? tanhf(p.gate[0]) : p.gate[0];
-  if (p.gate_mode == MQDET_VEC_PER_ROW && row < p.M) gate_s = p.gate_tanh ? tanhf(p.gate[row]) : p.gate[row];
-  float brow = 0.f;
-  if (p.bias_mode == MQDET_VEC_PER_ROW && row < p.M) brow = p.bias[z1 * p.bias_b1 + z2 * p.bias_b2 + row];
-  const float* bias_col = (p.bias_mode == MQDET_VEC_PER_COL) ? p.bias + z1 * p.bias_b1 + z2 * p.bias_b2 : nullptr;
-  const float* gate_col = (p.gate_mode == MQDET_VEC_PER_COL) ? p.gate : nullptr;
-  // parameter block -> registers once (the compiler otherwise re-reads the constant bank inside the unrolled loops)
-  const float alpha = p.alpha, clampv = p.clamp;
-  const int act = p.act;
-  const bool sab = p.scale_after_bias != 0, gate_tanh = p.gate_tanh != 0;
-  const bool has_gate_s = (p.gate_mode == MQDET_VEC_SCALAR) || (p.gate_mode == MQDET_VEC_PER_ROW);
-  const float brow_eff = sab ? alpha * brow : brow;  // alpha*(acc + b) == fma(alpha, acc, alpha*b)
-  constexpr int LDS = BN + 4;  // fallback staging row stride (floats)
-  float* stage32 = reinterpret_cast<float*>(stg);
-  const int nthr_epi = 128 * nhalf;
-  const bool issuer = (ew == 0 && half == 0 && lane == 0);
-  const uint32_t t_row = tmem_acc + ((uint32_t)(ew * 32) << 16);
-  const int c_begin = cw0 + half * (cw / nhalf), c_end = cw0 + (half + 1) * (cw / nhalf);
-  // Software pipeline over 16-column chunks: the tcgen05.ld of chunk i+1 is in flight while chunk i is converted.
-  uint32_t r[16];
-  tmem_ld_32x16(t_row + (uint32_t)c_begin, r);
-  if (p.use_tma_store && tmem_empty_bar && !pend) {
-    // persistent kernel, ONE staging tile: the previous tile's TMA store must have read it before it is rewritten
-    if (issuer) tma_store_wait_read_all();
-    asm volatile("bar.sync 1, %0;" ::"r"(nthr_epi) : "memory");
-  }
-#pragma unroll 1
-  for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-    tmem_ld_wait_dep(r);
-    float acc[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) acc[i] = __uint_as_float(r[i]);
-    if (c0 + 16 < c_end) tmem_ld_32x16(t_row + (uint32_t)(c0 + 16), r);
-    const long col0 = (long)n_tile * BN + c0;
-    // Every mode test below is warp-uniform and hoisted around a whole straight-line 16-element loop: the epilogue
-    // is issue-bound (4 warps per tile), so per-element predicates/parameter reloads are what must be avoided.
-    float v[16];
-    const bool inb = col0 + 16 <= p.N;
-    if (bias_col) {
-      float b[16];
-      if (inb && ((reinterpret_cast<uintptr_t>(bias_col + col0) & 15) == 0)) {
-        const float4* b4 = reinterpret_cast<const float4*>(bias_col + col0);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 t = b4[q];
-          b[4 * q] = t.x; b[4 * q + 1] = t.y; b[4 * q + 2] = t.z; b[4 * q + 3] = t.w;
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) b[i] = (col0 + i < p.N) ? bias_col[col0 + i] : 0.f;
-      }
-      if (sab) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = alpha * (acc[i] + b[i]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = fmaf(alpha, acc[i], b[i]);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = fmaf(alpha, acc[i], brow_eff);
-    }
-    if (act == MQDET_ACT_GELU) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = gelu_erf(v[i]);
-    } else if (act == MQDET_ACT_RELU) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
-    }
-    if (clampv > 0.f) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = fminf(fmaxf(v[i], -clampv), clampv);
-    }
-    if (gate_col) {
-      if (inb) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] *= gate_tanh ? tanhf(gate_col[col0 + i]) : gate_col[col0 + i];
-      } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          if (col0 + i < p.N) v[i] *= gate_tanh ? tanhf(gate_col[col0 + i]) : gate_col[col0 + i];
-      }
-    } else if (has_gate_s) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] *= gate_s;
-    }
-    if (p.use_tma_store) {
-      if (p.c_dtype == MQDET_F16) {
-        // column block of 64 halfs (128 B rows); this thread's 16 columns = chunks j0, j0+1
-        uint8_t* blk = stg + ((c0 - cw0) >> 6) * (BM * 128) + r_local * 128;
-        const int j0 = (c0 & 63) >> 3;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          __half2 h0 = __floats2half2_rn(v[8 * h + 0], v[8 * h + 1]);
-          __half2 h1 = __floats2half2_rn(v[8 * h + 2], v[8 * h + 3]);
-          __half2 h2 = __floats2half2_rn(v[8 * h + 4], v[8 * h + 5]);
-          __half2 h3 = __floats2half2_rn(v[8 * h + 6], v[8 * h + 7]);
-          uint4 u;
-          u.x = *reinterpret_cast<uint32_t*>(&h0);
-          u.y = *reinterpret_cast<uint32_t*>(&h1);
-          u.z = *reinterpret_cast<uint32_t*>(&h2);
-          u.w = *reinterpret_cast<uint32_t*>(&h3);
-          *reinterpret_cast<uint4*>(blk + (((j0 + h) ^ (r_local & 7)) << 4)) = u;
-        }
-      } else {
-        // column block of 32 floats (128 B rows); 16 columns = chunks j0 .. j0+3
-        uint8_t* blk = stg + ((c0 - cw0) >> 5) * (BM * 128) + r_local * 128;
-        const int j0 = (c0 & 31) >> 2;
-#pragma unroll
-        for (int h = 0; h < 4; ++h)
-          *reinterpret_cast<float4*>(blk + (((j0 + h) ^ (r_local & 7)) << 4)) =
-              make_float4(v[4 * h], v[4 * h + 1], v[4 * h + 2], v[4 * h + 3]);
-      }
-    } else {
-      float4* dst = reinterpret_cast<float4*>(stage32 + r_local * LDS + c0);
-#pragma unroll
-      for (int h = 0; h < 4; ++h) dst[h] = make_float4(v[4 * h], v[4 * h + 1], v[4 * h + 2], v[4 * h + 3]);
-    }
-  }
-  tc_fence_before();
-  if (tmem_empty_bar && release) {  // persistent kernel: the accumulator buffer may be overwritten by the next tile's MMAs
-    __syncwarp();
-    if (lane == 0) mbar_arrive(tmem_empty_bar);
-  }
-  if (p.use_tma_store) {
-    fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
-    // two staging tiles (pend): the store issued one tile ago used the OTHER tile, which the next epilogue rewrites
-    // right after this barrier -> it must have been read by now (it had a whole tile time; this wait is ~free)
-    if (pend && issuer) tma_store_wait_read_all();
-    asm volatile("bar.sync 1, %0;" ::"r"(nthr_epi) : "memory");
-    if (issuer) {
-      const int cz1 = p.nb1 == 1 ? 0 : z1, cz2 = p.nb2 == 1 ? 0 : z2;
-      const int cpb = (p.c_dtype == MQDET_F16) ? 64 : 32;  // columns per 128-byte block
-      for (int cb = 0; cb * cpb < cw; ++cb) {
-        const long cc = (long)n_tile * BN + cw0 + cb * cpb;
-        if (cc < p.N && !(p.debug & 2)) tma_store_4d(tma_c, stg + cb * (BM * 128), (int)cc, m_tile * BM, cz1, cz2);
-      }
-      // one-shot kernel: the CTA exits next, shared memory must outlive the read.  Persistent kernel: the read is
-      // awaited where the staging tile is reused (above) and once more before the kernel ends.
-      if (tmem_empty_bar) tma_store_commit(); else tma_store_commit_and_wait_read();
-    }
-  } else {
-    asm volatile("bar.sync 1, %0;" ::"r"(nthr_epi) : "memory");
-    constexpr int LPR = BN / 8;    // lanes per row (8 columns each)
-    constexpr int RPW = 32 / LPR;  // rows per warp per iteration
-    const int lc = (lane % LPR) * 8;
-    const long col = (long)n_tile * BN + lc;
-    if (col < p.N) {
-      const bool full = col + 8 <= p.N;
-      const bool c_vec = full && ((p.ldc & 7) == 0) && ((p.c_b1 & 7) == 0) && ((p.c_b2 & 7) == 0) &&
-                         ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-      const bool r_vec = full && p.R && ((p.ldr & 7) == 0) && ((p.r_b1 & 7) == 0) && ((p.r_b2 & 7) == 0) &&
-                         ((reinterpret_cast<uintptr_t>(p.R) & 15) == 0);
-      const long c_base = z1 * p.c_b1 + z2 * p.c_b2 + col;
-      const long r_base = z1 * p.r_b1 + z2 * p.r_b2 + col;
-#pragma unroll 1
-      for (int rl = (ew + 4 * half) * RPW + lane / LPR; rl < BM; rl += 4 * nhalf * RPW) {
-        const long grow = (long)m_tile * BM + rl;
-        if (grow >= p.M) break;
-        const float4 s0 = *reinterpret_cast<const float4*>(stage32 + rl * LDS + lc);
-        const float4 s1 = *reinterpret_cast<const float4*>(stage32 + rl * LDS + lc + 4);
-        float v[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-        if (p.R) {
-          if (r_vec) {
-            if (p.r_dtype == MQDET_F32) {
-              const float* rp = reinterpret_cast<const float*>(p.R) + r_base + grow * p.ldr;
-              const float4 a = *reinterpret_cast<const float4*>(rp);
-              const float4 b = *reinterpret_cast<const float4*>(rp + 4);
-              v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w;
-              v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
-            } else {
-              const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(p.R) + r_base + grow * p.ldr);
-              const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float2 f = __half22float2(h[i]);
-                v[2 * i] += f.x;
-                v[2 * i + 1] += f.y;
-              }
-            }
-          } else {
-#pragma unroll 1
-            for (int i = 0; i < 8; ++i)
-              if (col + i < p.N) v[i] += ld_residual(p, grow, col + i, z1, z2);
-          }
-        }
-        if (c_vec) {
-          if (p.c_dtype == MQDET_F32) {
-            float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.C) + c_base + grow * p.ldc);
-            dst[0] = make_float4(v[0], v[1], v[2], v[3]);
-            dst[1] = make_float4(v[4], v[5], v[6], v[7]);
-          } else {
-            __half2 h0 = __floats2half2_rn(v[0], v[1]);
-            __half2 h1 = __floats2half2_rn(v[2], v[3]);
-            __half2 h2 = __floats2half2_rn(v[4], v[5]);
-            __half2 h3 = __floats2half2_rn(v[6], v[7]);
-            uint4 u;
-            u.x = *reinterpret_cast<uint32_t*>(&h0);
-            u.y = *reinterpret_cast<uint32_t*>(&h1);
-            u.z = *reinterpret_cast<uint32_t*>(&h2);
-            u.w = *reinterpret_cast<uint32_t*>(&h3);
-            *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.C) + c_base + grow * p.ldc) = u;
-          }
-        } else {
-#pragma unroll 1
-          for (int i = 0; i < 8; ++i)
-            if (col + i < p.N) store_one(p, v[i], grow, col + i, z1, z2);
-        }
-      }
-    }
-  }
-  if (tmem_empty_bar && !p.use_tma_store) asm volatile("bar.sync 1, %0;" ::"r"(nthr_epi) : "memory");
-}
-
-// ---- fast epilogue of the persistent kernel ---------------------------------------------------------------------------
-// v = act(acc * S + T) (+ residual), optional clamp, fp16/fp32 output through the swizzled
-// staging tile + TMA store, where the gate is folded into the scale:  S = alpha * g,  T = b * g (or alpha * b * g).
-// S/T are either uniform per thread (no per-column vector) or read from two shared-memory rows filled once per tile/item.
-// Kept apart from the generic epilogue so that its loop is ~2 instructions per element (packed FFMA2, F2FP pairs, 128-bit
-// shared accesses) and contiguous in the instruction cache: with K <= 256 a 128x256 tile has only ~2000 tensor-pipe
-// cycles to hide 32768 outputs.  Two register sets ping-pong so that the tcgen05.ld (and the residual loads) of the next
-// 16 columns are in flight while this one is converted.
-struct FastEpi {
-  const float* s_vec;  // shared: per-column scale (nullptr -> uniform s_u / t_u)
-  const float* t_vec;  // shared: per-column addend
-  float s_u, t_u;
-  const void* res;     // residual row of this thread (already offset to row / batch), nullptr -> none
-  int res_f16;
-};
-
-template <int BN, bool PLAIN>  // PLAIN: fp16 output, no activation, no residual (the hot products) -> compact straight code
-__device__ __forceinline__ void epilogue_fast(const GemmP& p, const CUtensorMap* tma_c, uint32_t tmem_acc, uint8_t* stg,
-                                              const FastEpi& fe, int m_tile, int n_tile, int z1, int z2, int ew, int lane,
-                                              uint64_t* tmem_empty_bar, bool dbl, int half, int cw0, int cw, bool release) {
-  const int r_local = ew * 32 + lane;
-  const bool issuer = (ew == 0 && half == 0 && lane == 0);
-  const uint32_t t_row = tmem_acc + ((uint32_t)(ew * 32) << 16);
-  const int c_begin = cw0 + half * (cw >> 1);  // (cw / 2) % 32 == 0
-  // columns at or beyond N (partial last n tile) are clipped by the TMA store: do not convert them (32-column steps)
-  const long n_left = p.N - (long)n_tile * BN;
-  const int c_lim = (int)(n_left < (long)BN ? ((n_left + 31) & ~31L) : (long)BN);
-  const int c_end = min(c_begin + (cw >> 1), c_lim);
-  const float clampv = p.clamp;
-  const int act = PLAIN ? MQDET_ACT_NONE : p.act;
-  const bool f16 = PLAIN || p.c_dtype == MQDET_F16;
-  const int sw = r_local & 7;
-  const uint32_t stg_row = smem_u32(stg) + r_local * 128;
-  const bool vec = fe.s_vec != nullptr;
-  const uint32_t s_addr = vec ? smem_u32(fe.s_vec) : 0u, t_addr = vec ? smem_u32(fe.t_vec) : 0u;
-  const float s_u = fe.s_u, t_u = fe.t_u;
-  const bool has_res = !PLAIN && fe.res != nullptr, res16 = fe.res_f16 != 0;
-  const long ncol0 = (long)n_tile * BN;
-  uint32_t ra[16], rb[16];
-  uint4 qa[4], qb[4];
-  // residual of 16 columns: 2 (fp16) or 4 (fp32) 16-byte loads; N % (16 / elem) == 0 (TMA-store rule) so a vector is
-  // either fully inside the row or fully outside
-  auto load_res = [&](uint4 (&q)[4], int c0) {
-    const long col = ncol0 + c0;
-    if (res16) {
-      const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(fe.res) + col);
-#pragma unroll
-      for (int k = 0; k < 2; ++k) q[k] = (col + 8 * k < p.N) ? __ldg(src + k) : make_uint4(0, 0, 0, 0);
-    } else {
-      const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(fe.res) + col);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) q[k] = (col + 4 * k < p.N) ? __ldg(src + k) : make_uint4(0, 0, 0, 0);
-    }
-  };
-  if (c_begin < c_end) {
-    tmem_ld_32x16(t_row + (uint32_t)c_begin, ra);
-    if (has_res) load_res(qa, c_begin);
-  }
-  if (!dbl) {  // ONE staging tile: the previous tile's TMA store must have read it before it is rewritten
-    if (issuer) tma_store_wait_read_all();
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-  }
-  auto emit = [&](uint32_t (&r)[16], uint4 (&q)[4], int c0) {
-    float v[16];
-    if (vec) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float4 sv = lds128f(s_addr + (uint32_t)(c0 * 4 + k * 16));
-        const float4 tv = lds128f(t_addr + (uint32_t)(c0 * 4 + k * 16));
-        ffma2v(v[4 * k], v[4 * k + 1], __uint_as_float(r[4 * k]), __uint_as_float(r[4 * k + 1]), sv.x, sv.y, tv.x, tv.y);
-        ffma2v(v[4 * k + 2], v[4 * k + 3], __uint_as_float(r[4 * k + 2]), __uint_as_float(r[4 * k + 3]), sv.z, sv.w, tv.z, tv.w);
-      }
-    } else {
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        ffma2(v[2 * k], v[2 * k + 1], __uint_as_float(r[2 * k]), __uint_as_float(r[2 * k + 1]), s_u, t_u, t_u);
-    }
-    if (act == MQDET_ACT_GELU) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) gelu_fast2(v[2 * k], v[2 * k + 1]);
-    } else if (act == MQDET_ACT_RELU) {
-#pragma unroll
-      for (int k = 0; k < 16; ++k) v[k] = fmaxf(v[k], 0.f);
-    }
-    if (has_res) {
-      if (res16) {
-        const __half2* h2 = reinterpret_cast<const __half2*>(q);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float2 f = __half22float2(h2[k]);
-          v[2 * k] += f.x;
-          v[2 * k + 1] += f.y;
-        }
-      } else {
-        const float* f = reinterpret_cast<const float*>(q);
-#pragma unroll
-        for (int k = 0; k < 16; ++k) v[k] += f[k];
-      }
-    }
-    if (f16) {
-      __half2 h[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) h[k] = __floats2half2_rn(v[2 * k], v[2 * k + 1]);
-      if (clampv > 0.f) {  // clamp after rounding == rounding after clamp (rounding is monotonic)
-        const __half2 hi = __float2half2_rn(clampv), lo = __float2half2_rn(-clampv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) h[k] = __hmax2(__hmin2(h[k], hi), lo);
-      }
-      // column block of 64 halfs (128 B rows); this thread's 16 columns = 16-byte chunks j0, j0+1
-      const uint32_t blk = stg_row + ((c0 - cw0) >> 6) * (BM * 128);
-      const int j0 = (c0 & 63) >> 3;
-      const uint32_t* hv = reinterpret_cast<const uint32_t*>(h);
-      sts128(blk + (((j0) ^ sw) << 4), hv[0], hv[1], hv[2], hv[3]);
-      sts128(blk + (((j0 + 1) ^ sw) << 4), hv[4], hv[5], hv[6], hv[7]);
-    } else {
-      if (clampv > 0.f) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = fminf(fmaxf(v[i], -clampv), clampv);
-      }
-      // column block of 32 floats (128 B rows); 16 columns = chunks j0 .. j0+3
-      const uint32_t blk = stg_row + ((c0 - cw0) >> 5) * (BM * 128);
-      const int j0 = (c0 & 31) >> 2;
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        sts128(blk + (((j0 + k) ^ sw) << 4), __float_as_uint(v[4 * k]), __float_as_uint(v[4 * k + 1]), __float_as_uint(v[4 * k + 2]),
-               __float_as_uint(v[4 * k + 3]));
-    }
-  };
-#pragma unroll 1
-  for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-    tmem_ld_wait_dep(ra);
-    tmem_ld_32x16(t_row + (uint32_t)(c0 + 16), rb);
-    if (has_res) load_res(qb, c0 + 16);
-    emit(ra, qa, c0);
-    tmem_ld_wait_dep(rb);
-    if (c0 + 32 < c_end) {
-      tmem_ld_32x16(t_row + (uint32_t)(c0 + 32), ra);
-      if (has_res) load_res(qa, c0 + 32);
-    }
-    emit(rb, qb, c0 + 16);
-  }
-  tc_fence_before();
-  if (release) {  // the accumulator buffer may be overwritten by the next tile's MMAs
-    __syncwarp();
-    if (lane == 0) mbar_arrive(tmem_empty_bar);
-  }
-  fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
-  // two staging tiles: the store issued one call ago used the OTHER tile, which the next call rewrites right after this
-  // barrier -> it must have been read by now
-  if (dbl && issuer) tma_store_wait_read_all();
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  if (issuer) {
-    const int cz1 = p.nb1 == 1 ? 0 : z1, cz2 = p.nb2 == 1 ? 0 : z2;
-    const int cpb = f16 ? 64 : 32;  // columns per 128-byte block
-    for (int cb = 0; cb * cpb < cw; ++cb) {
-      const long cc = ncol0 + cw0 + cb * cpb;
-      if (cc < p.N) tma_store_4d(tma_c, stg + cb * (BM * 128), (int)cc, m_tile * BM, cz1, cz2);
-    }
-    tma_store_commit();  // the read is awaited where the staging tile is reused and once more before the kernel ends
-  }
-}
-
 template <int BN, int STAGES>
-struct TcCfg {
+struct WgCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
+  if constexpr (BN == 128)
+    wgmma_ss_m64n128_kk(acc, da, db, 1);
+  else
+    wgmma_ss_m64n64_kk(acc, da, db, 1);
+}
+
+// 128 x 64 tiles: two CTAs per SM (96 KB of shared memory each), so one CTA's epilogue overlaps the other's main loop
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(256) gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a,
-                                                      const __grid_constant__ CUtensorMap tma_b,
-                                                      const __grid_constant__ CUtensorMap tma_c, const GemmP p) {
-  using Cfg = TcCfg<BN, STAGES>;
+__global__ void __launch_bounds__(384, BN == 128 ? 1 : 2) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma_a,
+                                                                        const __grid_constant__ CUtensorMap tma_b, const GemmP p) {
+  using Cfg = WgCfg<BN, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte alignment.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full_bar = bars + 2 * STAGES;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int n_tile = blockIdx.x, m_tile = blockIdx.y;
   const int z1 = blockIdx.z % p.nb1, z2 = blockIdx.z / p.nb1;
   const int num_kb = (int)((p.K + BK - 1) / BK);
@@ -534,354 +132,71 @@ __global__ void __launch_bounds__(256) gemm_tc_kernel(const __grid_constant__ CU
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-    if (p.use_tma_store) tma_prefetch_desc(&tma_c);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 256);  // every consumer thread arrives once its wgmma group has read the slot
     }
-    mbar_init(tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (tid == 0) {
       const int az1 = p.a_bcast1 ? 0 : z1, az2 = p.a_bcast2 ? 0 : z2;
       const int bz1 = p.b_bcast1 ? 0 : z1, bz2 = p.b_bcast2 ? 0 : z2;
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
+        mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
         mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
         tma_load_4d(smem_a + s * Cfg::A_BYTES, &tma_a, &full_bar[s], kb * BK, m_tile * BM, az1, az2);
         tma_load_4d(smem_b + s * Cfg::B_BYTES, &tma_b, &full_bar[s], kb * BK, n_tile * BN, bz1, bz2);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, BN, 0);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem_a + s * Cfg::A_BYTES);
-        const uint32_t b_addr = smem_u32(smem_b + s * Cfg::B_BYTES);
+    return;
+  }
+  const int g = wg - 1;  // rows 64 g .. 64 g + 63 of the tile
+  float acc[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 16 fp16 = 32 B along K inside the 128B swizzle row
-          const uint64_t da = umma_desc_k_sw128(a_addr + k * 32);
-          const uint64_t db = umma_desc_k_sw128(b_addr + k * 32);
-          tc_mma_f16(tmem_base, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        tc_commit(&empty_bar[s]);  // slot reusable once these MMAs have read it
-      }
-      tc_commit(tmem_full_bar);  // accumulator complete
-    }
-  } else if (warp >= 4) {
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    // the operand ring is idle once tmem_full fires, so it doubles as the staging tile
-    epilogue_tile<BN>(p, &tma_c, tmem_base, smem, m_tile, n_tile, z1, z2, warp - 4, lane, nullptr);
-  }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Persistent variant: one CTA per SM walks tiles (n fastest, so neighbouring CTAs share the A panel through L2).
-//   * the TMA ring keeps streaming across tile boundaries (no pipeline drain/fill per tile),
-//   * TWO TMEM accumulators (2*BN columns): the MMA warp fills buffer i&1 while the epilogue warps drain the other,
-//   * the epilogue has its own staging tile, so TMEM->smem->TMA-store overlaps the next tile's loads and MMAs,
-//   * barrier init / TMEM allocation / descriptor prefetch are paid once per SM instead of once per tile.
-// ---------------------------------------------------------------------------------------------
-//   * BRES (K <= 256): the B tile (BN x K) stays resident in shared memory while the CTA walks a run of M tiles, so only A
-//     is streamed -> half the L2->SM traffic of the short-K products that are otherwise bound by it.
-constexpr int BRES_KB = 4;  // resident B covers K <= 4*64
-
-template <int BN, int STAGES, bool BRES>
-struct TcpCfg {
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = BRES ? A_BYTES : A_BYTES + B_BYTES;
-  static constexpr int RING_BYTES = STAGES * STAGE_BYTES + (BRES ? BRES_KB * B_BYTES : 0);
-  // fp32 padded rows (fallback epilogue) >= swizzled tiles; the 256-wide tile is only dispatched with the fp16 TMA-store
-  // epilogue (64 KB) because its fallback tile would not fit next to the ring
-  // the B-resident 256-wide tile leaves room for two 64-column windows only (128 KB B + 48 KB A ring + 32 KB)
-  static constexpr int STG_BYTES = BN == 256 ? (BRES ? 2 * BM * 64 * 2 : BM * BN * 2) : ((BM * (BN + 4) * 4 + 1023) / 1024) * 1024;
-  static constexpr int SMEM_BYTES = RING_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*epilogue scale / addend rows*/;
-};
-
-template <int BN, int STAGES, bool BRES>
-__global__ void __launch_bounds__(384, 1) gemm_tcp_kernel(const __grid_constant__ CUtensorMap tma_a,
-                                                          const __grid_constant__ CUtensorMap tma_b,
-                                                          const __grid_constant__ CUtensorMap tma_c, const GemmP p,
-                                                          int tiles_m, int tiles_n, int total_items, int mc) {
-  // Work items.  !BRES: item == tile (n fastest).  BRES: item == (z, chunk of `mc` consecutive M tiles, n tile), n fastest,
-  // so CTAs running side by side share the A panel through L2 while each keeps its own B tile resident.
-  using Cfg = TcpCfg<BN, STAGES, BRES>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;  // ring stages (!BRES) or the resident B tile (BRES)
-  uint8_t* stg = smem + Cfg::RING_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES + Cfg::STG_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full_bar = bars + 2 * STAGES;       // [2]
-  uint64_t* tmem_empty_bar = bars + 2 * STAGES + 2;  // [2]
-  uint64_t* b_full_bar = bars + 2 * STAGES + 4;
-  uint64_t* b_empty_bar = bars + 2 * STAGES + 5;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 6);
-  float* s_vec = reinterpret_cast<float*>(bars + 32);  // [BN] per-column scale and [BN] addend of the current tile
-  float* t_vec = s_vec + BN;                            // (fast epilogue)
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_kb = (int)((p.K + BK - 1) / BK);
-  // fp16 TMA-store tiles are 32 KB (BN=128): two of them fit the staging area -> stores of tile i overlap tile i+1
-  const bool stg2 = p.use_tma_store && p.c_dtype == MQDET_F16 && 2 * BM * BN * 2 <= Cfg::STG_BYTES;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tma_a);
-    tma_prefetch_desc(&tma_b);
-    if (p.use_tma_store) tma_prefetch_desc(&tma_c);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full_bar[b], 1);
-      mbar_init(&tmem_empty_bar[b], 8);  // one arrival per epilogue warp (8 of them)
-    }
-    mbar_init(b_full_bar, 1);
-    mbar_init(b_empty_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_base_slot, 2 * BN);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
-
-  // Work distribution.
-  //  !BRES: item == tile (n fastest), dealt round-robin.
-  //   BRES: the tiles are laid out as [z][M chunk of `mc` tiles][n tile][m inside the chunk] and every CTA takes ONE
-  //         contiguous span of ceil(total / grid) of them (perfect balance; spans cut inside a run simply reload the
-  //         resident B tile).  A segment = consecutive m tiles with the same (z, n) = one residency of a B tile; CTAs with
-  //         neighbouring spans work on the same rows of A at the same time and share them through L2.
-  const int share = BRES ? (total_items + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-  const int w_begin = BRES ? (int)blockIdx.x * share : (int)blockIdx.x;
-  const int w_end = BRES ? min(total_items, w_begin + share) : total_items;
-  auto next_item = [&](int& cur, int& z, int& m0, int& mcount, int& n_tile) -> bool {
-    if (cur >= w_end) return false;
-    if (BRES) {
-      const int per_z = tiles_m * tiles_n;
-      z = cur / per_z;
-      const int u = cur - z * per_z;
-      const int c = u / (mc * tiles_n);
-      const int v = u - c * mc * tiles_n;
-      const int sc = min(mc, tiles_m - c * mc);
-      n_tile = v / sc;
-      const int mi = v - n_tile * sc;
-      m0 = c * mc + mi;
-      mcount = min(sc - mi, w_end - cur);
-      cur += mcount;
-    } else {
-      n_tile = cur % tiles_n;
-      m0 = (cur / tiles_n) % tiles_m;
-      z = cur / (tiles_n * tiles_m);
-      mcount = 1;
-      cur += gridDim.x;
-    }
-    return true;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int it = 0, li = 0;  // ring position / local item counter
-      int z, m0, mcount, n_tile;
-      for (int cur = w_begin; next_item(cur, z, m0, mcount, n_tile); ++li) {
-        const int z1 = z % p.nb1, z2 = z / p.nb1;
-        const int az1 = p.a_bcast1 ? 0 : z1, az2 = p.a_bcast2 ? 0 : z2;
-        const int bz1 = p.b_bcast1 ? 0 : z1, bz2 = p.b_bcast2 ? 0 : z2;
-        if (BRES) {
-          mbar_wait(b_empty_bar, (li & 1) ^ 1);  // the previous item's MMAs no longer read the resident tile
-          mbar_expect_tx(b_full_bar, num_kb * Cfg::B_BYTES);
-          for (int kb = 0; kb < num_kb; ++kb)
-            tma_load_4d(smem_b + kb * Cfg::B_BYTES, &tma_b, b_full_bar, kb * BK, n_tile * BN, bz1, bz2);
-        }
-        for (int mt = 0; mt < mcount; ++mt) {
-          for (int kb = 0; kb < num_kb; ++kb, ++it) {
-            const int s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait(&empty_bar[s], ph ^ 1);
-            if ((p.debug & 4) && it >= STAGES) {
-              mbar_arrive(&full_bar[s]);
-              continue;
-            }
-            mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-            tma_load_4d(smem_a + s * Cfg::A_BYTES, &tma_a, &full_bar[s], kb * BK, (m0 + mt) * BM, az1, az2);
-            if (!BRES) tma_load_4d(smem_b + s * Cfg::B_BYTES, &tma_b, &full_bar[s], kb * BK, n_tile * BN, bz1, bz2);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, BN, 0);
-      int it = 0, lt = 0, li = 0;
-      int z, m0, mcount, n_tile;
-      for (int cur = w_begin; next_item(cur, z, m0, mcount, n_tile); ++li) {
-        if (BRES) {
-          mbar_wait(b_full_bar, li & 1);
-          tc_fence_after();
-        }
-        for (int mt = 0; mt < mcount; ++mt, ++lt) {
-          const int buf = lt & 1;
-          mbar_wait(&tmem_empty_bar[buf], ((lt >> 1) & 1) ^ 1);  // epilogue has drained this accumulator
-          tc_fence_after();
-          const uint32_t acc = tmem_base + (uint32_t)(buf * BN);
-          for (int kb = 0; kb < num_kb; ++kb, ++it) {
-            const int s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait(&full_bar[s], ph);
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(smem_a + s * Cfg::A_BYTES);
-            const uint32_t b_addr = smem_u32(smem_b + (BRES ? kb : s) * Cfg::B_BYTES);
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(&full_bar[s], (kb / STAGES) & 1);
+    const uint32_t a_addr = smem_u32(smem_a + s * Cfg::A_BYTES) + g * (64 * 128);
+    const uint32_t b_addr = smem_u32(smem_b + s * Cfg::B_BYTES);
+    wgmma_fence_acc(acc);
+    wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t da = umma_desc_k_sw128(a_addr + k * 32);
-              const uint64_t db = umma_desc_k_sw128(b_addr + k * 32);
-              tc_mma_f16(acc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-            tc_commit(&empty_bar[s]);
-          }
-          tc_commit(&tmem_full_bar[buf]);
-        }
-        if (BRES) tc_commit(b_empty_bar);  // fires when this item's last MMA has consumed the resident tile
-      }
-    }
-  } else if (warp >= 4) {
-    int lt = 0, wcount = 0;
-    const int ew = (warp - 4) & 3, half = (warp - 4) >> 2, tid_e = threadIdx.x - 128;
-    // the fast epilogue covers everything without an activation when the output takes the TMA store (host: fast_epilogue_ok)
-    const bool fast = p.fast_epi != 0;
-    const bool plain = fast && p.c_dtype == MQDET_F16 && p.act == MQDET_ACT_NONE && p.R == nullptr;
-    const bool bcol = p.bias_mode == MQDET_VEC_PER_COL, brow = p.bias_mode == MQDET_VEC_PER_ROW;
-    const bool gcol = p.gate_mode == MQDET_VEC_PER_COL, grow = p.gate_mode == MQDET_VEC_PER_ROW;
-    const bool vec = bcol || gcol;
-    const float bscale = p.scale_after_bias ? p.alpha : 1.f;  // alpha * (acc + b) == fma(alpha, acc, alpha * b)
-    float g_u = 1.f;
-    if (fast && p.gate_mode == MQDET_VEC_SCALAR) g_u = p.gate_tanh ? tanhf(p.gate[0]) : p.gate[0];
-    int z, m0, mcount, n_tile;
-    for (int cur = w_begin; next_item(cur, z, m0, mcount, n_tile);) {
-      const int z1 = z % p.nb1, z2 = z / p.nb1;
-      for (int mt = 0; mt < mcount; ++mt, ++lt) {
-        const int buf = lt & 1;
-        if (fast) {
-          // per-column / per-row parameters are fetched BEFORE waiting for the accumulator: their latency is never exposed
-          const bool refresh = vec && (!BRES || mt == 0);
-          float s_pre = p.alpha, t_pre = 0.f;
-          if (refresh && tid_e < BN) {
-            const long col = (long)n_tile * BN + tid_e;
-            float g = g_u, bv = 0.f;
-            if (col < p.N) {
-              if (gcol) g = p.gate_tanh ? tanhf(p.gate[col]) : p.gate[col];
-              if (bcol) bv = p.bias[z1 * p.bias_b1 + z2 * p.bias_b2 + col];
-            }
-            s_pre = p.alpha * g;
-            t_pre = bscale * bv * g;
-          }
-          const long row = (long)(m0 + mt) * BM + ew * 32 + lane;
-          FastEpi fe;
-          fe.s_vec = vec ? s_vec : nullptr;
-          fe.t_vec = t_vec;
-          float g_r = g_u, b_r = 0.f;
-          if (row < p.M) {
-            if (grow) g_r = p.gate_tanh ? tanhf(p.gate[row]) : p.gate[row];
-            if (brow) b_r = p.bias[z1 * p.bias_b1 + z2 * p.bias_b2 + row];
-          }
-          fe.s_u = p.alpha * g_r;
-          fe.t_u = bscale * b_r * g_r;
-          fe.res = nullptr;
-          fe.res_f16 = p.r_dtype == MQDET_F16;
-          if (p.R && row < p.M) {
-            const long off = z1 * p.r_b1 + z2 * p.r_b2 + row * p.ldr;
-            fe.res = fe.res_f16 ? (const void*)(reinterpret_cast<const __half*>(p.R) + off)
-                                : (const void*)(reinterpret_cast<const float*>(p.R) + off);
-          }
-          mbar_wait(&tmem_full_bar[buf], (lt >> 1) & 1);
-          tc_fence_after();
-          if (p.debug & 1) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
-            continue;
-          }
-          if (refresh) {  // every epilogue warp left the previous tile's column loop at its closing barrier
-            if (tid_e < BN) {
-              s_vec[tid_e] = s_pre;
-              t_vec[tid_e] = t_pre;
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-          }
-          if constexpr (BN == 256 && BRES) {
-            // four 64-column windows through two alternating 16 KB staging tiles (fp16 TMA-store epilogue only)
-#pragma unroll 1
-            const long nl = p.N - (long)n_tile * BN;
-            const int nwin = nl >= BN ? 4 : (int)((nl + 63) >> 6);  // windows entirely beyond N are skipped
-            for (int w = 0; w < nwin; ++w, ++wcount) {  // wcount: the two staging tiles strictly alternate across tiles
-              uint8_t* const st_win = stg + (wcount & 1) * (BM * 128);
-              if (plain)
-                epilogue_fast<BN, true>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), st_win, fe, m0 + mt, n_tile, z1, z2, ew, lane,
-                                        &tmem_empty_bar[buf], true, half, w * 64, 64, w == nwin - 1);
-              else
-                epilogue_fast<BN, false>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), st_win, fe, m0 + mt, n_tile, z1, z2, ew, lane,
-                                         &tmem_empty_bar[buf], true, half, w * 64, 64, w == nwin - 1);
-            }
-          } else {
-            uint8_t* const st_tile = stg + (stg2 ? (lt & 1) * (BM * BN * 2) : 0);
-            if (plain)
-              epilogue_fast<BN, true>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), st_tile, fe, m0 + mt, n_tile, z1, z2, ew, lane,
-                                      &tmem_empty_bar[buf], stg2, half, 0, BN, true);
-            else
-              epilogue_fast<BN, false>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), st_tile, fe, m0 + mt, n_tile, z1, z2, ew, lane,
-                                       &tmem_empty_bar[buf], stg2, half, 0, BN, true);
-          }
-          continue;
-        }
-        mbar_wait(&tmem_full_bar[buf], (lt >> 1) & 1);
-        tc_fence_after();
-        if (p.debug & 1) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
-          continue;
-        }
-        if constexpr (BN == 256 && BRES) {
-          // (dispatched with the TMA-store epilogue only) four 64-column windows, two alternating 16 KB staging tiles
-#pragma unroll 1
-          for (int w = 0; w < 4; ++w)
-            epilogue_tile<BN>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), stg + (w & 1) * (BM * 128), m0 + mt, n_tile, z1, z2, ew,
-                              lane, &tmem_empty_bar[buf], 1, half, 2, w * 64, 64, w == 3);
-        } else {
-          epilogue_tile<BN>(p, &tma_c, tmem_base + (uint32_t)(buf * BN), stg + (stg2 ? (lt & 1) * (BM * BN * 2) : 0), m0 + mt,
-                            n_tile, z1, z2, ew, lane, &tmem_empty_bar[buf], stg2 ? 1 : 0, half, 2);
-        }
-      }
-    }
-    if (threadIdx.x == 128) tma_store_wait_read_all();
+    for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(acc, wg_desc_k_sw128(a_addr + k * 32), wg_desc_k_sw128(b_addr + k * 32));
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's group has retired: its slot may be refilled
+    wgmma_fence_acc(acc);
+    if (kb > 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * BN);
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+
+  // ---- epilogue from the accumulator fragments: bias / act / clamp / gate / residual, column pairs per store ----
+  float gate_s = 1.f;
+  if (p.gate_mode == MQDET_VEC_SCALAR) gate_s = p.gate_tanh ? tanhf(p.gate[0]) : p.gate[0];
+  const long row0 = (long)m_tile * BM + g * 64, col0 = (long)n_tile * BN;
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const long row = row0 + wg_row(tid, i), col = col0 + wg_col(tid, i);
+    if (row >= p.M || col >= p.N) continue;
+    const float v0 = epi_one(p, acc[i], row, col, z1, z2, gate_s);
+    if (col + 1 < p.N) {
+      const float v1 = epi_one(p, acc[i + 1], row, col + 1, z1, z2, gate_s);
+      if (p.vec2) {
+        const long off = z1 * p.c_b1 + z2 * p.c_b2 + row * p.ldc + col;
+        if (p.c_dtype == MQDET_F32)
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + off) = make_float2(v0, v1);
+        else
+          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.C) + off) = __floats2half2_rn(v0, v1);
+        continue;
+      }
+      store_one(p, v1, row, col + 1, z1, z2);
+    }
+    store_one(p, v0, row, col, z1, z2);
   }
 }
 
@@ -934,107 +249,24 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const GemmP p) {
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-// make_operand_map / make_output_map / num_sms / ensure_dyn_smem: capi.cu (shared with biattn.cu; tensor maps are cached)
-static int make_output_map(CUtensorMap* map, const GemmP& p) {
-  return make_store_map(map, p.C, p.c_dtype, p.M, p.N, p.ldc, p.nb1, p.c_b1, p.nb2, p.c_b2);
-}
-
-// What the persistent kernel's fast epilogue covers (everything else takes the generic one, which has no TMA-store +
-// residual variant): no activation; the gate folds into the scale, so a clamp (applied BEFORE the gate) excludes gates,
-// and a per-row gate/bias excludes per-column vectors; residual rows must take 16-byte loads.
-static bool fast_epilogue_ok(const GemmP& p) {
-  // order of the full epilogue: bias -> activation -> clamp -> gate -> residual; the fast one computes acc * S + T with the
-  // gate folded in, then activation, residual, clamp: identical unless an activation or clamp meets a gate / residual
-  if (p.act != MQDET_ACT_NONE && p.gate_mode != MQDET_VEC_NONE) return false;
-  if (p.clamp > 0.f && (p.gate_mode != MQDET_VEC_NONE || p.R)) return false;
-  const bool colv = p.bias_mode == MQDET_VEC_PER_COL || p.gate_mode == MQDET_VEC_PER_COL;
-  const bool rowv = p.bias_mode == MQDET_VEC_PER_ROW || p.gate_mode == MQDET_VEC_PER_ROW;
-  if (colv && rowv) return false;
-  if (p.R) {
-    const long al = p.r_dtype == MQDET_F16 ? 8 : 4;
-    if ((reinterpret_cast<uintptr_t>(p.R) & 15) || (p.ldr % al) || (p.nb1 > 1 && (p.r_b1 % al)) || (p.nb2 > 1 && (p.r_b2 % al)))
-      return false;
-  }
-  return true;
-}
-
-// TMA store needs 16-byte aligned rows/batches; a residual only goes with it in the persistent kernel's fast epilogue.
-static bool can_tma_store(const GemmP& p, int BN, bool persistent = false) {
-  const int es = (p.c_dtype == MQDET_F16) ? 2 : 4;
-  const long al = 16 / es;
-  if (BN < 128 / es) return false;
-  if (p.R && !(persistent && BN >= 64 && fast_epilogue_ok(p))) return false;
-  if (p.N % al) return false;  // the TMA unit bounds the innermost dimension at 16-byte granularity (measured): a ragged
-                               // N would spill into the row padding, so those shapes take the masked fallback
-  if ((reinterpret_cast<uintptr_t>(p.C) & 15) || (p.ldc % al) || (p.nb1 > 1 && (p.c_b1 % al)) || (p.nb2 > 1 && (p.c_b2 % al)))
-    return false;
-  if (p.nb1 > 1 && p.c_b1 == 0) return false;
-  if (p.nb2 > 1 && p.c_b2 == 0) return false;
-  return true;
-}
-
+// make_operand_map / num_sms / ensure_dyn_smem: capi.cu (shared with the other TMA kernels; tensor maps are cached)
 template <int BN, int STAGES>
-static int launch_tc(const GemmP& p0, cudaStream_t st) {
-  using Cfg = TcCfg<BN, STAGES>;
+static int launch_wg(const GemmP& p0, cudaStream_t st) {
+  using Cfg = WgCfg<BN, STAGES>;
   GemmP p = p0;
   CUtensorMap ma, mb;
   int rc = make_operand_map(&ma, p.A, p.M, p.K, p.lda, p.nb1, p.a_b1, p.nb2, p.a_b2, BM, &p.a_bcast1, &p.a_bcast2);
   if (rc) return rc;
   rc = make_operand_map(&mb, p.B, p.N, p.K, p.ldb, p.nb1, p.b_b1, p.nb2, p.b_b2, BN, &p.b_bcast1, &p.b_bcast2);
   if (rc) return rc;
-  CUtensorMap mc = ma;  // placeholder when unused
-  p.use_tma_store = can_tma_store(p, BN) ? 1 : 0;
-  if (p.use_tma_store) {
-    rc = make_output_map(&mc, p);
-    if (rc) return rc;
-  }
-  rc = ensure_dyn_smem(reinterpret_cast<const void*>(&gemm_tc_kernel<BN, STAGES>), Cfg::SMEM_BYTES);
+  const long al = p.c_dtype == MQDET_F16 ? 2 : 1;  // pair stores: 4-byte (fp16) / 8-byte (fp32) aligned
+  p.vec2 = (p.ldc % 2 == 0) && (p.nb1 == 1 || p.c_b1 % 2 == 0) && (p.nb2 == 1 || p.c_b2 % 2 == 0) &&
+           (reinterpret_cast<uintptr_t>(p.C) % (4 * (3 - al))) == 0;
+  rc = ensure_dyn_smem(reinterpret_cast<const void*>(&gemm_wg_kernel<BN, STAGES>), Cfg::SMEM_BYTES);
   if (rc) return rc;
   dim3 grid(cdiv(p.N, BN), cdiv(p.M, BM), p.nb1 * p.nb2);
-  gemm_tc_kernel<BN, STAGES><<<grid, 256, Cfg::SMEM_BYTES, st>>>(ma, mb, mc, p);
-  return check_launch("gemm_tc_kernel");
-}
-
-template <int BN, int STAGES, bool BRES>
-static int launch_tcp(const GemmP& p0, cudaStream_t st) {
-  using Cfg = TcpCfg<BN, STAGES, BRES>;
-  GemmP p = p0;
-  CUtensorMap ma, mb;
-  int rc = make_operand_map(&ma, p.A, p.M, p.K, p.lda, p.nb1, p.a_b1, p.nb2, p.a_b2, BM, &p.a_bcast1, &p.a_bcast2);
-  if (rc) return rc;
-  rc = make_operand_map(&mb, p.B, p.N, p.K, p.ldb, p.nb1, p.b_b1, p.nb2, p.b_b2, BN, &p.b_bcast1, &p.b_bcast2);
-  if (rc) return rc;
-  CUtensorMap mc_map = ma;
-  p.use_tma_store = can_tma_store(p, BN, true) ? 1 : 0;
-  p.fast_epi = (p.use_tma_store && BN >= 64 && fast_epilogue_ok(p)) ? 1 : 0;
-  if (p.use_tma_store) {
-    rc = make_output_map(&mc_map, p);
-    if (rc) return rc;
-  }
-  rc = ensure_dyn_smem(reinterpret_cast<const void*>(&gemm_tcp_kernel<BN, STAGES, BRES>), Cfg::SMEM_BYTES);
-  if (rc) return rc;
-  const int tm = cdiv(p.M, BM), tn = cdiv(p.N, BN);
-  const long Z = (long)p.nb1 * p.nb2;
-  int mc = 1;
-  long total = (long)tm * tn * Z;
-  if (BRES) {
-    // every CTA takes one contiguous span of the [z][chunk][n][m] tile order (see the kernel): chunk length = the span
-    // length, so that a span normally is ONE (chunk, n) cell and the CTAs of a chunk share its rows of A through L2;
-    // with a single n tile the chunk is the whole M range (spans cut it anywhere)
-    const long sms = num_sms();
-    const long g = total < sms ? total : sms;
-    const long share = (total + g - 1) / g;
-    mc = tn == 1 ? tm : (int)(share < 1 ? 1 : (share > tm ? tm : share));
-  }
-  const int grid = (int)(total < num_sms() ? total : num_sms());
-  if (const char* dbg = getenv("MQDET_GEMM_DEBUG")) {
-    GemmP q = p;
-    q.debug = atoi(dbg);
-    gemm_tcp_kernel<BN, STAGES, BRES><<<grid, 384, Cfg::SMEM_BYTES, st>>>(ma, mb, mc_map, q, tm, tn, (int)total, mc);
-    return check_launch("gemm_tcp_kernel");
-  }
-  gemm_tcp_kernel<BN, STAGES, BRES><<<grid, 384, Cfg::SMEM_BYTES, st>>>(ma, mb, mc_map, p, tm, tn, (int)total, mc);
-  return check_launch("gemm_tcp_kernel");
+  gemm_wg_kernel<BN, STAGES><<<grid, 384, Cfg::SMEM_BYTES, st>>>(ma, mb, p);
+  return check_launch("gemm_wg_kernel");
 }
 
 }  // namespace mqdet
@@ -1069,41 +301,13 @@ extern "C" int mqdet_gemm_f16(const mqdet_gemm_args* a, int impl, void* stream) 
     gemm_simt_kernel<<<grid, 256, 0, st>>>(p);
     return check_launch("gemm_simt_kernel");
   }
-  MQ_REQUIRE(impl == MQDET_GEMM_IMPL_TCGEN05 || impl == MQDET_GEMM_IMPL_TCGEN05_ONESHOT, "gemm: unknown impl %d", impl);
+  MQ_REQUIRE(impl == MQDET_GEMM_IMPL_TC || impl == MQDET_GEMM_IMPL_TC_ONESHOT, "gemm: unknown impl %d", impl);
   MQ_REQUIRE((a->K % 8) == 0 && (a->lda % 8) == 0 && (a->ldb % 8) == 0, "gemm: K/lda/ldb must be multiples of 8");
   MQ_REQUIRE((a->a_b1 % 8) == 0 && (a->a_b2 % 8) == 0 && (a->b_b1 % 8) == 0 && (a->b_b2 % 8) == 0,
              "gemm: batch strides must be multiples of 8");
   MQ_REQUIRE(((uintptr_t)a->A % 16) == 0 && ((uintptr_t)a->B % 16) == 0, "gemm: A/B must be 16-byte aligned");
-  const long mt = cdiv(p.M, BM), z = (long)p.nb1 * p.nb2;
-  if (impl == MQDET_GEMM_IMPL_TCGEN05_ONESHOT) {
-    // one output tile per CTA, two CTAs per SM (the round-1a kernel, kept for A/B measurements)
-    if (p.N >= 256 && p.K >= 1024 && mt * cdiv(p.N, 256) * z >= 148) return launch_tc<256, 4>(p, st);
-    if (p.N > 64 && (mt * cdiv(p.N, 128) * z >= 120 || p.N > 1024)) return launch_tc<128, 3>(p, st);
-    if (p.N > 32) return launch_tc<64, 4>(p, st);
-    return launch_tc<32, 4>(p, st);
-  }
-  // Persistent kernel.  Short-K products (K <= 256) are L2->SM bandwidth bound at 128-wide tiles, so they keep the B tile
-  // resident (BRES) and stream only A; tile-N = the widest tile that still yields >= ~1 tile per SM.
-  // 128- vs 64-wide tiles: fewer waves x tile cost (MMA time per tile ~ BN) wins; ties go to the wider tile (fewer loads)
-  const long t128 = mt * cdiv(p.N, 128) * z, t64 = mt * cdiv(p.N, 64) * z;
-  const long w128 = (t128 + num_sms() - 1) / num_sms(), w64 = (t64 + num_sms() - 1) / num_sms();
-  const bool wide = p.N > 64 && (w128 * 128 * 10 <= w64 * 64 * 12);  // the narrow tile must win by > 20 %
-  if (p.K <= BRES_KB * BK && mt * cdiv(p.N, 128) * z >= 2L * num_sms()) {
-    // 128x128 MMAs (both operands from shared memory) run at about half the tensor rate of 128x256 (measured: 684 vs
-    // 1750 TFLOP/s with loads and epilogue disabled), so the 256-wide resident tile is used whenever the output can take
-    // the fp16 TMA-store epilogue
-    // ... unless the 256-wide tiling pads N by more than `waste` (e.g. N = 288 -> 512): those products are output / epilogue
-    // bound and take the 128-wide resident tile (MQDET_BRES256_MAXWASTE overrides the threshold for A/B runs)
-    static const float waste = getenv("MQDET_BRES256_MAXWASTE") ? (float)atof(getenv("MQDET_BRES256_MAXWASTE")) : 2.0f;
-    const bool fits256 = (float)(cdiv(p.N, 256) * 256) <= waste * (float)p.N;
-    if (p.N >= 256 && fits256 && p.c_dtype == MQDET_F16 && can_tma_store(p, 256, true) && mt * cdiv(p.N, 256) * z >= num_sms())
-      return launch_tcp<256, 3, true>(p, st);
-    if (wide) return launch_tcp<128, 4, true>(p, st);
-  }
-  if (p.K >= 512 && p.N >= 256 && p.c_dtype == MQDET_F16 && mt * cdiv(p.N, 256) * z >= num_sms() && can_tma_store(p, 256, true))
-    return launch_tcp<256, 3, false>(p, st);  // long-K: 128x256 tiles halve the A re-reads (MMA/L2 bound regime)
-  if (wide) return launch_tcp<128, 4, false>(p, st);
-  if (p.N > 32) return launch_tcp<64, 4, false>(p, st);
-  return launch_tcp<32, 4, false>(p, st);
+  // 128-wide tiles when they still give every SM a tile, 64-wide ones (two CTAs per SM) otherwise
+  const long tiles128 = (long)cdiv(p.M, BM) * cdiv(p.N, 128) * p.nb1 * p.nb2;
+  if (p.N > 64 && tiles128 >= num_sms()) return launch_wg<128, 4>(p, st);
+  return launch_wg<64, 4>(p, st);
 }
-

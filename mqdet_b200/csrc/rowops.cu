@@ -1110,7 +1110,7 @@ extern "C" int mqdet_sum_splits_cast(const float* part, int64_t nb2, int64_t nb1
 extern "C" int mqdet_cast_f32_f16(const float* x, void* y, int64_t n, void* stream) {
   MQ_REQUIRE(x && y && n > 0, "cast: bad args");
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   cast_f32_f16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, (__half*)y, n);
   return check_launch("cast_f32_f16_kernel");
 }
@@ -1126,7 +1126,7 @@ extern "C" int mqdet_contrastive_mask(float* logits, const uint8_t* text_token_m
 extern "C" int mqdet_cast_f16_f32(const void* x, float* y, int64_t n, void* stream) {
   MQ_REQUIRE(x && y && n > 0, "cast: bad args");
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   cast_f16_f32_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)x, y, n);
   return check_launch("cast_f16_f32_kernel");
 }

@@ -6,7 +6,7 @@
 //            maskrcnn_benchmark/modeling/backbone/fpn.py FPN.forward :59-129, LastLevelP6P7 :137-154;
 //            generalized_vl_rcnn_new.py flatten_fpn_features :291-293 (AvgPool2d(2)).
 // Token layout everywhere: [B][H*W][C], row-major (h, w).  The dense projections (qkv, proj, MLP, reductions, 1x1/3x3
-// convolutions) run on the tcgen05 GEMM; these kernels only gather/scatter and do the 49x49 window attention.
+// convolutions) run on the wgmma GEMM; these kernels only gather/scatter and do the 49x49 window attention.
 #include "common.cuh"
 #include "../../include/mqdet_b200.h"
 
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) patchify4_kernel(const float* __restrict_
 // One CTA (4 warps) per (window, head).  The window's q / k / v head slices (64 B per token each) are staged in shared
 // memory with 16-byte loads (v transposed: the B fragments of P.V need two consecutive KEYS per register); warp w then
 // takes the 16-query tiles w, w+4, ...: S = Q K^T and O = P V on mma.sync.m16n8k16 (fp16 in, fp32 accumulate — a
-// 49x49x32 / 144x144x32 problem per head is far below a tcgen05 tile), softmax in the accumulator fragments (quad
+// 49x49x32 / 144x144x32 problem per head is far below a wgmma tile), softmax in the accumulator fragments (quad
 // shuffles), P re-used as the A fragment of the second product (no shared-memory round trip).
 __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm volatile(

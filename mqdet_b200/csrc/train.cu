@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
 
 static inline unsigned ew_blocks(long n) {
   long b = (n + 255) / 256;
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > 132 * 8) b = 132 * 8;
   return (unsigned)(b < 1 ? 1 : b);
 }
 

@@ -8,7 +8,7 @@
 // One CTA (4 warps) per (64 queries, head, image); a warp owns 16 queries.  Keys / values stream through shared memory in
 // chunks of 64 tokens (16-byte global loads of the NEXT chunk are in flight while the current one is consumed; V is stored
 // transposed because the B fragments of P.V need two consecutive KEYS per register).  S = Q K^T and O += P V run on
-// mma.sync.m16n8k16 (a 16 x 64 x 32 problem per warp and chunk is far below a tcgen05 tile); the softmax is the online
+// mma.sync.m16n8k16 (a 16 x 64 x 32 problem per warp and chunk is far below a wgmma tile); the softmax is the online
 // (running max / running sum) form in the accumulator fragments, fp32 throughout, P travels as fp16.
 #include "common.cuh"
 #include "../../include/mqdet_b200.h"

@@ -1,4 +1,4 @@
-"""FPN (P3-P5 + conv P6/P7) on sm_100a kernels.
+"""FPN (P3-P5 + conv P6/P7) on sm_90a kernels.
 
 Drop-in for maskrcnn_benchmark/modeling/backbone/fpn.py (``FPN`` :6-129 in the SWINT-FPN-RETINANET configuration of
 modeling/backbone/__init__.py:37-80: in_channels_list [0, C3, C4, C5], plain convs with bias, ``LastLevelP6P7``

@@ -1,4 +1,4 @@
-"""Swin Transformer backbone on sm_100a kernels.
+"""Swin Transformer backbone on sm_90a kernels.
 
 Drop-in for maskrcnn_benchmark/modeling/backbone/swint.py (``SwinTransformer`` :434-615, ``SwinTransformerBlock``
 :145-242, ``WindowAttention`` :64-142, ``PatchMerging`` :245-284, ``PatchEmbed`` :393-431) with the reference's

@@ -9,7 +9,7 @@ three places, all handled by the shared implementation:
   * masks are boolean with True = padding and are filled with -inf (:201-214), for the text tokens AND for the image tokens;
   * the block takes / returns flat ``[B, N, C]`` tensors (no FPN-level lists).
 The scores are materialised in fp32 here (the global maximum is needed before either softmax), i.e. this is the explicit path,
-not the fused tcgen05 attention kernels of the GLIP tower.
+not the fused wgmma attention kernels of the GLIP tower.
 """
 import torch
 from torch import nn

@@ -1,4 +1,4 @@
-"""MQ-GroundingDINO-T forward on sm_100a kernels, drop-in for groundingdino_new/models/GroundingDINO/groundingdino.py:93-709
+"""MQ-GroundingDINO-T forward on sm_90a kernels, drop-in for groundingdino_new/models/GroundingDINO/groundingdino.py:93-709
 (``GroundingDINO``), backbone/backbone.py:155-221 (``Joiner`` of Swin-T + ``PositionEmbeddingSineHW``) and bertwarper.py:28-223
 (``BertModelWarper`` around the vision-conditioned ``QVBertModel``), inference only (BASELINE config 4).
 

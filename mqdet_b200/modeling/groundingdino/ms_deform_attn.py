@@ -1,4 +1,4 @@
-"""Multi-scale deformable attention of the GroundingDINO encoder / decoder on sm_100a kernels.
+"""Multi-scale deformable attention of the GroundingDINO encoder / decoder on sm_90a kernels.
 
 Drop-in for groundingdino_new/models/GroundingDINO/ms_deform_attn.py:136-352 (``MultiScaleDeformableAttention``): same
 constructor arguments, parameter names (``sampling_offsets``, ``attention_weights``, ``value_proj``, ``output_proj``) and forward

@@ -1,4 +1,4 @@
-"""GroundingDINO's encoder / decoder on sm_100a kernels, drop-in for groundingdino_new/models/GroundingDINO/transformer.py
+"""GroundingDINO's encoder / decoder on sm_90a kernels, drop-in for groundingdino_new/models/GroundingDINO/transformer.py
 (``Transformer`` :40-403, ``TransformerEncoder`` :406-590, ``TransformerDecoder`` :593-716, ``DeformableTransformerEncoderLayer``
 :719-760, ``DeformableTransformerDecoderLayer`` :763-878) and transformer_vanilla.py:72-123 (``TransformerEncoderLayer``, the text
 enhancer) under the shipped MQ-GroundingDINO-T settings (config/defaults.py:944-987: two_stage_type "standard", embed_init_tgt,
@@ -7,7 +7,7 @@ text enhancer, fusion layers, text cross-attention, post-norm, relu, dropout 0),
 Same constructor arguments and ``state_dict`` keys as the reference (``nn.MultiheadAttention`` / ``nn.Linear`` / ``nn.LayerNorm``
 objects are parameter containers); all arithmetic runs in libmqdet_b200.so:
 
-  * every Linear / attention product: the tcgen05 GEMM (fp16 operands, fp32 accumulation, fused bias / relu / residual epilogues);
+  * every Linear / attention product: the wgmma GEMM (fp16 operands, fp32 accumulation, fused bias / relu / residual epilogues);
   * ``nn.MultiheadAttention`` (text enhancer with the per-category block mask, decoder self-attention over the 900 queries, decoder
     text cross-attention with the padding mask): Q|K|V^T projections, scores laid out [B, Lq, H, Lk] so one mask row serves the H
     heads of a query, ``softmax_rows`` with the mask folded in, P.V, output projection;

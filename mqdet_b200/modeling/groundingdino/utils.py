@@ -16,7 +16,7 @@ from ...utils.weights import f32, w16
 
 
 class MLP(nn.Module):
-    """utils.py:171-185 — Linear + relu ... Linear; parameter names ``layers.N``.  Every layer is one tcgen05 GEMM with the bias /
+    """utils.py:171-185 — Linear + relu ... Linear; parameter names ``layers.N``.  Every layer is one wgmma GEMM with the bias /
     relu (and, on the last layer, an optional residual) in the epilogue."""
 
     def __init__(self, input_dim, hidden_dim, output_dim, num_layers):
@@ -88,7 +88,7 @@ class ContrastiveEmbed(nn.Module):
     @torch.no_grad()
     def forward(self, x, text_dict):
         """x [bs, nq, d_model]; text_dict = {'encoded_text': [bs, T, d_model], 'text_token_mask': [bs, T] bool (True =
-        token in use)} -> [bs, nq, max_text_len] fp32, -inf on padding and beyond T.  One tcgen05 product (fp16 operands,
+        token in use)} -> [bs, nq, max_text_len] fp32, -inf on padding and beyond T.  One wgmma product (fp16 operands,
         fp32 accumulate/output) + the in-place mask/pad kernel."""
         assert isinstance(text_dict, dict)
         y = text_dict["encoded_text"]

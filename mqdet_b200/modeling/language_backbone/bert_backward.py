@@ -1,4 +1,4 @@
-"""Activation backward of a (frozen) post-LN BERT layer on sm_100a kernels — the part of the modulated pre-training backward that
+"""Activation backward of a (frozen) post-LN BERT layer on sm_90a kernels — the part of the modulated pre-training backward that
 carries the loss gradient through ``encoder.layer.N`` between two Gated Class-scalable Perceiver blocks (QVBertEncoder.forward,
 modeling_bert_new.py:566-610: GCP block i-6 sits BEFORE BERT layer i, so the gradient of block i-6 needs the backward of layers i..11).
 BERT itself is frozen in the MQ pre-training (tools/train_net.py:70-77): only dL/d(input) is produced, no weight gradients.
@@ -6,7 +6,7 @@ BERT itself is frozen in the MQ pre-training (tools/train_net.py:70-77): only dL
     BertLayerTrain(layer).forward(h32, h16, colmask)   the inference kernels, keeping the activations the backward needs
     BertLayerTrain(layer).backward(dout)               dL/dh, fp32 [B,T,D]
 
-Every product of the backward is a tcgen05 GEMM: dX = dY W with the cached transposed weight (``wT16``); the attention backward
+Every product of the backward is a wgmma GEMM: dX = dY W with the cached transposed weight (``wT16``); the attention backward
 (dP = dC V^T, dQ = dS K, dK = dS^T Q, dV = P^T dC) takes its K-major operands from operand-swapped projections (K^T = W_k h^T, like
 the forward's V^T) or from ``mqdet_transpose_cast_batched``; softmax / LayerNorm / GELU backward are the kernels of csrc/train.cu.
 Pre-activations of the GELU and the V / K^T / Q^T projections are recomputed rather than stored.

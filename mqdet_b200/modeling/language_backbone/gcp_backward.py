@@ -1,4 +1,4 @@
-"""Training forward / backward of the Gated Class-scalable Perceiver block on sm_100a kernels — SURVEY.md §8(b2)'s ``gcp_block_fwd`` /
+"""Training forward / backward of the Gated Class-scalable Perceiver block on sm_90a kernels — SURVEY.md §8(b2)'s ``gcp_block_fwd`` /
 ``gcp_block_bwd`` (BASELINE config 5: "GCP backward kernel").  In the reference these blocks (``encoder.qv_layer.N``) and PreSelect are
 the ONLY trainable parameters of the modulated pre-training (tools/train_net.py:70-77, solver/build.py:46-49); their backward is
 autograd over modeling_bert_new.py:186-248,298-374.  Here:
@@ -7,7 +7,7 @@ autograd over modeling_bert_new.py:186-248,298-374.  Here:
     dx, dvision, grads = GCPBlockTrain(block).backward(dy)   grads: {parameter name -> fp32 gradient}, names as in block.state_dict()
 
 Forward arithmetic is the inference path (same kernels, same order).  Backward: every activation gradient dX = dY W and weight
-gradient dW = dY^T X is one tcgen05 GEMM (fp16 operands, fp32 accumulation; both operands of a weight gradient are brought to
+gradient dW = dY^T X is one wgmma GEMM (fp16 operands, fp32 accumulation; both operands of a weight gradient are brought to
 K-major by ``mqdet_transpose_cast``); LayerNorm / GELU / gate / sparse-attention backward, the scalar ff_gate gradient and the scatter
 of dK / dV onto the unique query rows are the kernels of csrc/train.cu.  Pre-activations of the two GELUs are recomputed (one GEMM
 each) instead of being stored.  Gradients w.r.t. the text stream are fp32; fp16 intermediates (dq, d(out), dz) can underflow for tiny

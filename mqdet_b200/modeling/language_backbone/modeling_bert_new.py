@@ -1,4 +1,4 @@
-"""Vision-conditioned BERT: Gated Class-scalable Perceiver (GCP) blocks + PreSelect + BERT layers on sm_100a kernels.
+"""Vision-conditioned BERT: Gated Class-scalable Perceiver (GCP) blocks + PreSelect + BERT layers on sm_90a kernels.
 
 Drop-in for maskrcnn_benchmark/modeling/language_backbone/modeling_bert_new.py: same class names, constructor
 arguments, parameter names (``attn.norm``, ``attn.norm_kv``, ``attn.to_q``, ``attn.to_kv``, ``attn.to_out``,

@@ -1,4 +1,4 @@
-"""Training forward / backward of PreSelect (modeling_bert_new.py:377-448) on sm_100a kernels — with the GCP blocks the only trainable
+"""Training forward / backward of PreSelect (modeling_bert_new.py:377-448) on sm_90a kernels — with the GCP blocks the only trainable
 parameters of the modulated pre-training (``'pre_select' in key``: tools/train_net.py:70-77, solver/build.py:46-49).
 
     PreSelectTrain(module).forward(vision, image)   -> vision' fp32 [B,V,out_dim]  (the input of every GCP block)
@@ -6,7 +6,7 @@ parameters of the modulated pre-training (``'pre_select' in key``: tools/train_n
 
 The training forward materialises the attention probabilities (the inference path's flash-style ``mqdet_dense_cross_attn`` keeps none);
 the image tokens come from the frozen FPN, so no gradient flows into them.  As in gcp_backward.py every dX = dY W / dW = dY^T X /
-attention-backward product is a tcgen05 GEMM and the K-major operands come from ``mqdet_transpose_cast(_batched)``.
+attention-backward product is a wgmma GEMM and the K-major operands come from ``mqdet_transpose_cast(_batched)``.
 """
 import torch
 from torch import nn

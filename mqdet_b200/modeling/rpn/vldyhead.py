@@ -1,4 +1,4 @@
-"""VL deep-fusion head (VLDyHead) on sm_100a kernels.
+"""VL deep-fusion head (VLDyHead) on sm_90a kernels.
 
 Drop-in for the hot-path slice of maskrcnn_benchmark/modeling/rpn/vldyhead.py: ``Conv3x3Norm`` (:111-152), ``DyConv``
 (:155-247), ``BertEncoderLayer`` (:250-301), ``VLFuse`` (MHA-B, :364-574), ``VLDyHead`` (:594-900) with the

@@ -8,11 +8,11 @@ import ctypes
 import torch
 
 from . import _lib
-from ._lib import (ACT_GELU, ACT_NONE, ACT_RELU, F16, F32, IMPL_SIMT, IMPL_TCGEN05, IMPL_TCGEN05_ONESHOT, VEC_NONE, VEC_PER_COL,
+from ._lib import (ACT_GELU, ACT_NONE, ACT_RELU, F16, F32, IMPL_SIMT, IMPL_TC, IMPL_TC_ONESHOT, VEC_NONE, VEC_PER_COL,
                    VEC_PER_ROW, VEC_SCALAR, GemmArgs, check, load)
 
 # tests flip this to IMPL_SIMT to cross-check the tensor-core kernel against the plain FMA kernel
-DEFAULT_GEMM_IMPL = IMPL_TCGEN05
+DEFAULT_GEMM_IMPL = IMPL_TC
 
 # number of kernels launched through this module since the last reset (bench.py's gpu_launches)
 launch_count = 0
@@ -146,7 +146,7 @@ def gemm(a, b, out=None, *, out_dtype=torch.float16, alpha=1.0, bias=None, bias_
     gbytes = 2.0 * M * K * (a4.shape[0] * a4.shape[1]) + 2.0 * N * K * (b4.shape[0] * b4.shape[1]) + float(es_o) * M * N * nb
     if residual is not None:
         gbytes += (2.0 if residual.dtype == torch.float16 else 4.0) * M * N * nb
-    with _Timed("gemm_tcp_kernel", 2.0 * M * N * K * nb, gbytes):
+    with _Timed("gemm_wg_kernel", 2.0 * M * N * K * nb, gbytes):
         check(load().mqdet_gemm_f16(ctypes.byref(g), DEFAULT_GEMM_IMPL if impl is None else impl, _stream()), "gemm")
     if GEMM_PROFILE is not None:
         e1.record()

@@ -1,4 +1,4 @@
-"""Optimizer of the modulated pre-training on sm_100a kernels, drop-in for maskrcnn_benchmark/solver/build.py:8-57 (``make_optimizer``
+"""Optimizer of the modulated pre-training on sm_90a kernels, drop-in for maskrcnn_benchmark/solver/build.py:8-57 (``make_optimizer``
 with SOLVER.OPTIMIZER "ADAMW" and full-model gradient clipping): per-parameter learning rate / weight decay groups chosen by the
 reference's substring rules, ``torch.nn.utils.clip_grad_norm_`` over ALL trainable parameters, then ``torch.optim.AdamW``.
 

@@ -1,4 +1,4 @@
-"""Bi-directional image<->text multi-head attention of the VL deep-fusion tower on sm_100a kernels.
+"""Bi-directional image<->text multi-head attention of the VL deep-fusion tower on sm_90a kernels.
 
 Drop-in for maskrcnn_benchmark/utils/fuse_helper.py: ``BiMultiHeadAttention`` (:171-303) and
 ``BiAttentionBlockForCheckpoint`` (:344-426), same constructor arguments / parameter names / forward signatures,
@@ -8,7 +8,7 @@ Layout: the 5 FPN levels are kept concatenated as ONE fp16 tensor v [B, N, 256] 
 ``permute_and_flatten`` + ``cat`` the reference builds at :398-404 — so the tower never converts back to NCHW between
 layers (``forward_flat``).  ``forward`` keeps the reference's NCHW-in / NCHW-out signature for drop-in use.
 
-Every product is a K-major x K-major tcgen05 GEMM; transposed operands are produced by swapping operand roles
+Every product is a K-major x K-major wgmma GEMM; transposed operands are produced by swapping operand roles
 (V^T = W . x^T), never by a transpose kernel:
     Q  = (LN(v) Wv^T + b) * d^-1/2      [B,N,E]      K  = LN(l) Wl^T + b          [B,T,E]
     VvT= Wvv LN(v)^T + b (per row)      [B,E,N]      VlT= Wvl LN(l)^T + b         [B,E,T]
@@ -161,7 +161,7 @@ class BiMultiHeadAttention(nn.Module):
         operands of [256 x 256] fold the projections into the text side (tiny GEMMs over the T = 256 tokens):
             gT_h = K_h (d^-1/2 Wq_h)            S = (vn Wq_h^T + bq_h) d^-1/2 K_h^T == vn gT_h^T + gbias_h,  gbias_h = d^-1/2 bq_h . K_h
             mT_h = Wout_h Vl_h^T                (P Vl_h) Wout_h^T == P mT_h^T
-          image side: ONE kernel = S (TMEM) -> masked row softmax -> P . mT accumulated over the heads -> layer scale + residual;
+          image side: ONE kernel = S (registers) -> masked row softmax -> P . mT accumulated over the heads -> layer scale + residual;
                       it also emits the column maxima of the scores;
           text side : ONE kernel = S^T recomputed from gT and the image tokens -> exp(. - column max) -> P^T . vn (the image
                       tokens themselves; the value projection follows as a small per-head GEMM because sum_n p[n] = 1) with

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — builds the REFERENCE's own native extension (maskrcnn_benchmark/csrc: ml_nms,
-modulated_deform_conv_forward, ...) for sm_100a from the sources where they lie under /root/reference into
-oracle/_ref/ (git-ignored, shipped to the GPU box with the snapshot).  No reference source is copied into this repo.
+modulated_deform_conv_forward, ...) for sm_90a from the reference sources (directory MQDET_REFERENCE, see
+oracle/ref_loader.py) into oracle/_ref/ (git-ignored).  No reference source is copied into this repo.
 
     python oracle/build_ref.py
 
@@ -21,7 +21,7 @@ def main():
         print("reference sources not present; nothing to build")
         return 0
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "8")
     from torch.utils.cpp_extension import load
     srcs = glob.glob(os.path.join(csrc, "*.cpp")) + glob.glob(os.path.join(csrc, "cpu", "*.cpp")) + \
@@ -29,7 +29,7 @@ def main():
     load(name="mqdet_ref_C", sources=srcs, extra_include_paths=[csrc], build_directory=OUT, with_cuda=True,
          extra_cflags=["-DWITH_CUDA", "-O2"],
          extra_cuda_cflags=["-DWITH_CUDA", "-DCUDA_HAS_FP16=1", "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__",
-                            "-D__CUDA_NO_HALF2_OPERATORS__", "-gencode", "arch=compute_100a,code=sm_100a"],
+                            "-D__CUDA_NO_HALF2_OPERATORS__", "-gencode", "arch=compute_90a,code=sm_90a"],
          is_python_module=True, verbose=False)
     print("built", glob.glob(os.path.join(OUT, "*.so")))
     return 0

@@ -1,14 +1,14 @@
 """Same-box speed comparators (BASELINE.md §3, SURVEY.md §2.3 / §8d; VERDICT round 1 "missing" item 6) — measurements recorded
 as a GPU test because only tests/ may touch oracle/ and oracle/_ref:
 
-  * the reference's own CUDA kernels, built unmodified for sm_100a (oracle/_ref/mqdet_ref_C.so): ``ml_nms`` and
-    ``modulated_deform_conv_forward`` next to ``mqdet_ml_nms`` / ``mqdet_dcn_cols`` + the tcgen05 GEMM at the bench operating
-    point ("beat the reference kernel compiled for sm_100a on the same box");
-  * the reference ALGORITHM in eager PyTorch on the same B200 (oracle/restate.py moved to CUDA: the reference modules themselves
+  * the reference's own CUDA kernels, built unmodified for sm_90a (oracle/_ref/mqdet_ref_C.so): ``ml_nms`` and
+    ``modulated_deform_conv_forward`` next to ``mqdet_ml_nms`` / ``mqdet_dcn_cols`` + the wgmma GEMM at the bench operating
+    point ("beat the reference kernel compiled for sm_90a on the same box");
+  * the reference ALGORITHM in eager PyTorch on the same GPU (oracle/restate.py moved to CUDA: the reference modules themselves
     cannot be imported on the GPU box) for one GCP block and one BiAttention fusion layer at the BASELINE config 2 shapes
     ("fused GCP kernel vs reference PyTorch attention"), fp32 and fp16 autocast.
 
-Times: CUDA events, warm-up + 10 repetitions; written to gpurun_out/comparators.json (summarised in profiles/).
+Times: CUDA events, warm-up + 10 repetitions; written to comparators.json in the run's output directory.
 """
 import json
 import os
@@ -88,7 +88,7 @@ def _eager_gcp_block(x, vision, idx, sd, heads=8, dim_head=64):
 
 def test_speed_comparators(dev):
     from test_nms_gpu import _boxes
-    from test_ref_kernels_gpu import _ref, _ref_dcn
+    from test_ref_kernels_gpu import _ref_dcn, _ref_module
     from mqdet_b200 import ops
     from mqdet_b200.config import mq_glip_t_cfg
     from mqdet_b200.modeling.language_backbone.modeling_bert_new import GatedCrossAttentionBlock
@@ -98,11 +98,11 @@ def test_speed_comparators(dev):
     from util import load_sd, vq_cfg
     out = {}
     # ---- ml_nms at the bench operating point: ~3600 candidates per image, 80 labels --------------------------------
-    ref = _ref()
+    ref = _ref_module()  # the reference's compiled kernels are timed where oracle/_ref has been built
     boxes, scores, labels = _boxes(77, 3600, 80)
     scores = scores + torch.arange(3600) * 1e-7
     b, s, l = boxes.to(dev), scores.to(dev), labels.to(dev)
-    out["ml_nms_3600x80"] = {"reference_kernel_ms": _time(lambda: ref.ml_nms(b, s, l, 0.6)),
+    out["ml_nms_3600x80"] = {"reference_kernel_ms": _time(lambda: ref.ml_nms(b, s, l, 0.6)) if ref else None,
                              "mqdet_ms": _time(lambda: ops.ml_nms_device(b, s, l, 0.6)),
                              "note": "reference = ATen sort + nms kernel + D2H of the mask + host scan (csrc/cuda/ml_nms.cu:79-149); "
                                      "mqdet = device argsort + bitmask + device scan, no D2H"}
@@ -130,11 +130,11 @@ def test_speed_comparators(dev):
 
     y_i, y_c = ours_implicit().float(), ours().float()
     assert (y_i - y_c).abs().max().item() <= 2e-3 * y_c.abs().max().item()
-    out["dcnv2_3x3_B8_100x168_256ch"] = {"reference_kernel_ms": _time(lambda: _ref_dcn(ref, x, off, msk, w, bias, 1)),
+    out["dcnv2_3x3_B8_100x168_256ch"] = {"reference_kernel_ms": _time(lambda: _ref_dcn(ref, x, off, msk, w, bias, 1)) if ref else None,
                                          "mqdet_ms": _time(ours_implicit), "mqdet_cols_gemm_ms": _time(ours),
                                          "note": "reference = fp32 im2col + per-image SGEMM (deform_conv_cuda.cu:496-575); "
-                                                 "mqdet = implicit GEMM (mqdet_dcn_conv: sampling fused into the tcgen05 mainloop, "
-                                                 "no column matrix); mqdet_cols_gemm = the fp16 NHWC sampling kernel + tcgen05 GEMM "
+                                                 "mqdet = implicit GEMM (mqdet_dcn_conv: sampling fused into the wgmma mainloop, "
+                                                 "no column matrix); mqdet_cols_gemm = the fp16 NHWC sampling kernel + wgmma GEMM "
                                                  "pair it replaced"}
     # ---- eager-PyTorch reference algorithm vs the fused kernels: one BiAttention fusion layer, B = 8, N = 22400 ------
     sd = synth.bi_attention_sd(gen)

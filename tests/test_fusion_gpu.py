@@ -35,7 +35,7 @@ def test_bi_attention_vs_oracle_and_golden(dev):
 
 
 def test_bi_attention_fused_equals_unfused(dev):
-    """The product path (image-side kernel: scores in TMEM -> softmax -> P.V_l -> out-projection -> layer scale + residual;
+    """The product path (image-side kernel: scores in registers -> softmax -> P.V_l -> out-projection -> layer scale + residual;
     text-side kernel on the image tokens with in-kernel column sums) against the two unfused variants kept for A/B runs:
     "f32" (fp32 score matrices in HBM, softmax_rows, plain GEMMs) and "f16" (round-1 path: fp16 score matrix, fused text
     side with external statistics / transposed column softmax).  Ragged N (not a multiple of 64 / 128), T < 256, masks."""
@@ -126,7 +126,7 @@ def test_conv3x3_small_equals_conv2d(dev):
                                              ([(40, 56), (20, 28), (10, 14), (5, 7), (3, 4)], 2, True),
                                              ([(13, 17), (7, 9), (4, 5)], 2, False), ([(9, 11)], 2, True)])
 def test_dcn_conv_implicit_equals_cols_gemm(dev, sizes, B, with_om):
-    """mqdet_dcn_conv (sampling fused into the tcgen05 mainloop, three branches in one launch) against the sampling kernel +
+    """mqdet_dcn_conv (sampling fused into the wgmma mainloop, three branches in one launch) against the sampling kernel +
     GEMM pair it replaces: same fp16 operands, same fp32 accumulation, the mask folded into the corner weights (one fp32
     rounding apart) -> equal up to an fp16 ulp of the column values.  Sizes make tiles straddle levels, images and the ragged
     last tile; large offsets push samples outside the maps."""
@@ -205,12 +205,11 @@ def test_vldyhead_tower(dev):
     # 18 chained stages with fp16 operands; DCNv2 sampling positions and DyReLU branch choices depend on the features,
     # so rounding noise (~5e-4 per fp16-operand product, the per-operator tests above) is amplified layer over layer —
     # by ~1.5x per layer with these deliberately lively synthetic weights (offsets of whole pixels, x20 token projection).
-    # Round-2 attribution (tests/test_parity_experiment_gpu.py, profiles/r02_parity_experiment.md): every stage fed the
-    # oracle's input stays <= 1.1e-3 on its own; keeping the attention scores in fp32 does not change the end-to-end figure;
-    # and the fp32 CPU oracle ITSELF moves by 1.4e-2 (logits) when nothing but its inter-stage visual stream is rounded to
-    # fp16 (profiles/r02_fp16_storage_amplification.json).  The end-to-end deviation is therefore the chaotic amplification
-    # of fp16 STORAGE noise by these weights — it varies 1.2e-2 ... 1.8e-2 between bit-different but equally accurate
-    # kernel variants — and not a defect of a stage; test_tower_reference_like_init checks the same tower at 3e-3 with
+    # Attribution (tests/test_parity_experiment_gpu.py): every stage fed the oracle's input stays at the per-operator scale on
+    # its own; keeping the attention scores in fp32 does not change the end-to-end figure; and the fp32 CPU oracle ITSELF moves
+    # by 1.4e-2 (logits) when nothing but its inter-stage visual stream is rounded to fp16 (tools/fp16_storage_experiment.py).
+    # The end-to-end deviation is therefore the chaotic amplification of fp16 STORAGE noise by these weights — it moves between
+    # bit-different but equally accurate kernel variants — and not a defect of a stage; test_tower_reference_like_init checks the same tower at 3e-3 with
     # weights scaled like the reference's initialisation.  The per-operator bound stays at the north-star 1e-3.
     bad = []
     assert_close(r["hidden"], ref["hidden"], 4e-3, "tower: language stream", defer=bad)

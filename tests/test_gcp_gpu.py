@@ -99,7 +99,7 @@ def test_gcp_block(dev, B, ncls, ragged):
     assert s.cpu()[no_cls].abs().max().item() == 0.0
 
 
-def test_gcp_block_tcgen05_matches_simt(dev):
+def test_gcp_block_tensor_core_matches_simt(dev):
     """Same block with the GEMMs routed through the plain FMA kernel: isolates tensor-core/TMA addressing errors."""
     from mqdet_b200 import ops
     from mqdet_b200.modeling.language_backbone.modeling_bert_new import GatedCrossAttentionBlock
@@ -112,8 +112,8 @@ def test_gcp_block_tcgen05_matches_simt(dev):
         ops.DEFAULT_GEMM_IMPL = ops.IMPL_SIMT
         b = blk(x.to(dev), vision.to(dev), mask.to(dev))
     finally:
-        ops.DEFAULT_GEMM_IMPL = ops.IMPL_TCGEN05
-    assert_close(a, b, 2e-4, "tcgen05 vs simt")
+        ops.DEFAULT_GEMM_IMPL = ops.IMPL_TC
+    assert_close(a, b, 2e-4, "tensor-core vs simt")
 
 
 @pytest.mark.parametrize("B,ncls", [(1, 10), (2, 80)])

@@ -167,10 +167,22 @@ def _build_transformer(sd, nq, el, dl, dev):
     return load_sd(T, sd).to(dev).eval()
 
 
-def _run_transformer(T, srcs, masks, poss, enc_text, tmask, pid, sam, dev):
+def _run_transformer(T, srcs, masks, poss, enc_text, tmask, pid, sam, dev, proposals=None):
     geo = T.prepare([m.to(dev) for m in masks], [p.to(dev) for p in poss], tmask.to(dev), pid.to(dev), sam.to(dev))
     src = torch.cat([s.flatten(2).transpose(1, 2) for s in srcs], 1).contiguous().to(dev)
-    return T.forward_flat(src, geo, enc_text.to(dev).contiguous(), all_layers=True)
+    return T.forward_flat(src, geo, enc_text.to(dev).contiguous(), all_layers=True,
+                          proposals=None if proposals is None else proposals.to(dev))
+
+
+def _selection_equivalent(ours, ref_idx, ref_logits, bound):
+    """The two-stage top-k selections agree up to near-ties: every position selected by one side only has an oracle logit within
+    `bound` (the class-logit tolerance) of the oracle's k-th largest one, i.e. its rank is decided by fp16 noise."""
+    for b in range(ref_idx.shape[0]):
+        kth = ref_logits[b].sort(descending=True).values[ref_idx.shape[1] - 1]
+        diff = set(ours[b].tolist()) ^ set(ref_idx[b].tolist())
+        if any(abs(float(ref_logits[b, i] - kth)) > bound for i in diff):
+            return False
+    return True
 
 
 def test_transformer_small_vs_oracle_and_golden(dev):
@@ -184,15 +196,23 @@ def test_transformer_small_vs_oracle_and_golden(dev):
                                     enc_layers=el, dec_layers=dl, return_all=True)
     T = _build_transformer(sd, nq, el, dl, dev)
     out = _run_transformer(T, c["srcs"], c["masks"], poss, c["enc_text"], c["tmask"], c["pid"], c["sam"], dev)
-    hs, refs = out["hs"], out["references"]
     errs = []
     # padded / invalid memory positions all carry the same class logit (their memory row is zeroed): torch.topk picks any of those
-    # ties, mqdet_topk_desc the lowest indices -- the selected BOXES (references[0]) are what has to agree
+    # ties, mqdet_topk_desc the lowest indices; and two valid positions whose logits differ by less than the fp16 noise of the
+    # encoder may swap ranks.  The selection has to agree up to such near-ties; everything downstream of it is then compared on
+    # the oracle's selection, so that a swapped rank does not pair up different queries
+    fin = torch.isfinite(ref["enc_class"])
+    ec = torch.where(fin, ref["enc_class"], torch.full((), -1e30))
+    bound = 3e-3 * torch.where(fin, ref["enc_class"], torch.zeros(())).abs().max().item() + 3e-3  # the class-logit tolerance below
     same_sel = torch.equal(out["topk_proposals"].cpu(), ref["topk"])
+    assert _selection_equivalent(out["topk_proposals"].cpu(), ref["topk"], ec.max(-1).values, bound), \
+        (out["topk_proposals"].cpu(), ref["topk"])
+    if not same_sel:
+        out = _run_transformer(T, c["srcs"], c["masks"], poss, c["enc_text"], c["tmask"], c["pid"], c["sam"], dev, proposals=ref["topk"])
+    hs, refs = out["hs"], out["references"]
     assert_close(refs[0], ref["references"][0], 2e-3, "gdino transformer: two-stage selected boxes", defer=errs)
     assert_close(out["memory"], ref["memory"], 3e-3, "gdino transformer: encoder memory", defer=errs)
     assert_close(out["memory_text"], ref["memory_text"], 3e-3, "gdino transformer: enhanced text", defer=errs)
-    fin = torch.isfinite(ref["enc_class"])
     assert torch.equal(torch.isfinite(out["enc_class"]).cpu(), fin)
     assert_close(torch.where(fin, out["enc_class"].cpu(), torch.zeros(())), torch.where(fin, ref["enc_class"], torch.zeros(())), 3e-3,
                  "gdino transformer: two-stage class logits", defer=errs)

@@ -1,4 +1,4 @@
-"""GPU parity of the GroundingDINO reuse row (SURVEY.md §8 a18): ContrastiveEmbed through the C ABI (tcgen05 product +
+"""GPU parity of the GroundingDINO reuse row (SURVEY.md §8 a18): ContrastiveEmbed through the C ABI (wgmma product +
 mask/pad kernel) against the CPU oracle and the golden vectors recorded from the reference's own class."""
 import os
 

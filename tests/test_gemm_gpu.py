@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM (through the C ABI) against a plain PyTorch fp32 reference of the same op and
+"""GPU parity of the wgmma GEMM (through the C ABI) against a plain PyTorch fp32 reference of the same op and
 against the SIMT validation kernel.  Tolerance: fp32 accumulation of fp16-exact products, so only summation order
 differs: |err| <= 2e-3*|ref|_max*sqrt(K)/sqrt(K) ~ rtol 1e-4; fp16 outputs add one fp16 rounding (2^-11 relative)."""
 import math
@@ -52,17 +52,15 @@ def test_plain(dev, M, N, K, out_dtype):
     _check(out, ref, out_dtype == torch.float16)
     simt = ops.gemm(a, b, out_dtype=out_dtype, impl=ops.IMPL_SIMT)
     _check(simt, ref, out_dtype == torch.float16)
-    oneshot = ops.gemm(a, b, out_dtype=out_dtype, impl=ops.IMPL_TCGEN05_ONESHOT)  # non-persistent tcgen05 variant
+    oneshot = ops.gemm(a, b, out_dtype=out_dtype, impl=ops.IMPL_TC_ONESHOT)
     _check(oneshot, ref, out_dtype == torch.float16)
 
 
 def test_persistent_many_tiles_per_cta(dev):
-    """> 148 tiles so every CTA of the persistent kernel loops (ring wrap, both TMEM buffers, staging reuse), with a
+    """Many more tiles than SMs (several waves of CTAs, 128- and 64-wide tiles, K from one k-block to a wrapping ring), with a
     ragged last M tile and batches."""
     from mqdet_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(77)
-    # the last three shapes have K <= 256 and >= 2 tiles per SM: they take the B-resident (BRES) variant, including a
-    # ragged M-chunk tail and per-batch B tiles
     for (Bz, M, N, K) in [(1, 128 * 40 + 37, 512, 256), (5, 1000, 384, 192), (1, 70000, 128, 64), (1, 128 * 100 + 5, 512, 256),
                           (6, 128 * 30, 256, 192), (3, 22400, 256, 256)]:
         a = (torch.randn(Bz, M, K, generator=g) * 0.5).half().to(dev)
@@ -75,9 +73,8 @@ def test_persistent_many_tiles_per_cta(dev):
 
 
 def test_persistent_epilogue_modes(dev):
-    """Every epilogue combination the forward uses, at sizes that take the persistent kernels (>= 2 tiles per SM):
-    the compact fast epilogue (scale/addend folding, residual prefetch, clamp), the generic one (GELU) and the
-    128x256 B-resident / long-K tiles with their 64-column staging windows."""
+    """Every epilogue combination the forward uses (scale / bias folding, per-row and per-column vectors, gates, residuals,
+    clamp, GELU), at sizes with several tiles per SM and long K."""
     from mqdet_b200 import ops
     from mqdet_b200._lib import ACT_GELU, VEC_PER_COL, VEC_PER_ROW, VEC_SCALAR
     g = torch.Generator(device="cpu").manual_seed(21)

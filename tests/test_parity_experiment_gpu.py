@@ -6,7 +6,7 @@ layer on the GPU next to the fp32 CPU oracle, twice per attention-score precisio
   * teacher-forced: every GPU stage consumes the ORACLE's input of that stage (rounded to the stage's storage type) ->
                     the error each stage adds on its own.
 Score precisions (``BiMultiHeadAttention.score_precision``): "fused" = the product path, "f16" = the round-1 fp16-stored score
-matrix, "f32" = diagnostic fp32 score matrix in HBM.  Results go to gpurun_out/parity_experiment.json (summarised in profiles/).
+matrix, "f32" = diagnostic fp32 score matrix in HBM.  Results go to parity_experiment.json in the run's output directory.
 """
 import json
 import os

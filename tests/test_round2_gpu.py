@@ -293,10 +293,11 @@ def test_prompt_cache_invalidation(dev):
 def test_ml_nms_score_ties_equal_reference_kernel(dev):
     """Exact ties between boxes of DIFFERENT labels (ties inside a label would make the reference's unstable device sort
     decide the result): kept set bit-identical to csrc/cuda/ml_nms.cu."""
+    from refpin import equal, pinned
     from test_nms_gpu import _boxes
-    from test_ref_kernels_gpu import _ref
+    from test_ref_kernels_gpu import _ref_module
     from mqdet_b200 import ops
-    ref = _ref()
+    ref = _ref_module()  # live where oracle/_ref has been built, else the kept set recorded from it (refpin.py)
     n, nlabels = 3000, 40
     boxes, _, _ = _boxes(4242, n, nlabels)
     g = torch.Generator().manual_seed(5)
@@ -306,9 +307,10 @@ def test_ml_nms_score_ties_equal_reference_kernel(dev):
     labels = torch.cat([torch.randint(1, nlabels // 2 + 1, (m,), generator=g),
                         torch.randint(nlabels // 2 + 1, nlabels + 1, (m,), generator=g)]).float()   # ... on different labels
     boxes = boxes[: 2 * m]
-    want = ref.ml_nms(boxes.to(dev), scores.to(dev), labels.to(dev), 0.6).cpu()
+    want = pinned("ref_ml_nms_score_ties", lambda: ref.ml_nms(boxes.to(dev), scores.to(dev), labels.to(dev), 0.6).cpu(), full=True,
+                  live=ref is not None)
     got = ops.ml_nms(boxes.to(dev), scores.to(dev), labels.to(dev), 0.6).cpu()
-    assert torch.equal(got, want)
+    assert equal(got, want)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

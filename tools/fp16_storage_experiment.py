@@ -5,7 +5,7 @@ The fp32 oracle tower (oracle/restate.py, same seed/weights as test_vldyhead_tow
 stream rounded to fp16 after every stage (what any fp16 pipeline — including the reference under its own fp16 autocast,
 engine/trainer.py:119-120 — stores), everything else in fp32.  Prints/records the deviation of the logits.
 
-    python -m tools.fp16_storage_experiment > profiles/r02_fp16_storage_amplification.json
+    python -m tools.fp16_storage_experiment > fp16_storage_amplification.json
 """
 import json
 import os

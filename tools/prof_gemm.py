@@ -62,10 +62,10 @@ for i, (M, N, K, what) in enumerate(SHAPES):
     torch.cuda.synchronize()
     cms = e0.elapsed_time(e1) / 10
     for _ in range(3):
-        ops.gemm(a, b, out=c, impl=ops.IMPL_TCGEN05_ONESHOT)
+        ops.gemm(a, b, out=c, impl=ops.IMPL_TC_ONESHOT)
     e0.record()
     for _ in range(10):
-        ops.gemm(a, b, out=c, impl=ops.IMPL_TCGEN05_ONESHOT)
+        ops.gemm(a, b, out=c, impl=ops.IMPL_TC_ONESHOT)
     e1.record()
     torch.cuda.synchronize()
     oms = e0.elapsed_time(e1) / 10

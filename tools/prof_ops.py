@@ -1,7 +1,7 @@
 """Single hot operators at the bench shape (B=8, 800x1344), for ncu captures and CUDA-event timings:
 
     python tools/prof_ops.py swin_fc1|swin_fc2|swin_qkv|swin_proj|dcn|conv_off|ln1 [reps]
-    ncu --set full --import-source on --clock-control none -k regex:gemm_tcp -c 1 -o gpurun_out/x python tools/prof_ops.py swin_fc1 1
+    ncu --set full --import-source on --clock-control none -k regex:gemm_wg -c 1 -o prof_swin_fc1 python tools/prof_ops.py swin_fc1 1
 
 Prints the median CUDA-event time per call (256 MiB L2 flush between calls) with the algorithmic GB/s and TFLOP/s.
 """

@@ -1,7 +1,7 @@
 """Reduce an ncu launch list (``--metrics gpu__time_duration.sum[,dram__bytes_read.sum,dram__bytes_write.sum] --csv``) of a
-bench command to ONE forward: per-kernel share of the step, and the DRAM traffic of the tcgen05 kernels.
+bench command to ONE forward: per-kernel share of the step, and the DRAM traffic of the tensor-core kernels.
 
-    python tools/summarize_launches.py gpurun_out/r02_launches.csv profiles/r02_launch_summary.csv [profiles/r02_traffic.json]
+    python tools/summarize_launches.py <launches.csv> <summary.csv> [<traffic.json>]
 
 One forward = the launches from the LAST ``patchify4_kernel`` (the first kernel of a forward) to the end of the list or the next
 one.  Per-launch times under ncu are cold-cache and serialised: only the kernel SHARES compare with bench.py.
@@ -66,11 +66,11 @@ def main():
         for k, (t, n, d) in sorted(agg.items(), key=lambda kv: -kv[1][0]):
             f.write(f"{100 * t / total:.1f},{t / 1e6:.3f},{n},{d / 1e6:.1f},{k}\n")
     if len(sys.argv) > 3:
-        gem = [e for e in fw if any(k in e["name"] for k in ("gemm_tcp_kernel", "dcn_conv_kernel", "biattn_image_kernel", "biattn_text_kernel"))]
+        gem = [e for e in fw if any(k in e["name"] for k in ("gemm_wg_kernel", "dcn_conv_kernel", "biattn_image_kernel", "biattn_text_kernel"))]
         d = sum(byts(e, "dram__bytes_read.sum") + byts(e, "dram__bytes_write.sum") for e in gem)
-        json.dump({"kernel": "tcgen05 kernels (gemm_tcp, dcn_conv, biattn_image, biattn_text: all launches of one forward)", "launches": len(gem),
+        json.dump({"kernel": "tensor-core kernels (gemm_wg, dcn_conv, biattn_image, biattn_text: all launches of one forward)", "launches": len(gem),
                    "dram_bytes_per_step": d, "dram_bytes_per_launch": d / max(1, len(gem)),
-                   "source": f"ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum over the tcgen05 launches of one forward ({src})"},
+                   "source": f"ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum over the tensor-core launches of one forward ({src})"},
                   open(sys.argv[3], "w"), indent=1)
 
 
