@@ -39,9 +39,9 @@ extern "C" {
 #define MQDET_VEC_PER_COL 2 /* length N */
 #define MQDET_VEC_PER_ROW 3 /* length M */
 
-#define MQDET_GEMM_IMPL_TC 0      /* TMA + wgmma, warp-specialised, one tile per CTA (product path) */
+#define MQDET_GEMM_IMPL_TC 0      /* TMA + wgmma, warp-specialised, persistent: min(tiles, SMs) CTAs (product path) */
 #define MQDET_GEMM_IMPL_SIMT 1    /* plain shared-memory tiled fp32-FMA kernel (validation only) */
-#define MQDET_GEMM_IMPL_TC_ONESHOT 2 /* the same tensor-core kernel (value kept so that callers selecting it stay valid) */
+#define MQDET_GEMM_IMPL_TC_ONESHOT 2 /* the same tensor-core kernel launched with one CTA per tile (bit-identical results) */
 
 const char* mqdet_last_error(void);
 int mqdet_version(void);

@@ -2,12 +2,16 @@
 //
 //   D[z][m,n] = epi( sum_k A[z][m,k] * B[z][n,k] )      (both operands K-contiguous: "TN")
 //
-// Product kernel (gemm_wg_kernel): warp-specialised, one 128 x BN output tile per CTA (BN = 64 or 128).
-//   warpgroup 0    : TMA producer — one thread issues cp.async.bulk.tensor (4-D maps, 128B swizzle) into a STAGES-deep ring
+// Product kernel (gemm_wg_kernel): warp-specialised and persistent, 128 x BN output tiles (BN = 64 or 128), one CTA per SM
+// walking a static tile schedule (n-tiles fastest, so the CTAs running side by side share the A row-panel through L2).
+//   warpgroup 0    : TMA producer — one thread issues cp.async.bulk.tensor (4-D maps, 128B swizzle) into a STAGES-deep ring,
+//                                   running ahead into the next tile's k-blocks while the consumers finish the current one
+//                                   (setmaxnreg hands its registers to the consumers)
 //   warpgroups 1-2 : consumers    — rows 0-63 / 64-127 of the tile: wgmma.m64nBNk16 from the swizzled ring (fp32
 //                                   accumulators in registers, one commit group per k-block, the previous k-block's slot
-//                                   released as soon as its group retires), then the epilogue straight from the fragments
-// The grid runs n-tiles fastest so the A row-panel is shared through L2.
+//                                   released as soon as its group retires), then the epilogue: fragments -> fp32 shared staging
+//                                   -> a rolled loop over rows (consecutive threads on consecutive columns: coalesced
+//                                   residual loads and output stores)
 //
 // Validation kernel (gemm_simt_kernel): plain 64x64 shared-memory tiled FMA kernel with the same
 // epilogue, used by the tests to cross-check the tensor-core path (never by the product path).
@@ -100,8 +104,40 @@ struct WgCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int PITCH = BN + 8;  // fp32 staging row pitch: fragment writes (8 rows x 32 B per warp) are conflict-free
+  static constexpr int OUT_BYTES = 64 * PITCH * 4;  // one consumer warpgroup's 64 x BN accumulators
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * OUT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
+
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void sts64f(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float2 lds64f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+
+// Static persistent schedule: tile t -> (batch z, m-tile, n-tile), n-tiles fastest so the CTAs running side by side share
+// their A row-panels through L2.
+struct TileIdx {
+  int n_tile, m_tile, z1, z2;
+};
+__device__ __forceinline__ TileIdx tile_idx(int t, int n_tiles, int m_tiles, int nb1) {
+  TileIdx r;
+  const int per_z = n_tiles * m_tiles;
+  const int z = t / per_z, rem = t - z * per_z;
+  r.m_tile = rem / n_tiles;
+  r.n_tile = rem - r.m_tile * n_tiles;
+  r.z1 = z % nb1;
+  r.z2 = z / nb1;
+  return r;
+}
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
@@ -111,22 +147,26 @@ __device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, ui
     wgmma_ss_m64n64_kk(acc, da, db, 1);
 }
 
-// 128 x 64 tiles: two CTAs per SM (96 KB of shared memory each), so one CTA's epilogue overlaps the other's main loop
+// Persistent: CTA c computes tiles c, c + gridDim.x, ... (static schedule, no device-side counters, so a captured graph
+// replays without resets).  The producer thread runs ahead through the ring into the next tile's k-blocks while the
+// consumers run the current tile's epilogue; the accumulators live in the consumers' registers, so a ring slot is the only
+// resource the two sides hand over.  gridDim.x = number of tiles gives one tile per CTA (MQDET_GEMM_IMPL_TC_ONESHOT).
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(384, BN == 128 ? 1 : 2) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma_a,
-                                                                        const __grid_constant__ CUtensorMap tma_b, const GemmP p) {
+__global__ void __launch_bounds__(384, 1) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma_a,
+                                                         const __grid_constant__ CUtensorMap tma_b, const GemmP p) {
   using Cfg = WgCfg<BN, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte alignment.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint8_t* smem_c = smem + STAGES * Cfg::STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + 2 * Cfg::OUT_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-  const int n_tile = blockIdx.x, m_tile = blockIdx.y;
-  const int z1 = blockIdx.z % p.nb1, z2 = blockIdx.z / p.nb1;
+  const int n_tiles = (int)((p.N + BN - 1) / BN), m_tiles = (int)((p.M + BM - 1) / BM);
+  const int tiles = n_tiles * m_tiles * p.nb1 * p.nb2;
   const int num_kb = (int)((p.K + BK - 1) / BK);
 
   if (threadIdx.x == 0) {
@@ -141,62 +181,104 @@ __global__ void __launch_bounds__(384, BN == 128 ? 1 : 2) gemm_wg_kernel(const _
   __syncthreads();
 
   if (wg == 0) {
+    setmaxnreg_dec<40>();
     if (tid == 0) {
-      const int az1 = p.a_bcast1 ? 0 : z1, az2 = p.a_bcast2 ? 0 : z2;
-      const int bz1 = p.b_bcast1 ? 0 : z1, bz2 = p.b_bcast2 ? 0 : z2;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
-        mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-        tma_load_4d(smem_a + s * Cfg::A_BYTES, &tma_a, &full_bar[s], kb * BK, m_tile * BM, az1, az2);
-        tma_load_4d(smem_b + s * Cfg::B_BYTES, &tma_b, &full_bar[s], kb * BK, n_tile * BN, bz1, bz2);
+      int it = 0;  // k-blocks issued by this CTA, over all its tiles
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const TileIdx ti = tile_idx(t, n_tiles, m_tiles, p.nb1);
+        const int az1 = p.a_bcast1 ? 0 : ti.z1, az2 = p.a_bcast2 ? 0 : ti.z2;
+        const int bz1 = p.b_bcast1 ? 0 : ti.z1, bz2 = p.b_bcast2 ? 0 : ti.z2;
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
+          mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+          tma_load_4d(smem_a + s * Cfg::A_BYTES, &tma_a, &full_bar[s], kb * BK, ti.m_tile * BM, az1, az2);
+          tma_load_4d(smem_b + s * Cfg::B_BYTES, &tma_b, &full_bar[s], kb * BK, ti.n_tile * BN, bz1, bz2);
+        }
       }
     }
     return;
   }
-  const int g = wg - 1;  // rows 64 g .. 64 g + 63 of the tile
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(&full_bar[s], (kb / STAGES) & 1);
-    const uint32_t a_addr = smem_u32(smem_a + s * Cfg::A_BYTES) + g * (64 * 128);
-    const uint32_t b_addr = smem_u32(smem_b + s * Cfg::B_BYTES);
-    wgmma_fence_acc(acc);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(acc, wg_desc_k_sw128(a_addr + k * 32), wg_desc_k_sw128(b_addr + k * 32));
-    wgmma_commit();
-    wgmma_wait<1>();  // the previous k-block's group has retired: its slot may be refilled
-    wgmma_fence_acc(acc);
-    if (kb > 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
-  }
-  wgmma_wait<0>();
-  wgmma_fence_acc(acc);
-
-  // ---- epilogue from the accumulator fragments: bias / act / clamp / gate / residual, column pairs per store ----
+  setmaxnreg_inc<232>();
+  const int g = wg - 1;  // rows 64 g .. 64 g + 63 of every tile
   float gate_s = 1.f;
   if (p.gate_mode == MQDET_VEC_SCALAR) gate_s = p.gate_tanh ? tanhf(p.gate[0]) : p.gate[0];
-  const long row0 = (long)m_tile * BM + g * 64, col0 = (long)n_tile * BN;
+  const uint32_t stage_c = smem_u32(smem_c + g * Cfg::OUT_BYTES);
+  int it = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    const TileIdx ti = tile_idx(t, n_tiles, m_tiles, p.nb1);
+    const int z1 = ti.z1, z2 = ti.z2;
+    float acc[BN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; i += 2) {
-    const long row = row0 + wg_row(tid, i), col = col0 + wg_col(tid, i);
-    if (row >= p.M || col >= p.N) continue;
-    const float v0 = epi_one(p, acc[i], row, col, z1, z2, gate_s);
-    if (col + 1 < p.N) {
-      const float v1 = epi_one(p, acc[i + 1], row, col + 1, z1, z2, gate_s);
-      if (p.vec2) {
-        const long off = z1 * p.c_b1 + z2 * p.c_b2 + row * p.ldc + col;
-        if (p.c_dtype == MQDET_F32)
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + off) = make_float2(v0, v1);
-        else
-          *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.C) + off) = __floats2half2_rn(v0, v1);
-        continue;
-      }
-      store_one(p, v1, row, col + 1, z1, z2);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full_bar[s], (it / STAGES) & 1);
+      const uint32_t a_addr = smem_u32(smem_a + s * Cfg::A_BYTES) + g * (64 * 128);
+      const uint32_t b_addr = smem_u32(smem_b + s * Cfg::B_BYTES);
+      wgmma_fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(acc, wg_desc_k_sw128(a_addr + k * 32), wg_desc_k_sw128(b_addr + k * 32));
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's group has retired: its slot may be refilled
+      wgmma_fence_acc(acc);
+      if (kb > 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
-    store_one(p, v0, row, col, z1, z2);
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    mbar_arrive(&empty_bar[(it - 1) % STAGES]);  // the tile's last slot: the producer is already filling the next tile's
+
+    // ---- epilogue: fragments -> fp32 staging -> rows walked by consecutive threads (coalesced residual loads and stores).
+    // The per-element epilogue is not unrolled over the fragments: 64 inlined copies of it (erff, tanhf, every option's
+    // branch) made the kernel's code far larger than the instruction cache.
+    const long row0 = (long)ti.m_tile * BM + g * 64, col0 = (long)ti.n_tile * BN;
+    named_bar_sync(1 + g, 128);  // the previous tile's staging reads are done
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2)
+      sts64f(stage_c + (wg_row(tid, i) * Cfg::PITCH + wg_col(tid, i)) * 4, acc[i], acc[i + 1]);
+    named_bar_sync(1 + g, 128);
+    constexpr int TPR = BN / 2, RPI = 128 / TPR, U = 4;  // threads per row (two columns each), rows per pass, passes per batch
+    const int cc = 2 * (tid % TPR);
+    const long col = col0 + cc;
+    if (col >= p.N) continue;
+    const bool two = col + 1 < p.N;
+#pragma unroll 1
+    for (int r0 = tid / TPR; r0 < 64; r0 += RPI * U) {
+      float2 a[U], rv[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {  // every load of the batch is issued before the first store
+        const int r = r0 + u * RPI;
+        const long row = row0 + r;
+        a[u] = lds64f(stage_c + (r * Cfg::PITCH + cc) * 4);
+        rv[u] = make_float2(0.f, 0.f);
+        if (p.R && row < p.M) {
+          rv[u].x = ld_residual(p, row, col, z1, z2);
+          if (two) rv[u].y = ld_residual(p, row, col + 1, z1, z2);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const long row = row0 + r0 + u * RPI;
+        if (row >= p.M) break;
+        float v0 = epi_pre(p, a[u].x, row, col, z1, z2, gate_s);
+        if (p.R) v0 += rv[u].x;
+        if (two) {
+          float v1 = epi_pre(p, a[u].y, row, col + 1, z1, z2, gate_s);
+          if (p.R) v1 += rv[u].y;
+          if (p.vec2) {
+            const long off = z1 * p.c_b1 + z2 * p.c_b2 + row * p.ldc + col;
+            if (p.c_dtype == MQDET_F32)
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + off) = make_float2(v0, v1);
+            else
+              *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.C) + off) = __floats2half2_rn(v0, v1);
+            continue;
+          }
+          store_one(p, v1, row, col + 1, z1, z2);
+        }
+        store_one(p, v0, row, col, z1, z2);
+      }
+    }
   }
 }
 
@@ -251,7 +333,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const GemmP p) {
 // ---------------------------------------------------------------------------------------------
 // make_operand_map / num_sms / ensure_dyn_smem: capi.cu (shared with the other TMA kernels; tensor maps are cached)
 template <int BN, int STAGES>
-static int launch_wg(const GemmP& p0, cudaStream_t st) {
+static int launch_wg(const GemmP& p0, bool persistent, cudaStream_t st) {
   using Cfg = WgCfg<BN, STAGES>;
   GemmP p = p0;
   CUtensorMap ma, mb;
@@ -264,7 +346,9 @@ static int launch_wg(const GemmP& p0, cudaStream_t st) {
            (reinterpret_cast<uintptr_t>(p.C) % (4 * (3 - al))) == 0;
   rc = ensure_dyn_smem(reinterpret_cast<const void*>(&gemm_wg_kernel<BN, STAGES>), Cfg::SMEM_BYTES);
   if (rc) return rc;
-  dim3 grid(cdiv(p.N, BN), cdiv(p.M, BM), p.nb1 * p.nb2);
+  const long tiles = (long)cdiv(p.N, BN) * cdiv(p.M, BM) * p.nb1 * p.nb2;
+  MQ_REQUIRE(tiles < (1l << 31), "gemm: %ld tiles", tiles);
+  const int grid = persistent ? (int)(tiles < num_sms() ? tiles : num_sms()) : (int)tiles;
   gemm_wg_kernel<BN, STAGES><<<grid, 384, Cfg::SMEM_BYTES, st>>>(ma, mb, p);
   return check_launch("gemm_wg_kernel");
 }
@@ -308,6 +392,7 @@ extern "C" int mqdet_gemm_f16(const mqdet_gemm_args* a, int impl, void* stream) 
   MQ_REQUIRE(((uintptr_t)a->A % 16) == 0 && ((uintptr_t)a->B % 16) == 0, "gemm: A/B must be 16-byte aligned");
   // 128-wide tiles when they still give every SM a tile, 64-wide ones (two CTAs per SM) otherwise
   const long tiles128 = (long)cdiv(p.M, BM) * cdiv(p.N, 128) * p.nb1 * p.nb2;
-  if (p.N > 64 && tiles128 >= num_sms()) return launch_wg<128, 4>(p, st);
-  return launch_wg<64, 4>(p, st);
+  const bool persistent = impl == MQDET_GEMM_IMPL_TC;
+  if (p.N > 64 && tiles128 >= num_sms()) return launch_wg<128, 4>(p, persistent, st);
+  return launch_wg<64, 6>(p, persistent, st);
 }
