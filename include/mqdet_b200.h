@@ -478,6 +478,30 @@ int mqdet_clip_coef(const float* partials, int64_t count, float max_norm, float*
 int mqdet_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float beta1, float beta2,
                      float eps, float weight_decay, int64_t step, const float* grad_scale_dev, void* stream);
 
+/* ---- ATSS target assignment and the pre-training detection losses (modeling/rpn/loss.py ATSSLossComputation :519-1201) ---------
+ * One anchor per location, generated from the level table (level_hw [nlev][2], strides [nlev], base_anchors [nlev][4]) exactly as
+ * mqdet_atss_candidates does.  GTs come as a fixed-capacity pack: gt_boxes f32 [B][Gmax][4] (xyxy), gt_labels i32 [B][Gmax],
+ * gt_count i32 [B] (device; entries >= gt_count[b] are ignored), gt_tokens f32 [B][Gmax][T] (the positive_map rows).
+ *   mqdet_atss_assign : match i32 [B][N] = assigned GT or -1; img_stats f32 [B][2] (optional) = (positives, sum of centerness targets)
+ *                       per image; norm f32 [4] = the batch totals twice: [0:2] is what data-parallel ranks all-reduce (sum) before
+ *                       mqdet_atss_loss, [2:4] stays this rank's.  Per-level top-k ties go to the lower anchor index; an anchor claimed
+ *                       by several GTs goes to the highest IoU, then the lowest GT index.  workspace: mqdet_atss_assign_workspace_bytes
+ *   mqdet_atss_loss   : losses f32 [4] = (loss_reg, loss_centerness, loss_dot_product_token, loss_cls = 0); d_logits f32 [B][N][T] and
+ *                       d_reg_ctr f32 [B][N][5] = their gradient w.r.t. logits [B][N][T] and the raw box / centerness output reg_ctr
+ *                       [B][N][5] (channels 0-3 before the per-level Scale reg_scales [nlev]); text_mask f32 [B][T] (> 0 = in use) or
+ *                       NULL; world = number of ranks that summed norm[0:2].  No host synchronisation; reductions are deterministic.
+ *                       workspace: mqdet_atss_loss_workspace_floats */
+int64_t mqdet_atss_assign_workspace_bytes(int64_t B, int64_t N);
+int mqdet_atss_assign(const float* gt_boxes, const int32_t* gt_labels, const int32_t* gt_count, int64_t B, int64_t Gmax,
+                      const int32_t* level_hw, int64_t nlev, const float* strides, const float* base_anchors, int64_t topk, void* workspace,
+                      int32_t* match, float* img_stats, float* norm, void* stream);
+int64_t mqdet_atss_loss_workspace_floats(int64_t B, int64_t N);
+int mqdet_atss_loss(const float* logits, const float* reg_ctr, const int32_t* match, const float* gt_boxes, const int32_t* gt_labels,
+                    const float* gt_tokens, int64_t B, int64_t Gmax, int64_t T, const float* text_mask, const int32_t* level_hw, int64_t nlev,
+                    const float* strides, const float* base_anchors, const float* reg_scales, const float* norm, float world, float alpha,
+                    float gamma, float reg_weight, float token_weight, float* workspace, float* losses, float* d_logits, float* d_reg_ctr,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

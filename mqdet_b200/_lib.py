@@ -162,6 +162,13 @@ SIGNATURES = {
     "mqdet_clip_coef": (c_int, [c_void_p, c_int64, c_float, c_void_p, c_void_p]),
     "mqdet_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float, c_float, c_float, c_int64,
                                  c_void_p, c_void_p]),
+    "mqdet_atss_assign_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "mqdet_atss_assign": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p,
+                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_atss_loss_workspace_floats": (c_int64, [c_int64, c_int64]),
+    "mqdet_atss_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_float, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

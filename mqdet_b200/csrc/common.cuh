@@ -94,6 +94,48 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return 0.5f * x * (z < 0.f ? e : 2.f - e);
 }
 
+// ---- box coder / losses shared by the ATSS post-processing and the ATSS training losses -------------------------------
+constexpr float BOX_DECODE_CLAMP = 4.135166556742356f;  // log(1000 / 16)
+
+struct DecodedBox {
+  float x1, y1, x2, y2;
+  float pw, ph;  // decoded width / height before the -1 (exp(dw) * w): the gradient of x1/x2 w.r.t. dw is -+0.5 pw
+};
+// BoxCoder.decode (modeling/rpn/vldyhead.py:78-108), weights (10, 10, 5, 5), TO_REMOVE = 1: deltas p (after the level Scale)
+// applied to the anchor (ax1, ay1, ax2, ay2); dw / dh are clamped at BOX_DECODE_CLAMP.
+__device__ __forceinline__ DecodedBox box_decode(float p0, float p1, float p2, float p3, float ax1, float ay1, float ax2,
+                                                 float ay2) {
+  const float w = ax2 - ax1 + 1.f, h = ay2 - ay1 + 1.f;
+  const float cx = (ax2 + ax1) / 2.f, cy = (ay2 + ay1) / 2.f;
+  const float dx = p0 / 10.f, dy = p1 / 10.f;
+  const float dw = fminf(p2 / 5.f, BOX_DECODE_CLAMP), dh = fminf(p3 / 5.f, BOX_DECODE_CLAMP);
+  const float pcx = dx * w + cx, pcy = dy * h + cy;
+  const float pw = expf(dw) * w, ph = expf(dh) * h;
+  DecodedBox d;
+  d.x1 = pcx - 0.5f * (pw - 1.f);
+  d.y1 = pcy - 0.5f * (ph - 1.f);
+  d.x2 = pcx + 0.5f * (pw - 1.f);
+  d.y2 = pcy + 0.5f * (ph - 1.f);
+  d.pw = pw;
+  d.ph = ph;
+  return d;
+}
+
+// One element of token_sigmoid_binary_focal_loss (layers/sigmoid_focal_loss.py:130-171): logit x, target y ->
+// loss and d loss / d x.  alpha < 0: no alpha weighting.
+__device__ __forceinline__ void token_focal_elem(float x, float y, float alpha, float gamma, float& loss, float& dloss) {
+  const float p = 1.f / (1.f + expf(-x));
+  const float ce = fmaxf(x, 0.f) - x * y + log1pf(expf(-fabsf(x)));
+  const float pt = p * y + (1.f - p) * (1.f - y);
+  const float om = 1.f - pt;
+  const float mod = powf(om, gamma);
+  const float at = alpha >= 0.f ? alpha * y + (1.f - alpha) * (1.f - y) : 1.f;
+  loss = at * ce * mod;
+  // d/dx: ce' = p - y; (1 - pt)' = -(2y - 1) p (1 - p)
+  const float dmod = (om > 0.f) ? gamma * powf(om, gamma - 1.f) * (-(2.f * y - 1.f) * p * (1.f - p)) : 0.f;
+  dloss = at * ((p - y) * mod + ce * dmod);
+}
+
 // ---- mbarrier ------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));

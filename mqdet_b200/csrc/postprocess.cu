@@ -181,16 +181,8 @@ __global__ void __launch_bounds__(1024) atss_select_decode_kernel(const unsigned
     // anchor (anchor_generator.py:111-137): base window shifted by (x*stride, y*stride)
     const float sx = (float)(loc % Wl) * lv.stride[l], sy = (float)(loc / Wl) * lv.stride[l];
     const float ax1 = sx + lv.base[l][0], ay1 = sy + lv.base[l][1], ax2 = sx + lv.base[l][2], ay2 = sy + lv.base[l][3];
-    // BoxCoder.decode (vldyhead.py:78-108)
-    const float w = ax2 - ax1 + 1.f, h = ay2 - ay1 + 1.f;
-    const float cx = (ax2 + ax1) / 2.f, cy = (ay2 + ay1) / 2.f;
-    const float dx = r[0] * sc / 10.f, dy = r[1] * sc / 10.f;
-    const float clampv = 4.135166556742356f;  // log(1000/16)
-    const float dw = fminf(r[2] * sc / 5.f, clampv), dh = fminf(r[3] * sc / 5.f, clampv);
-    const float pcx = dx * w + cx, pcy = dy * h + cy;
-    const float pw = expf(dw) * w, ph = expf(dh) * h;
-    float x1 = pcx - 0.5f * (pw - 1.f), y1 = pcy - 0.5f * (ph - 1.f);
-    float x2 = pcx + 0.5f * (pw - 1.f), y2 = pcy + 0.5f * (ph - 1.f);
+    const DecodedBox d = box_decode(r[0] * sc, r[1] * sc, r[2] * sc, r[3] * sc, ax1, ay1, ax2, ay2);
+    float x1 = d.x1, y1 = d.y1, x2 = d.x2, y2 = d.y2;
     // clip_to_image(remove_empty=False), TO_REMOVE = 1
     x1 = fminf(fmaxf(x1, 0.f), img_w - 1.f);
     y1 = fminf(fmaxf(y1, 0.f), img_h - 1.f);

@@ -328,19 +328,7 @@ __global__ void __launch_bounds__(256) token_focal_loss_kernel(const float* __re
     const long b = i / NT;
     const int t = (int)(i % T);
     float l = 0.f, d = 0.f;
-    if (!text_mask || text_mask[b * T + t] > 0.f) {
-      const float x = logits[i], y = targets[i];
-      const float p = 1.f / (1.f + expf(-x));
-      const float ce = fmaxf(x, 0.f) - x * y + log1pf(expf(-fabsf(x)));
-      const float pt = p * y + (1.f - p) * (1.f - y);
-      const float om = 1.f - pt;
-      const float mod = powf(om, gamma);
-      const float at = alpha >= 0.f ? alpha * y + (1.f - alpha) * (1.f - y) : 1.f;
-      l = at * ce * mod;
-      // d/dx: ce' = p - y; (1 - pt)' = -(2y - 1) p (1 - p)
-      const float dmod = (om > 0.f) ? gamma * powf(om, gamma - 1.f) * (-(2.f * y - 1.f) * p * (1.f - p)) : 0.f;
-      d = at * ((p - y) * mod + ce * dmod);
-    }
+    if (!text_mask || text_mask[b * T + t] > 0.f) token_focal_elem(logits[i], targets[i], alpha, gamma, l, d);
     acc += l;
     if (dlogits) dlogits[i] = d * grad_scale;
   }

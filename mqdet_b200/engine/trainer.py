@@ -4,8 +4,11 @@ that touches a TRAINABLE parameter.
     reference step                                      here
     ------------------------------------------------    -------------------------------------------------------------------
     loss_dict = model(images, targets, captions, ...)    language backbone forward: ``QVBertModelTrain.forward`` (training kernels)
-      fusion tower, ATSS assignment, GIoU / centerness    NOT built (frozen modules; DESIGN.md §1 row f2) — the caller supplies
-      / token focal losses                                dL/d(hidden); ``ops.token_focal_loss`` gives loss + d(logits) on the device
+      fusion tower forward                                ``VLDyHead.forward_flat`` (inference kernels)
+      ATSS assignment, GIoU / centerness / token losses   ``VLDyHeadModule.forward_train_flat``: ``ops.atss_targets`` ->
+                                                          ``parallel.all_reduce_loss_normalizers`` -> ``ops.atss_loss`` = losses +
+                                                          d(logits), d(box / centerness output) on the device
+      backward through the frozen fusion tower            NOT built (DESIGN.md §1 row f2) — the caller supplies dL/d(hidden)
     scaler.scale(losses).backward()                      ``QVBertModelTrain.backward(d_hidden)`` -> gradients of all 119 trainable tensors
     DDP gradient all-reduce                               ``parallel.all_reduce_gradients`` (ONE flat NCCL all-reduce, averaged)
     clip_grad_norm_ + AdamW per parameter group           ``FusedAdamW.step`` (norm, clip coefficient, updates: all on the device)

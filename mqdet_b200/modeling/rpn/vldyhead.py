@@ -4,7 +4,8 @@ Drop-in for the hot-path slice of maskrcnn_benchmark/modeling/rpn/vldyhead.py: `
 (:155-247), ``BertEncoderLayer`` (:250-301), ``VLFuse`` (MHA-B, :364-574), ``VLDyHead`` (:594-900) with the
 reference's parameter names (``dyhead_tower.{3i,3i+1,3i+2}``, ``DyConv.{0,1,2}.{conv,bn}``, ``AttnConv.1``,
 ``relu.fc.{0,2}``, ``offset``, ``b_attn...``, ``dot_product_projection_text``, ``bias_lang``, ``bias0``, ``log_scale``,
-``scales.N.scale``, ``bbox_pred``, ``centerness``, ``cls_logits``), inference only.
+``scales.N.scale``, ``bbox_pred``, ``centerness``, ``cls_logits``); ``VLDyHeadModule`` also computes the ATSS training
+losses and their gradients at the head outputs (the tower itself has no backward here).
 
 Layout: the visual pyramid is ONE fp16 tensor [B, N, 256] (all levels concatenated, NHWC rows) through the whole
 tower; NCHW appears only at the reference-facing ``forward`` boundary.
@@ -337,8 +338,25 @@ class VLDyHead(nn.Module):
         return logits, bbox_reg, centerness, None, None, None, dots, None, None, fused_out
 
 
+_UNSHIPPED_LOSS_FLAGS = ("USE_CLASSIFICATION_LOSS", "USE_TOKEN_LOSS", "USE_CONTRASTIVE_ALIGN_LOSS", "USE_SHALLOW_CONTRASTIVE_LOSS",
+                         "USE_BACKBONE_SHALLOW_CONTRASTIVE_LOSS", "MLM_LOSS")
+
+
+def check_loss_config(cfg):
+    """The training losses are those of the MQ-GLIP pre-training configs (dot-product token loss, GIoU, centerness): refuse a
+    loss flag whose non-shipped value would add or change a term, never ignore it."""
+    fc = cfg.MODEL.DYHEAD.FUSE_CONFIG
+    for flag in _UNSHIPPED_LOSS_FLAGS:
+        if getattr(fc, flag, False):
+            raise NotImplementedError(f"FUSE_CONFIG.{flag}=True: only the MQ-GLIP pre-training losses (dot-product token focal loss, "
+                                      "GIoU, centerness) are implemented")
+    if not fc.USE_DOT_PRODUCT_TOKEN_LOSS:
+        raise NotImplementedError("FUSE_CONFIG.USE_DOT_PRODUCT_TOKEN_LOSS=False is not an MQ-GLIP configuration")
+
+
 class VLDyHeadModule(nn.Module):
-    """vldyhead.py:903-1077, inference branch: head -> anchors -> ATSS post-processing -> list[BoxList]."""
+    """vldyhead.py:903-1077: head -> anchors -> ATSS post-processing -> list[BoxList] at inference; in ``train()`` mode head ->
+    ATSS assignment -> losses + their gradients at the head outputs (``RPN_ONLY`` branch, :1017-1045)."""
 
     def __init__(self, cfg, **kwargs):
         super().__init__()
@@ -346,6 +364,7 @@ class VLDyHeadModule(nn.Module):
         self.head = VLDyHead(cfg)
         self._scales = None
         self._tokmap = None
+        self.last_train = None
 
     def _reg_scales(self):
         ps = [s.scale for s in self.head.scales]
@@ -380,6 +399,51 @@ class VLDyHeadModule(nn.Module):
         out["head"] = r
         return out
 
+    @torch.no_grad()
+    def forward_train_flat(self, pyr16, levels, image_sizes, lang_hidden, lang_masks, gt_pack):
+        """pyr16 [B,N,256] fp16 + the GT pack dict(boxes [B,Gmax,4] xyxy, labels [B,Gmax], count [B], tokens [B,Gmax,T]) ->
+        dict(losses fp32 [4] = (loss_reg, loss_centerness, loss_dot_product_token, loss_cls = 0), d_logits fp32 [B,N,T],
+        d_reg_ctr fp32 [B,N,5] (channels 0-3 w.r.t. the raw box output, before the frozen level Scale), head = the head outputs).
+        The loss normalisers are summed over the data-parallel ranks (one collective); nothing synchronises the host."""
+        import torch.distributed as dist
+        from ... import parallel
+        cfg = self.cfg
+        check_loss_config(cfg)
+        fc, atss = cfg.MODEL.DYHEAD.FUSE_CONFIG, cfg.MODEL.ATSS
+        r = self.head.forward_flat(pyr16, levels, lang_hidden, lang_masks)
+        strides, sizes = cfg.MODEL.RPN.ANCHOR_STRIDE[:levels.n], cfg.MODEL.RPN.ANCHOR_SIZES[:levels.n]
+        t = ops.atss_targets(gt_pack["boxes"], gt_pack["labels"], gt_pack["count"], levels, strides, sizes,
+                             topk=getattr(atss, "TOPK", 9))
+        parallel.all_reduce_loss_normalizers(t["norm"][:2])
+        world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        losses, d_logits, d_reg_ctr = ops.atss_loss(
+            r["dot_product_logits"], r["reg_ctr"], gt_pack["boxes"], gt_pack["labels"], gt_pack["count"], gt_pack["tokens"], levels,
+            strides, sizes, self._reg_scales()[:levels.n], lang_masks, targets=t, world=world, alpha=getattr(fc, "TOKEN_ALPHA", 0.25),
+            gamma=getattr(fc, "TOKEN_GAMMA", 2.0), reg_weight=getattr(atss, "REG_LOSS_WEIGHT", 2.0),
+            token_weight=getattr(fc, "DOT_PRODUCT_TOKEN_LOSS_WEIGHT", 1.0))
+        return {"losses": losses, "d_logits": d_logits, "d_reg_ctr": d_reg_ctr, "head": r}
+
+    @staticmethod
+    def pack_targets(targets, positive_map, T, device):
+        """list of BoxList (field ``labels``) + positive_map [sum G, T] (the reference trainer's inputs) -> the fixed-capacity GT pack
+        of ``forward_train_flat`` (Gmax = the largest GT count of the batch, at least 1)."""
+        counts = [len(t) for t in targets]
+        B, G = len(targets), max(counts + [1])
+        boxes = torch.zeros((B, G, 4), dtype=torch.float32, device=device)
+        labels = torch.zeros((B, G), dtype=torch.int32, device=device)
+        tokens = torch.zeros((B, G, T), dtype=torch.float32, device=device)
+        off = 0
+        for b, t in enumerate(targets):
+            g = counts[b]
+            if g:
+                boxes[b, :g] = t.convert("xyxy").bbox.to(device=device, dtype=torch.float32)
+                labels[b, :g] = t.get_field("labels").to(device=device, dtype=torch.int32)
+                tokens[b, :g] = positive_map[off:off + g].to(device=device, dtype=torch.float32)
+            off += g
+        if positive_map.shape[0] != off:
+            raise ValueError(f"positive_map has {positive_map.shape[0]} rows for {off} GT boxes")
+        return {"boxes": boxes, "labels": labels, "count": torch.tensor(counts, dtype=torch.int32).to(device), "tokens": tokens}
+
     @staticmethod
     def to_boxlists(det, num, image_sizes):
         """One device->host copy of the fixed-shape result, then BoxList(mode xyxy, fields labels/scores) per image."""
@@ -401,12 +465,21 @@ class VLDyHeadModule(nn.Module):
     @torch.no_grad()
     def forward(self, images, features, targets=None, language_dict_features=None, positive_map=None, captions=None,
                 swint_feature_c4=None):
-        """Reference signature: features = list of [B,256,h,w]; returns (list[BoxList], {}, fused_visual_features)."""
-        if self.training:
-            raise NotImplementedError("training (ATSS loss / backward) is SURVEY.md §8f")
+        """Reference signature: features = list of [B,256,h,w]; returns (list[BoxList], {}, fused_visual_features) at inference and
+        (None, {loss_reg, loss_centerness, loss_cls, loss_dot_product_token} as 0-dim device tensors, None) in ``train()`` mode, with
+        ``targets`` = list of BoxList (field ``labels``) and ``positive_map`` [sum G, T]; the gradients at the head outputs are in
+        ``self.last_train`` (see ``forward_train_flat``)."""
         sizes = images.image_sizes if hasattr(images, "image_sizes") else [tuple(images.shape[-2:])] * features[0].shape[0]
         levels = ops.get_levels([(f.shape[2], f.shape[3]) for f in features], features[0].device)
         v16 = ops.cast_f16(_flatten_levels(features))
+        if self.training:
+            hidden = language_dict_features["hidden"]
+            pack = self.pack_targets(targets, positive_map, hidden.shape[1], hidden.device)
+            out = self.forward_train_flat(v16, levels, sizes, hidden, language_dict_features["masks"], pack)
+            language_dict_features["hidden"] = out["head"]["hidden"]
+            self.last_train = out
+            l = out["losses"]
+            return None, {"loss_reg": l[0], "loss_centerness": l[1], "loss_cls": l[3], "loss_dot_product_token": l[2]}, None
         out = self.forward_flat(v16, levels, sizes, language_dict_features["hidden"], language_dict_features["masks"],
                                 positive_map)
         language_dict_features["hidden"] = out["head"]["hidden"]

@@ -816,6 +816,91 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
             "cand_labels": cl, "cand_totals": totals, "level_counts": lvl_counts, "level_keys": okey, "keep": keep}
 
 
+def _level_anchor_tables(strides, anchor_sizes, reg_scales=None):
+    import numpy as np
+    stride_h = np.ascontiguousarray(np.asarray(strides, dtype=np.float32))
+    base_h = np.ascontiguousarray(np.asarray([base_anchor(s, a) for s, a in zip(strides, anchor_sizes)], dtype=np.float32))
+    scale_h = None if reg_scales is None else np.ascontiguousarray(np.asarray(reg_scales, dtype=np.float32))
+    return stride_h, base_h, scale_h
+
+
+def _gt_pack(gt_boxes, gt_labels, gt_count, B):
+    _need_cuda(gt_boxes, gt_labels, gt_count)
+    if gt_boxes.dim() != 3 or gt_boxes.shape[0] != B or gt_boxes.shape[2] != 4:
+        raise ValueError(f"gt_boxes must be [B={B}, Gmax, 4]; got {tuple(gt_boxes.shape)}")
+    G = gt_boxes.shape[1]
+    if tuple(gt_labels.shape) != (B, G) or tuple(gt_count.shape) != (B,):
+        raise ValueError(f"gt_labels must be [B, Gmax] = {(B, G)} and gt_count [B]; got {tuple(gt_labels.shape)}, "
+                         f"{tuple(gt_count.shape)}")
+    return (gt_boxes.float().contiguous(), gt_labels.to(torch.int32).contiguous(), gt_count.to(torch.int32).contiguous(), G)
+
+
+def atss_targets(gt_boxes, gt_labels, gt_count, levels, strides, anchor_sizes, topk=9):
+    """ATSS target assignment (loss.py:655-832) for a fixed-capacity GT pack: gt_boxes [B, Gmax, 4] xyxy, gt_labels [B, Gmax],
+    gt_count [B] (device) -> dict(match int32 [B, N] (assigned GT, -1 = unmatched), img_stats fp32 [B, 2] (positives, sum of
+    centerness targets per image), norm fp32 [4] (the batch totals; ``norm[:2]`` is what data-parallel ranks all-reduce)).
+    All on the device, no host synchronisation."""
+    global launch_count
+    B = gt_count.shape[0]
+    gt_boxes, gt_labels, gt_count, G = _gt_pack(gt_boxes, gt_labels, gt_count, B)
+    dev = gt_boxes.device
+    stride_h, base_h, _ = _level_anchor_tables(strides, anchor_sizes)
+    N = levels.N
+    ws = torch.empty((int(load().mqdet_atss_assign_workspace_bytes(B, N)),), dtype=torch.uint8, device=dev)
+    match = torch.empty((B, N), dtype=torch.int32, device=dev)
+    img_stats = torch.empty((B, 2), dtype=torch.float32, device=dev)
+    norm = torch.empty((4,), dtype=torch.float32, device=dev)
+    check(load().mqdet_atss_assign(_ptr(gt_boxes), _ptr(gt_labels), _ptr(gt_count), B, G, levels.hw_ptr, levels.n,
+                                   stride_h.ctypes.data_as(ctypes.c_void_p), base_h.ctypes.data_as(ctypes.c_void_p), int(topk),
+                                   _ptr(ws), _ptr(match), _ptr(img_stats), _ptr(norm), _stream()), "atss_assign")
+    launch_count += 4
+    return {"match": match, "img_stats": img_stats, "norm": norm}
+
+
+def atss_loss(logits, reg_ctr, gt_boxes, gt_labels, gt_count, gt_tokens, levels, strides, anchor_sizes, reg_scales, text_mask=None, *,
+              targets=None, world=1, topk=9, alpha=0.25, gamma=2.0, reg_weight=2.0, token_weight=1.0):
+    """The MQ-GLIP pre-training detection losses (loss.py:850-1201 with the shipped flags) and their gradients at the head outputs.
+
+    logits fp32 [B, N, T] (dot-product token logits), reg_ctr fp32 [B, N, 5] (raw box / centerness GEMM output, before the per-level
+    ``reg_scales``), the GT pack of ``atss_targets`` plus gt_tokens [B, Gmax, T] (positive_map rows), text_mask [B, T] or None ->
+    (losses fp32 [4] = (loss_reg, loss_centerness, loss_dot_product_token, loss_cls = 0), d_logits fp32 [B, N, T],
+    d_reg_ctr fp32 [B, N, 5]).  ``targets``: the result of ``atss_targets`` (its ``norm[:2]`` summed over ``world`` ranks), else
+    computed here for one rank.  All on the device, no host synchronisation: capturable in a CUDA graph at a fixed Gmax."""
+    global launch_count
+    _need_cuda(logits, reg_ctr, gt_tokens, text_mask)
+    B, N, T = logits.shape
+    if N != levels.N or tuple(reg_ctr.shape) != (B, N, 5):
+        raise ValueError(f"logits [B, N={levels.N}, T] and reg_ctr [B, N, 5] required; got {tuple(logits.shape)}, "
+                         f"{tuple(reg_ctr.shape)}")
+    for t in (logits, reg_ctr):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise _lib.MqdetError("atss_loss: logits / reg_ctr must be contiguous fp32")
+    gt_boxes, gt_labels, gt_count, G = _gt_pack(gt_boxes, gt_labels, gt_count, B)
+    if tuple(gt_tokens.shape) != (B, G, T):
+        raise ValueError(f"gt_tokens must be [B, Gmax, T] = {(B, G, T)}; got {tuple(gt_tokens.shape)}")
+    if text_mask is not None and tuple(text_mask.shape) != (B, T):
+        raise ValueError(f"text_mask must be [B, T] = {(B, T)}; got {tuple(text_mask.shape)}")
+    if targets is None:
+        targets = atss_targets(gt_boxes, gt_labels, gt_count, levels, strides, anchor_sizes, topk=topk)
+    dev = logits.device
+    tok = gt_tokens.float().contiguous()
+    tm = None if text_mask is None else text_mask.float().contiguous()
+    stride_h, base_h, scale_h = _level_anchor_tables(strides, anchor_sizes, reg_scales)
+    ws = torch.empty((int(load().mqdet_atss_loss_workspace_floats(B, N)),), dtype=torch.float32, device=dev)
+    losses = torch.empty((4,), dtype=torch.float32, device=dev)
+    d_logits = torch.empty_like(logits)
+    d_reg_ctr = torch.empty_like(reg_ctr)
+    with _Timed("atss_loss", 0.0, 8.0 * B * N * T + 40.0 * B * N):
+        check(load().mqdet_atss_loss(_ptr(logits), _ptr(reg_ctr), _ptr(targets["match"]), _ptr(gt_boxes), _ptr(gt_labels), _ptr(tok), B, G,
+                                     T, _ptr(tm), levels.hw_ptr, levels.n, stride_h.ctypes.data_as(ctypes.c_void_p),
+                                     base_h.ctypes.data_as(ctypes.c_void_p), scale_h.ctypes.data_as(ctypes.c_void_p),
+                                     _ptr(targets["norm"]), float(world), float(alpha), float(gamma), float(reg_weight),
+                                     float(token_weight), _ptr(ws), _ptr(losses), _ptr(d_logits), _ptr(d_reg_ctr), _stream()),
+              "atss_loss")
+    launch_count += 3
+    return losses, d_logits, d_reg_ctr
+
+
 def anchors(grid_h, grid_w, stride, size, img_w, img_h, device):
     """Anchors [H*W, 4] + visibility [H*W] of one level (anchor_generator.py:72-109)."""
     import numpy as np

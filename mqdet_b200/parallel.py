@@ -87,6 +87,16 @@ def all_gather_chunks(packed_local, num_chunks, group=None):
     return out.index_select(0, idx)
 
 
+def all_reduce_loss_normalizers(buf, group=None):
+    """The ATSS loss normalisers (number of positives, sum of centerness targets; loss.py:1149-1151, :1188) summed over the ranks
+    in place with ONE collective, between the target assignment and the losses: ``buf`` = ``ops.atss_targets(...)["norm"][:2]``
+    (a view: the rank-local copies in ``norm[2:]`` stay untouched).  Identity when no process group is initialised."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return buf
+    dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
+    return buf
+
+
 def all_reduce_gradients(grads, group=None, average=True):
     """Data-parallel gradient exchange of the modulated pre-training (the reference wraps the model in DistributedDataParallel,
     tools/train_net.py:96-103; only the ~45.7 M GCP / PreSelect parameters carry gradients): ALL gradient tensors of a step are packed
