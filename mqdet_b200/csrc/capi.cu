@@ -113,7 +113,8 @@ int make_operand_map(CUtensorMap* map, const void* ptr, long rows, long K, long 
 }
 
 // 4-D map over an OUTPUT viewed as [b2][b1][M][N] (c_dtype MQDET_F16 / MQDET_F32); box = [1][1][128 rows][128 bytes],
-// 128B swizzle (TMA store; the unit clips the M / N edges).
+// 128B swizzle (the GEMM's TMA-store epilogue; the unit clips the M / N edges).  The caller guarantees a 16-byte aligned base,
+// ldc and the batch strides of batch dims > 1 multiples of 16 bytes; a batch dim of size 1 gets a harmless stride.
 int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2) {
   const MapKey key = {{(uint64_t)(uintptr_t)C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc, (uint64_t)nb1, (uint64_t)c_b1,
                        (uint64_t)nb2, (uint64_t)c_b2, (uint64_t)c_dtype, 0x200u}};

@@ -227,19 +227,16 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* s
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-__device__ __forceinline__ void tma_store_commit_and_wait_read1() {  // leave the newest group in flight
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-  asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-}
 __device__ __forceinline__ void tma_store_commit() {
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// the shared-memory sources of every committed store have been read (the staging may be overwritten)
 __device__ __forceinline__ void tma_store_wait_read_all() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
-__device__ __forceinline__ void tma_store_commit_and_wait_read() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+// every committed store has completed
+__device__ __forceinline__ void tma_store_wait_all() {
+  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 // ---- wgmma (sm_90a warpgroup MMA) -----------------------------------------------------------
