@@ -102,6 +102,14 @@ int mqdet_layernorm(const void* x, int in_dtype, int64_t ldx, const float* gamma
                     float eps, int64_t rows, int64_t D, void* out16, void* out32, int64_t ldo,
                     int64_t zero_row_period, void* stream);
 
+/* The MLP half of a Swin block (swint.py:240-241) in one kernel, for C = 96 / 192:
+ *   out[r] = x[r] + fc2(GELU(fc1(LN(x[r]))))
+ * x, out: fp32 [rows][C] contiguous, 16-byte aligned, not overlapping; ln_w / ln_b: fp32 [C]; w1: fp16 [4C][C], b1: fp32 [4C];
+ * w2: fp16 [C][4C], b2: fp32 [C] (nn.Linear layouts).  Bit-identical to mqdet_layernorm (fp16 out) -> mqdet_gemm_f16 (bias +
+ * GELU, fp16 out) -> mqdet_gemm_f16 (bias + fp32 residual x, fp32 out). */
+int mqdet_swin_mlp_f16(const float* x, int64_t rows, int64_t C, const float* ln_w, const float* ln_b, float eps,
+                       const void* w1, const float* b1, const void* w2, const float* b2, float* out, void* stream);
+
 /* residual add + LayerNorm:  y = LN(a + b).  a,b fp32 [rows, D]; writes fp32 and/or fp16. */
 int mqdet_add_layernorm(const float* a, const float* b, const float* gamma, const float* beta, float eps,
                         int64_t rows, int64_t D, float* out32, void* out16, float clamp, void* stream);

@@ -44,6 +44,8 @@ SIGNATURES = {
     "mqdet_gemm_f16": (c_int, [POINTER(GemmArgs), c_int, c_void_p]),
     "mqdet_layernorm": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p, c_float, c_int64, c_int64, c_void_p,
                                 c_void_p, c_int64, c_int64, c_void_p]),
+    "mqdet_swin_mlp_f16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_void_p]),
     "mqdet_add_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int64, c_int64, c_void_p,
                                     c_void_p, c_float, c_void_p]),
     "mqdet_gcp_sparse_attn": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,

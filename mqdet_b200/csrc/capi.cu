@@ -112,12 +112,14 @@ int make_operand_map(CUtensorMap* map, const void* ptr, long rows, long K, long 
   return MQDET_OK;
 }
 
-// 4-D map over an OUTPUT viewed as [b2][b1][M][N] (c_dtype MQDET_F16 / MQDET_F32); box = [1][1][128 rows][128 bytes],
-// 128B swizzle (the GEMM's TMA-store epilogue; the unit clips the M / N edges).  The caller guarantees a 16-byte aligned base,
-// ldc and the batch strides of batch dims > 1 multiples of 16 bytes; a batch dim of size 1 gets a harmless stride.
-int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2) {
+// 4-D map over an OUTPUT viewed as [b2][b1][M][N] (c_dtype MQDET_F16 / MQDET_F32); box = [1][1][box_rows][128 bytes],
+// 128B swizzle (the TMA-store epilogues of the GEMM (128 rows) and swin_mlp (64 rows); the unit clips the M / N edges).  The
+// caller guarantees a 16-byte aligned base, ldc and the batch strides of batch dims > 1 multiples of 16 bytes; a batch dim of
+// size 1 gets a harmless stride.
+int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2,
+                   int box_rows) {
   const MapKey key = {{(uint64_t)(uintptr_t)C, (uint64_t)M, (uint64_t)N, (uint64_t)ldc, (uint64_t)nb1, (uint64_t)c_b1,
-                       (uint64_t)nb2, (uint64_t)c_b2, (uint64_t)c_dtype, 0x200u}};
+                       (uint64_t)nb2, (uint64_t)c_b2, (uint64_t)c_dtype, 0x200u | ((uint64_t)box_rows << 12)}};
   if (const CUtensorMap* hit = g_maps.find(key)) {
     *map = *hit;
     return MQDET_OK;
@@ -128,7 +130,7 @@ int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long 
   cuuint64_t dims[4] = {(cuuint64_t)N, (cuuint64_t)M, (cuuint64_t)nb1, (cuuint64_t)nb2};
   cuuint64_t strides[3] = {(cuuint64_t)ldc * es, (cuuint64_t)(nb1 > 1 ? c_b1 : ldc * M) * es,
                            (cuuint64_t)(nb2 > 1 ? c_b2 : ldc * M) * es};
-  cuuint32_t box[4] = {(cuuint32_t)(128 / es), 128u, 1, 1};
+  cuuint32_t box[4] = {(cuuint32_t)(128 / es), (cuuint32_t)box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(map, c_dtype == MQDET_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, C, dims,
                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,

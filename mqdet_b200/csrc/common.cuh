@@ -53,7 +53,8 @@ static inline int fill_levels(LevelTable* t, const int32_t* hw, int64_t nlev) {
 // host helpers of the TMA / wgmma kernels (capi.cu): cached TMA tensor maps, per-device SM count / shared-memory opt-in
 int make_operand_map(CUtensorMap* map, const void* ptr, long rows, long K, long ld, int nb1, long s1, int nb2, long s2,
                      int box_rows, int* bcast1, int* bcast2);
-int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2);
+int make_store_map(CUtensorMap* map, void* C, int c_dtype, long M, long N, long ldc, int nb1, long c_b1, int nb2, long c_b2,
+                   int box_rows = 128);
 int num_sms();
 int ensure_dyn_smem(const void* func, int bytes);
 
@@ -153,6 +154,25 @@ __device__ __forceinline__ float4 lds128f(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
+__device__ __forceinline__ void sts16(uint32_t addr, __half x) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(__half_as_ushort(x)) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t x) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(x) : "memory"); }
+__device__ __forceinline__ void sts64f(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float2 lds64f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+// named barriers of the warp-specialised kernels (id 0 is __syncthreads), and the producer -> consumer register hand-off
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ float ex2_approx(float x) {  // one MUFU.EX2 (flushes results below 2^-126 to zero)
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

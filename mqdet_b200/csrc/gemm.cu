@@ -132,21 +132,6 @@ struct WgCfg {
   static_assert(EPI_BYTES % 1024 == 0, "swizzled boxes need 1024-byte alignment");
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-template <int R>
-__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R>
-__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-__device__ __forceinline__ void sts32(uint32_t addr, uint32_t x) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(x) : "memory"); }
-__device__ __forceinline__ void sts64f(uint32_t addr, float x, float y) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
-}
-__device__ __forceinline__ float2 lds64f(uint32_t addr) {
-  float2 v;
-  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
-  return v;
-}
 // Byte address of element (r, c) in the TMA-store staging: box c / BOX_COLS, 128-byte rows, 16-byte chunks XOR-swizzled by
 // r % 8 (the layout CU_TENSOR_MAP_SWIZZLE_128B reads).  A warp's fragment writes (8 rows x 4 threads) hit 8 distinct chunks.
 template <int ES>

@@ -55,6 +55,10 @@ class WindowAttention(nn.Module):
 
 
 class SwinTransformerBlock(nn.Module):
+    # C = 96 / 192 (Swin-T stages 1-2, Swin-L stage 1): LN2 -> fc1 -> GELU -> fc2 -> residual in one kernel (ops.swin_mlp,
+    # bit-identical); False keeps the three launches, for A/B runs
+    fused_mlp = True
+
     def __init__(self, dim, num_heads, window_size=7, shift_size=0, mlp_ratio=4.):
         super().__init__()
         self.dim, self.num_heads, self.window_size, self.shift_size = dim, num_heads, window_size, shift_size
@@ -73,6 +77,9 @@ class SwinTransformerBlock(nn.Module):
         o = ops.swin_window_attn(qkv, f32(a.qkv.bias), a.dense_bias(), B, H, W, self.num_heads, self.window_size,
                                  self.shift_size, a.scale)
         x32 = ops.gemm(o, w16(a.proj.weight), bias=f32(a.proj.bias), out_dtype=torch.float32, residual=x32)
+        if self.fused_mlp and self.dim in (96, 192) and self.mlp.fc1.out_features == 4 * self.dim:
+            return ops.swin_mlp(x32, f32(self.norm2.weight), f32(self.norm2.bias), self.norm2.eps, w16(self.mlp.fc1.weight),
+                                f32(self.mlp.fc1.bias), w16(self.mlp.fc2.weight), f32(self.mlp.fc2.bias))
         xn = ops.layernorm(x32, f32(self.norm2.weight), f32(self.norm2.bias), self.norm2.eps)
         h = ops.gemm(xn, w16(self.mlp.fc1.weight), bias=f32(self.mlp.fc1.bias), act=ACT_GELU)
         return ops.gemm(h, w16(self.mlp.fc2.weight), bias=f32(self.mlp.fc2.bias), out_dtype=torch.float32, residual=x32)

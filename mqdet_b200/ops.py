@@ -172,6 +172,28 @@ def layernorm(x, gamma, beta, eps=1e-5, *, out16=True, out32=False, zero_row_per
     return o16 if out16 else o32
 
 
+def swin_mlp(x32, ln_w, ln_b, eps, w1, b1, w2, b2):
+    """The MLP half of a Swin block in one kernel (mqdet_swin_mlp_f16): x32 + fc2(GELU(fc1(LN(x32)))) for a contiguous fp32
+    [rows, C] with C = 96 / 192; w1 fp16 [4C, C], w2 fp16 [C, 4C] (nn.Linear weights), fp32 LN affine and biases -> new fp32
+    [rows, C], bit-identical to layernorm -> gemm(bias, GELU) -> gemm(bias, fp32 residual)."""
+    global launch_count
+    _need_cuda(x32, ln_w, ln_b, w1, b1, w2, b2)
+    C = x32.shape[-1]
+    rows = x32.numel() // C
+    if x32.dtype != torch.float32 or not x32.is_contiguous():
+        raise _lib.MqdetError("swin_mlp: contiguous fp32 rows required")
+    for w, shape in ((w1, (4 * C, C)), (w2, (C, 4 * C))):
+        if w.dtype != torch.float16 or tuple(w.shape) != shape or not w.is_contiguous():
+            raise _lib.MqdetError(f"swin_mlp: weights must be contiguous fp16 {shape} (got {w.dtype} {tuple(w.shape)})")
+    out = torch.empty_like(x32)
+    # algorithmic work: fc1 + fc2 (2 * 2.rows.C.4C); bytes: the fp32 rows in and out, both weights once
+    with _Timed("swin_mlp_kernel", 2.0 * 2.0 * rows * C * 4 * C, 2.0 * 4.0 * rows * C + 2.0 * 2.0 * 4 * C * C):
+        check(load().mqdet_swin_mlp_f16(_ptr(x32), rows, C, _ptr(ln_w), _ptr(ln_b), float(eps), _ptr(w1), _ptr(b1), _ptr(w2),
+                                        _ptr(b2), _ptr(out), _stream()), "swin_mlp")
+    launch_count += 1
+    return out
+
+
 def add_layernorm(a, b, gamma, beta, eps, *, out16=True, out32=True, clamp=0.0):
     """LN(a + b) over the last dim; a, b contiguous fp32."""
     global launch_count
