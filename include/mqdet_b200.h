@@ -133,50 +133,28 @@ int mqdet_gcp_gate_residual_ln(const void* h1, const float* w2, int64_t Dg, cons
 int mqdet_gcp_build_index(const float* mask, int64_t B, int64_t V, int64_t T, int64_t S, int32_t* idx,
                           int32_t* counts_out, void* stream);
 
-/* Row softmax over the last dim with optional additive column mask (warp per row, fp32 math).
- *   x [rows, n] fp16/fp32 (row stride ldx) -> y fp16 [rows, n_pad] (row stride ldy); columns [n, n_pad) := 0.
+/* Row softmax of fp32 scores over the last dim with optional additive column mask (warp per row, fp32 math).
+ *   x [rows, n] fp32 (row stride ldx; in_dtype must be MQDET_F32, anything else is an error) -> y fp16 [rows, n_pad]
+ *   (row stride ldy); columns [n, n_pad) := 0.
  *   v = x*scale + (colmask[batch, c] == 0 ? mask_value : keep_add);  batch = row / rows_per_batch.
  *   BERT self-attention: mask_value -10000, keep_add 0.  BiAttention (fuse_helper.py:270-283): -9e15 / +1. */
 int mqdet_softmax_rows(const void* x, int in_dtype, int64_t ldx, void* y, int64_t ldy, int64_t rows, int64_t n,
                        int64_t n_pad, float scale, const float* colmask, int64_t rows_per_batch, float mask_value,
                        float keep_add, void* stream);
 
-/* Column softmax with transposed output: P[z][t][0:Np] = softmax_n(A[z][n][t]) (zero beyond N), fp16 in/out.
- * BiAttention text->image direction (fuse_helper.py:257-268) without a second QK^T product.  T <= 256, T % 8 == 0.
- * workspace: mqdet_colsoftmax_workspace_floats(Z, N, T) floats. */
-int64_t mqdet_colsoftmax_workspace_floats(int64_t Z, int64_t N, int64_t T);
-int mqdet_colsoftmax_transposed(const void* A, int64_t Z, int64_t N, int64_t T, void* P, int64_t Np, float* workspace,
-                                void* stream);
-
-/* Column statistics only: workspace (mqdet_colsoftmax_workspace_floats(Z, N, T) floats) receives, at float offset
- * Z * ceil(N/512) * 2 * T, stat[z][2][T] = (column max, 1 / column sum of exp) of A [Z][N][T] f16. */
-int mqdet_colsoftmax_stats(const void* A, int64_t Z, int64_t N, int64_t T, float* workspace, void* stream);
-
-/* T == 256: mqdet_colsoftmax_stats and the masked row softmax of the image -> text side in ONE pass over A, in place:
- * statistics of the unmasked scores as above; then A[z][n][:] <- softmax_t(A[z][n][t] + (colmask[z / z_per_mask][t] == 0 ?
- * mask_value : keep_add)) (fuse_helper.py:277-287).  colmask may be NULL (no mask). */
-int mqdet_colstats_rowsoftmax(void* A, int64_t Z, int64_t N, int64_t T, const float* colmask, int64_t z_per_mask,
-                              float mask_value, float keep_add, float* workspace, void* stream);
-
 /* Text -> image side of BiMultiHeadAttention (maskrcnn_benchmark/utils/fuse_helper.py:257-275,289-291) fused into one
- * wgmma kernel per (image, head, 64 text tokens): out[z][t][:] = sum_n softmax_n(clamp(k_t . q_n))[n] * Vv[n][:], without
- * materialising the transposed probabilities: S^T = K Q^T (wgmma, 64 image tokens per step) -> exp(fp16-rounded score
- * - column max) -> fp16 P (register operand) -> O += P Vv (wgmma) -> O / column sum.  stat[z][2][T] as produced by
- * mqdet_colsoftmax_stats from the SAME scores (q already carries the 1/sqrt(d) scale).  z = z2 * nb1 + z1.
- *   k [z][T][d], q [z][N][d], vvT [z][d][Np] f16 (Np >= N, zero padded), out [z][T][d] f16; *_ld = row stride, *_b1 / *_b2 =
- *   batch strides in elements (multiples of 8); d == 256, T <= 256. */
-int mqdet_biattn_text(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld, int64_t q_b1,
-                      int64_t q_b2, const void* vvT, int64_t v_ld, int64_t v_b1, int64_t v_b2, const float* stat, float clamp,
-                      void* out, int64_t o_ld, int64_t o_b1, int64_t o_b2, int64_t nb1, int64_t nb2, int64_t T, int64_t N,
-                      int64_t Np, int64_t d, void* stream);
-
-/* Same kernel, VN variant: the value operand is the layer-normed image-token tensor itself, vn [z][N][256] f16 (read MN-major
- * from the same [token x channel] tile), so that out[z][t][:] = sum_n softmax_n(clamp(k_t . q_n + rowbias_t))[n] * vn[n][:] — the
- * value projection W_vv is applied AFTER the token reduction by the caller (sum_n p[n] = 1 moves the bias out as well), and the
- * [B, E, N] value tensor is never built.  colmax [z][T] f32 = column maxima of the clamped fp32 scores (mqdet_biattn_image);
- * the column sums are accumulated in-kernel from the fp32 scores (no fp16 re-quantisation).  rowbias [z][T * rb_ld] f32 or NULL:
- * an additive score term per text token.  With k := gT (the query projection folded into the keys, see mqdet_biattn_image),
- * q := vn (head stride 0) and rowbias := gbias, the kernel streams only the image tokens: q [B,N,E] is never built. */
+ * wgmma kernel per (image, head, 64 text tokens), without materialising the transposed probabilities:
+ *   out[z][t][:] = sum_n softmax_n(clamp(k_t . q_n + rowbias_t))[n] * vn[n][:]
+ * S^T = K Q^T (wgmma, 64 image tokens per step) -> exp(score - column max) -> fp16 P (register operand) -> O += P vn (wgmma)
+ * -> O / column sum.  The value operand is the layer-normed image-token tensor itself, vn [z][N][256] f16 (read MN-major from
+ * the same [token x channel] tile): the value projection W_vv is applied AFTER the token reduction by the caller (sum_n p[n] = 1
+ * moves the bias out as well), and the [B, E, N] value tensor is never built.  colmax [z][T] f32 = column maxima of the clamped
+ * fp32 scores (mqdet_biattn_image); the column sums are accumulated in-kernel from the fp32 scores.  rowbias [z][T * rb_ld] f32
+ * or NULL: an additive score term per text token.  With k := gT (the query projection folded into the keys, see
+ * mqdet_biattn_image), q := vn (head stride 0) and rowbias := gbias, the kernel streams only the image tokens: q [B,N,E] is
+ * never built.  z = z2 * nb1 + z1.
+ *   k [z][T][256], q [z][N][256], vn [z][N][256], out [z][T][256] f16; *_ld = row stride, *_b1 / *_b2 = batch strides in
+ *   elements (multiples of 8); 1 <= T <= 256. */
 int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld, int64_t q_b1,
                          int64_t q_b2, const void* vn, int64_t vn_ld, int64_t vn_b1, int64_t vn_b2, const float* colmax,
                          const float* rowbias, int64_t rb_ld, float clamp, void* out, int64_t o_ld, int64_t o_b1, int64_t o_b2,

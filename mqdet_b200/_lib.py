@@ -55,14 +55,6 @@ SIGNATURES = {
     "mqdet_gcp_build_index": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "mqdet_softmax_rows": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64, c_float,
                                    c_void_p, c_int64, c_float, c_float, c_void_p]),
-    "mqdet_colsoftmax_workspace_floats": (c_int64, [c_int64, c_int64, c_int64]),
-    "mqdet_colsoftmax_transposed": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
-    "mqdet_colsoftmax_stats": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
-    "mqdet_colstats_rowsoftmax": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_float, c_float, c_void_p,
-                                          c_void_p]),
-    "mqdet_biattn_text": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
-                                  c_int64, c_int64, c_void_p, c_float, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
-                                  c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "mqdet_biattn_text_vn": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64,
                                      c_int64, c_int64, c_void_p, c_void_p, c_int64, c_float, c_void_p, c_int64, c_int64, c_int64,
                                      c_int64, c_int64, c_int64, c_int64, c_void_p]),

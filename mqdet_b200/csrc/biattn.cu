@@ -6,9 +6,9 @@
 //                         fragments -> P (fp16, registers: the A operand of the next wgmma) -> P . mT_h, summed over the heads
 //                         -> v' = residual + gamma * (acc + bias).  Neither the scores nor the per-head context reach HBM.
 //   biattn_text_kernel  : text -> image side (one CTA per (image, head, 64 text tokens), streams all image tokens):
-//                         S^T recomputed on the tensor cores, exp(S^T - column max), P . V accumulated in registers.
-//                         VN variant: V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile),
-//                         the value projection is applied AFTER the token reduction (sum_n p[n] = 1), and the column sums are
+//                         S^T recomputed on the tensor cores, exp(S^T - column max), P . V accumulated in registers, with
+//                         V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile): the value
+//                         projection is applied AFTER the token reduction (sum_n p[n] = 1), and the column sums are
 //                         accumulated in-kernel, so the [B, E, N] value tensor of the image side is never built.
 // Each CTA is one warpgroup; a 64-row tile keeps a 64 x 256 fp32 accumulator in its registers (128 per thread).  Operands arrive
 // by TMA (128B swizzle) through a two-stage ring; accumulator fragment: row / column of element i of thread t = wg_row / wg_col.
@@ -41,36 +41,35 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 // =====================================================================================================================
 // Fused text -> image side of the bi-directional attention (BiMultiHeadAttention, fuse_helper.py:257-275, 289-291):
-//     out[t, :] = sum_n softmax_n(clamp(k_t . q_n)) * Vv[n, :]        per (image, head), t = text token, n = image token
+//     out[t, :] = sum_n softmax_n(clamp(k_t . q_n + rowbias_t)) * vn[n, :]   per (image, head), t = text token, n = image token
 // One CTA per (z, 64 text tokens).  The transposed probabilities [T, N] never reach HBM.  Per step of 64 image tokens:
 //     S^T   = K_tile (64 x 256, resident) . Q_step^T           16 wgmma 64x64x16
-//     P     = exp(fp16(clamp(S^T)) - colmax_t)                  in the accumulator fragments -> fp16 A operand (registers)
-//     O    += P . Vv_step                                        4 wgmma 64x256x16, O (64 x 256) in registers
+//     P     = exp(clamp(S^T + rowbias) - colmax_t)             in the accumulator fragments -> fp16 A operand (registers)
+//     O    += P . vn_step                                        4 wgmma 64x256x16, O (64 x 256) in registers
 //     out   = O / colsum_t  -> fp16
-// colmax / colsum come from mqdet_colsoftmax_stats / mqdet_colstats_rowsoftmax over the SAME fp16 scores the image -> text
-// side uses, so no online rescaling is needed.
+// colmax comes from biattn_image_kernel (the column maxima of the same clamped fp32 scores), so no online rescaling is needed;
+// colsum is accumulated here from the fp32 scores.
 // =====================================================================================================================
 constexpr int BT_STEP = 64;  // image tokens per step
 struct BtCfg {
   static constexpr int KT_BYTES = 4 * KB_BYTES;       // resident K tile: 4 k-blocks of [64 x 64]
   static constexpr int Q_BYTES = 4 * KB_BYTES;        // Q step [64 n x 256 d]
-  static constexpr int V_BYTES = 256 * BT_STEP * 2;   // Vv^T tile [256 d x 64 n]  /  VN: image-token tile [64 n x 256 c]
+  static constexpr int V_BYTES = 256 * BT_STEP * 2;   // image-token tile [64 n x 256 c]
   static constexpr int STAGE_BYTES = Q_BYTES + V_BYTES;
   static constexpr int SMEM_BYTES = KT_BYTES + 2 * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 static_assert(BtCfg::SMEM_BYTES <= 232448, "biattn_text: dynamic shared memory above the 227 KB per-CTA limit");
 struct BtP {
-  const float* stat;  // [Z][2][T]: column max, 1 / column sum   (VN: [Z][T] column max only)
+  const float* stat;  // [Z][T] column max
   float clamp;
   int nb1, T, N, n_steps;
   int k_bc1, k_bc2, q_bc1, q_bc2, v_bc1, v_bc2;  // 1 -> batch coordinate pinned to 0
-  const float* rowbias;                           // VN: optional [Z][T * rb_ld] additive score bias per text token (folded q bias)
+  const float* rowbias;                           // optional [Z][T * rb_ld] additive score bias per text token (folded q bias)
   int rb_ld;
   __half* out;                                    // [nb2][nb1][T][256]
   long o_ld, o_b1, o_b2;
 };
 
-template <bool VN>
 __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_constant__ CUtensorMap tma_k,
                                                              const __grid_constant__ CUtensorMap tma_q,
                                                              const __grid_constant__ CUtensorMap tma_v, const BtP p) {
@@ -93,10 +92,8 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
     uint64_t* bar = &full[i & 1];
     mbar_expect_tx(bar, BtCfg::STAGE_BYTES);
     for (int kb = 0; kb < 4; ++kb) tma_load_4d(st + kb * KB_BYTES, &tma_q, bar, kb * BK, i * BT_STEP, qz1, qz2);
-    if (VN)  // image tokens themselves, [64 n x 256 c] as four [64 n x 64 c] blocks: the B operand of P.vn is read MN-major
-      for (int cb = 0; cb < 4; ++cb) tma_load_4d(st + BtCfg::Q_BYTES + cb * KB_BYTES, &tma_v, bar, cb * BK, i * BT_STEP, vz1, vz2);
-    else
-      tma_load_4d(st + BtCfg::Q_BYTES, &tma_v, bar, i * BT_STEP, 0, vz1, vz2);
+    // image tokens themselves, [64 n x 256 c] as four [64 n x 64 c] blocks: the B operand of P.vn is read MN-major
+    for (int cb = 0; cb < 4; ++cb) tma_load_4d(st + BtCfg::Q_BYTES + cb * KB_BYTES, &tma_v, bar, cb * BK, i * BT_STEP, vz1, vz2);
   };
   if (tid == 0) {
     tma_prefetch_desc(&tma_k);
@@ -121,13 +118,8 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
   for (int h = 0; h < 2; ++h) {
     const int t = mt * BM + wg_row(tid, 2 * h);
     if (t < p.T) {
-      if (VN) {
-        m_l2[h] = -p.stat[(long)z * p.T + t] * L2E;
-        if (p.rowbias) gb[h] = p.rowbias[((long)z * p.T + t) * p.rb_ld];
-      } else {
-        m_l2[h] = -p.stat[((long)z * 2) * p.T + t] * L2E;
-        inv[h] = p.stat[((long)z * 2 + 1) * p.T + t];
-      }
+      m_l2[h] = -p.stat[(long)z * p.T + t] * L2E;
+      if (p.rowbias) gb[h] = p.rowbias[((long)z * p.T + t) * p.rb_ld];
     }
   }
   const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
@@ -158,12 +150,9 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
     for (int j = 0; j < 32; ++j) {
       const int h = (j >> 1) & 1;
       const float a = fminf(fmaxf(sc[j] + gb[h], -clampv), clampv);
-      // !VN: the score as the fp16 matrix A holds it (the statistics were taken from those values);
-      //  VN: the fp32 score itself (the column maxima come from the fp32 scores of the image-side kernel)
-      const float f = VN ? a : __half2float(__float2half_rn(a));
-      float e = ex2_approx(fmaf(f, L2E, m_l2[h]));
+      float e = ex2_approx(fmaf(a, L2E, m_l2[h]));
       if (wg_col(tid, j) >= nrem) e = 0.f;  // image tokens beyond N (zero-filled q rows) must not contribute exp(-max)
-      if (VN) lsum[h] += e;
+      lsum[h] += e;
       sc[j] = e;
     }
     uint32_t pa[4][4];
@@ -173,12 +162,9 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
-      // VN: B = vn tile read MN-major (N = channel contiguous): 16 image tokens per MMA = 2 KB further down the block,
+      // B = vn tile read MN-major (N = channel contiguous): 16 image tokens per MMA = 2 KB further down the block,
       // next 8 tokens (SBO) 1 KB apart, next 64 channels (LBO) one [64 n x 64 c] block = 8 KB apart
-      if (VN)
-        wgmma_rs_m64n256_kmn(o, pa[kk], wg_desc_mn_sw128(v0 + kk * 2048, KB_BYTES, 1024), 1);
-      else
-        wgmma_rs_m64n256_kk(o, pa[kk], wg_desc_k_sw128(v0 + kk * 32), 1);
+      wgmma_rs_m64n256_kmn(o, pa[kk], wg_desc_mn_sw128(v0 + kk * 2048, KB_BYTES, 1024), 1);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -186,12 +172,11 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
     __syncthreads();  // every wgmma of the warpgroup has read stage s
     if (tid == 0 && i + 2 < NS) issue(i + 2);
   }
-  if (VN) {  // total column sum of this text token: the four threads of a quad hold its columns
+  // total column sum of this text token: the four threads of a quad hold its columns
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float tot = quad_sum(lsum[h]);
-      inv[h] = tot > 0.f ? 1.f / tot : 0.f;
-    }
+  for (int h = 0; h < 2; ++h) {
+    const float tot = quad_sum(lsum[h]);
+    inv[h] = tot > 0.f ? 1.f / tot : 0.f;
   }
   // ---- epilogue: O / colsum -> fp16 ----
   __half* out = p.out + z1 * p.o_b1 + z2 * p.o_b2;
@@ -426,36 +411,33 @@ __global__ void colmax_reduce_kernel(const float* __restrict__ part, int tiles, 
 
 using namespace mqdet;
 
-static int text_launch(bool vn, const float* rowbias, int64_t rb_ld, const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld, int64_t q_b1,
-                       int64_t q_b2, const void* v, int64_t v_ld, int64_t v_b1, int64_t v_b2, const float* stat, float clamp,
-                       void* out, int64_t o_ld, int64_t o_b1, int64_t o_b2, int64_t nb1, int64_t nb2, int64_t T, int64_t N,
-                       int64_t Np, int64_t d, void* stream) {
-  MQ_REQUIRE(k && q && v && stat && out, "biattn_text: null pointer");
-  MQ_REQUIRE(d == 256, "biattn_text: head dim must be 256 (embed 2048 / 8 heads, fuse_helper.py:186-189), got %ld", (long)d);
-  MQ_REQUIRE(T >= 1 && T <= 256 && N >= 1 && Np >= N && (Np % 8) == 0, "biattn_text: need 1 <= T <= 256, Np >= N, Np %% 8 == 0");
-  MQ_REQUIRE(nb1 >= 1 && nb2 >= 1 && nb1 * nb2 <= 65535, "biattn_text: bad batch");
-  const int64_t lds[] = {k_ld, k_b1, k_b2, q_ld, q_b1, q_b2, v_ld, v_b1, v_b2, o_ld, o_b1, o_b2};
-  for (int64_t x : lds) MQ_REQUIRE((x % 8) == 0, "biattn_text: strides must be multiples of 8 elements");
-  MQ_REQUIRE(((uintptr_t)k % 16) == 0 && ((uintptr_t)q % 16) == 0 && ((uintptr_t)v % 16) == 0 && ((uintptr_t)out % 16) == 0,
-             "biattn_text: operands must be 16-byte aligned");
+extern "C" int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld,
+                                    int64_t q_b1, int64_t q_b2, const void* vn, int64_t vn_ld, int64_t vn_b1, int64_t vn_b2,
+                                    const float* colmax, const float* rowbias, int64_t rb_ld, float clamp, void* out, int64_t o_ld,
+                                    int64_t o_b1, int64_t o_b2, int64_t nb1, int64_t nb2, int64_t T, int64_t N, void* stream) {
+  MQ_REQUIRE(k && q && vn && colmax && out, "biattn_text_vn: null pointer");
+  MQ_REQUIRE(T >= 1 && T <= 256 && N >= 1, "biattn_text_vn: need 1 <= T <= 256, N >= 1");
+  MQ_REQUIRE(nb1 >= 1 && nb2 >= 1 && nb1 * nb2 <= 65535, "biattn_text_vn: bad batch");
+  const int64_t lds[] = {k_ld, k_b1, k_b2, q_ld, q_b1, q_b2, vn_ld, vn_b1, vn_b2, o_ld, o_b1, o_b2};
+  for (int64_t x : lds) MQ_REQUIRE((x % 8) == 0, "biattn_text_vn: strides must be multiples of 8 elements");
+  MQ_REQUIRE(((uintptr_t)k % 16) == 0 && ((uintptr_t)q % 16) == 0 && ((uintptr_t)vn % 16) == 0 && ((uintptr_t)out % 16) == 0,
+             "biattn_text_vn: operands must be 16-byte aligned");
   CUtensorMap mk, mq, mv;
   BtP p;
   memset(&p, 0, sizeof(p));
-  int rc = make_operand_map(&mk, k, T, d, k_ld, (int)nb1, k_b1, (int)nb2, k_b2, BM, &p.k_bc1, &p.k_bc2);
+  int rc = make_operand_map(&mk, k, T, 256, k_ld, (int)nb1, k_b1, (int)nb2, k_b2, BM, &p.k_bc1, &p.k_bc2);
   if (rc) return rc;
-  rc = make_operand_map(&mq, q, N, d, q_ld, (int)nb1, q_b1, (int)nb2, q_b2, BT_STEP, &p.q_bc1, &p.q_bc2);
+  rc = make_operand_map(&mq, q, N, 256, q_ld, (int)nb1, q_b1, (int)nb2, q_b2, BT_STEP, &p.q_bc1, &p.q_bc2);
   if (rc) return rc;
-  if (vn)  // image tokens [N][256 c]: box [64 n x 64 c]
-    rc = make_operand_map(&mv, v, N, 256, v_ld, (int)nb1, v_b1, (int)nb2, v_b2, BT_STEP, &p.v_bc1, &p.v_bc2);
-  else     // Vv^T [256 d][Np]: box [256 d x 64 n]
-    rc = make_operand_map(&mv, v, d, Np, v_ld, (int)nb1, v_b1, (int)nb2, v_b2, 256, &p.v_bc1, &p.v_bc2);
+  // image tokens [N][256 c]: box [64 n x 64 c]
+  rc = make_operand_map(&mv, vn, N, 256, vn_ld, (int)nb1, vn_b1, (int)nb2, vn_b2, BT_STEP, &p.v_bc1, &p.v_bc2);
   if (rc) return rc;
-  MQ_REQUIRE((nb1 == 1 || o_b1 != 0) && (nb2 == 1 || o_b2 != 0), "biattn_text: output batch strides must be non-zero");
+  MQ_REQUIRE((nb1 == 1 || o_b1 != 0) && (nb2 == 1 || o_b2 != 0), "biattn_text_vn: output batch strides must be non-zero");
   p.out = (__half*)out;
   p.o_ld = o_ld;
   p.o_b1 = o_b1;
   p.o_b2 = o_b2;
-  p.stat = stat;
+  p.stat = colmax;
   p.clamp = clamp;
   p.nb1 = (int)nb1;
   p.T = (int)T;
@@ -464,32 +446,10 @@ static int text_launch(bool vn, const float* rowbias, int64_t rb_ld, const void*
   p.rowbias = rowbias;
   p.rb_ld = (int)(rb_ld > 0 ? rb_ld : 1);
   dim3 grid((unsigned)((T + BM - 1) / BM), (unsigned)(nb1 * nb2));
-  if (vn) {
-    rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel<true>), BtCfg::SMEM_BYTES);
-    if (rc) return rc;
-    biattn_text_kernel<true><<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
-  } else {
-    rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel<false>), BtCfg::SMEM_BYTES);
-    if (rc) return rc;
-    biattn_text_kernel<false><<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
-  }
+  rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel), BtCfg::SMEM_BYTES);
+  if (rc) return rc;
+  biattn_text_kernel<<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
   return check_launch("biattn_text_kernel");
-}
-
-extern "C" int mqdet_biattn_text(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld,
-                                 int64_t q_b1, int64_t q_b2, const void* vvT, int64_t v_ld, int64_t v_b1, int64_t v_b2,
-                                 const float* stat, float clamp, void* out, int64_t o_ld, int64_t o_b1, int64_t o_b2,
-                                 int64_t nb1, int64_t nb2, int64_t T, int64_t N, int64_t Np, int64_t d, void* stream) {
-  return text_launch(false, nullptr, 0, k, k_ld, k_b1, k_b2, q, q_ld, q_b1, q_b2, vvT, v_ld, v_b1, v_b2, stat, clamp, out, o_ld, o_b1, o_b2,
-                     nb1, nb2, T, N, Np, d, stream);
-}
-
-extern "C" int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, int64_t k_b2, const void* q, int64_t q_ld,
-                                    int64_t q_b1, int64_t q_b2, const void* vn, int64_t vn_ld, int64_t vn_b1, int64_t vn_b2,
-                                    const float* colmax, const float* rowbias, int64_t rb_ld, float clamp, void* out, int64_t o_ld,
-                                    int64_t o_b1, int64_t o_b2, int64_t nb1, int64_t nb2, int64_t T, int64_t N, void* stream) {
-  return text_launch(true, rowbias, rb_ld, k, k_ld, k_b1, k_b2, q, q_ld, q_b1, q_b2, vn, vn_ld, vn_b1, vn_b2, colmax, clamp, out, o_ld, o_b1,
-                     o_b2, nb1, nb2, T, N, (N + 7) / 8 * 8, 256, stream);
 }
 
 extern "C" int64_t mqdet_biattn_image_workspace_floats(int64_t B, int64_t H, int64_t N, int64_t T) {

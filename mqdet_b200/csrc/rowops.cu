@@ -232,28 +232,27 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(const float* __restr
   }
 }
 
-// Masked row softmax, warp per row. x fp16 or fp32 -> y fp16. Columns [n, n_pad) are written as 0.
-template <typename T>
-__global__ void __launch_bounds__(256) softmax_rows_kernel(const T* __restrict__ x, long ldx, __half* __restrict__ y, long ldy,
+// Masked row softmax, warp per row. x fp32 -> y fp16. Columns [n, n_pad) are written as 0.
+__global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ x, long ldx, __half* __restrict__ y, long ldy,
                                                            long rows, int n, int n_pad, float scale,
                                                            const float* __restrict__ colmask, long rows_per_batch,
                                                            float mask_value, float keep_add) {
   const long row = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const T* xr = x + row * ldx;
+  const float* xr = x + row * ldx;
   __half* yr = y + row * ldy;
   const float* cm = colmask ? colmask + (row / rows_per_batch) * n : nullptr;
   float mx = -INFINITY;
   for (int i = lane; i < n; i += 32) {
-    float v = ld_as_float(xr + i) * scale;
+    float v = xr[i] * scale;
     if (cm) v += (cm[i] == 0.f) ? mask_value : keep_add;
     mx = fmaxf(mx, v);
   }
   mx = warp_max(mx);
   float sum = 0.f;
   for (int i = lane; i < n; i += 32) {
-    float v = ld_as_float(xr + i) * scale;
+    float v = xr[i] * scale;
     if (cm) v += (cm[i] == 0.f) ? mask_value : keep_add;
     sum += expf(v - mx);
   }
@@ -262,64 +261,11 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const T* __restrict__
   for (int i = lane; i < n_pad; i += 32) {
     float o = 0.f;
     if (i < n) {
-      float v = ld_as_float(xr + i) * scale;
+      float v = xr[i] * scale;
       if (cm) v += (cm[i] == 0.f) ? mask_value : keep_add;
       o = expf(v - mx) * inv;
     }
     yr[i] = __float2half_rn(o);
-  }
-}
-
-// Hot case of the fusion tower (A [B*H*N, 256 tokens], in place): one warp owns RW consecutive rows per step and issues all
-// RW 16-byte loads before touching any of them (4x the bytes in flight of the generic kernel), exp via FFMA + MUFU.EX2.
-template <int RW>
-__global__ void __launch_bounds__(256) softmax_rows256_kernel(const __half* __restrict__ x, long ldx, __half* __restrict__ y,
-                                                              long ldy, long rows, float scale, const float* __restrict__ colmask,
-                                                              long rows_per_batch, float mask_value, float keep_add) {
-  const int lane = threadIdx.x & 31;
-  const long r0 = ((long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * RW;
-  if (r0 >= rows) return;
-  constexpr float L2E = 1.4426950408889634f;
-  uint4 u[RW];
-#pragma unroll
-  for (int j = 0; j < RW; ++j)
-    u[j] = (r0 + j < rows) ? *reinterpret_cast<const uint4*>(x + (r0 + j) * ldx + lane * 8) : make_uint4(0, 0, 0, 0);
-#pragma unroll
-  for (int j = 0; j < RW; ++j) {
-    const long row = r0 + j;
-    if (row >= rows) break;
-    float v[8];
-    const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 f = __half22float2(h[i]);
-      v[2 * i] = f.x * scale;
-      v[2 * i + 1] = f.y * scale;
-    }
-    if (colmask) {
-      const float* cm = colmask + (row / rows_per_batch) * 256 + lane * 8;
-      const float4 m0 = *reinterpret_cast<const float4*>(cm);
-      const float4 m1 = *reinterpret_cast<const float4*>(cm + 4);
-      const float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] += (mm[i] == 0.f) ? mask_value : keep_add;
-    }
-    float mx = v[0];
-#pragma unroll
-    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, v[i]);
-    mx = warp_max(mx);
-    const float ms = -mx * L2E;
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      v[i] = exp2f(fmaf(v[i], L2E, ms));
-      sum += v[i];
-    }
-    const float inv = 1.f / warp_sum(sum);
-    __half2 o[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = __floats2half2_rn(v[2 * i] * inv, v[2 * i + 1] * inv);
-    *reinterpret_cast<uint4*>(y + row * ldy + lane * 8) = *reinterpret_cast<uint4*>(o);
   }
 }
 
@@ -456,436 +402,6 @@ __global__ void __launch_bounds__(256) sum_splits_cast_kernel(const float4* __re
   u.x = *reinterpret_cast<const uint32_t*>(&h0);
   u.y = *reinterpret_cast<const uint32_t*>(&h1);
   *reinterpret_cast<uint2*>(o) = u;
-}
-
-// Vectorised fp16 row softmax (rows 16-byte aligned, n % 8 == 0): one warp per row, 8 halfs per lane per step.
-//   ITERS > 0 : the whole row (n <= ITERS*256) lives in registers -> one read, one write      (A: n = 256 tokens)
-//   ITERS == 0: two passes, online max/sum then normalise                                     (At: n = 22400 locations)
-template <int ITERS>
-__global__ void __launch_bounds__(256) softmax_rows_f16v_kernel(const __half* __restrict__ x, long ldx, __half* __restrict__ y,
-                                                                long ldy, long rows, int n, int n_pad, float scale,
-                                                                const float* __restrict__ colmask, long rows_per_batch,
-                                                                float mask_value, float keep_add) {
-  const long row = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const __half* xr = x + row * ldx;
-  __half* yr = y + row * ldy;
-  const float* cm = colmask ? colmask + (row / rows_per_batch) * n : nullptr;
-  auto load8 = [&](int c, float (&v)[8]) {
-    const uint4 u = *reinterpret_cast<const uint4*>(xr + c);
-    const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 f = __half22float2(h[i]);
-      v[2 * i] = f.x * scale;
-      v[2 * i + 1] = f.y * scale;
-    }
-    if (cm) {
-      const float4 m0 = *reinterpret_cast<const float4*>(cm + c);
-      const float4 m1 = *reinterpret_cast<const float4*>(cm + c + 4);
-      const float mm[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] += (mm[i] == 0.f) ? mask_value : keep_add;
-    }
-  };
-  auto store8 = [&](int c, const float (&v)[8]) {
-    __half2 h[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    *reinterpret_cast<uint4*>(yr + c) = *reinterpret_cast<uint4*>(h);
-  };
-  if (ITERS > 0) {
-    float v[ITERS > 0 ? ITERS : 1][8];
-    float mx = -INFINITY;
-#pragma unroll
-    for (int it = 0; it < ITERS; ++it) {
-      const int c = it * 256 + lane * 8;
-      if (c < n) {
-        load8(c, v[it]);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) mx = fmaxf(mx, v[it][i]);
-      }
-    }
-    mx = warp_max(mx);
-    float sum = 0.f;
-#pragma unroll
-    for (int it = 0; it < ITERS; ++it) {
-      const int c = it * 256 + lane * 8;
-      if (c < n) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          v[it][i] = expf(v[it][i] - mx);
-          sum += v[it][i];
-        }
-      }
-    }
-    const float inv = 1.f / warp_sum(sum);
-#pragma unroll
-    for (int it = 0; it < ITERS; ++it) {
-      const int c = it * 256 + lane * 8;
-      if (c < n) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[it][i] *= inv;
-        store8(c, v[it]);
-      } else if (c < n_pad) {
-        const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        store8(c, z);
-      }
-    }
-  } else {
-    float mx = -INFINITY, sum = 0.f;  // online (max, sum) per lane, merged across the warp afterwards
-    for (int c = lane * 8; c < n; c += 256) {
-      float v[8];
-      load8(c, v);
-      float m2 = mx;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) m2 = fmaxf(m2, v[i]);
-      float s2 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s2 += expf(v[i] - m2);
-      sum = sum * expf(mx - m2) + s2;
-      mx = m2;
-    }
-    const float gmx = warp_max(mx);
-    const float gsum = warp_sum(sum * expf(mx - gmx));  // lanes with no element: mx = -inf -> contributes 0
-    const float inv = 1.f / gsum;
-    for (int c = lane * 8; c < n_pad; c += 256) {
-      float v[8];
-      if (c < n) {
-        load8(c, v);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = expf(v[i] - gmx) * inv;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = 0.f;
-      }
-      store8(c, v);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Column softmax with transposed output: P[z][t][n] = softmax over n of A[z][n][t]   (BiAttention text->image side,
-// fuse_helper.py:257-268: softmax_N(A^T - rowmax(A^T))).  Replaces a second QK^T product + row softmax:
-//   1. colsoftmax_stats  : per (z, 256-row chunk) online (max, sum-exp) per column        -> partial[z][chunk][2][T]
-//   2. colsoftmax_finish : merges the chunks                                                -> stat[z][2][T] (max, 1/sum)
-//   3. colsoftmax_write  : 64-row tiles through shared memory, 16-byte coalesced transposed stores
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int CS_ROWS = 512;
-
-// generic fallback (T not a power of two): thread == column, serial online softmax over the chunk's rows
-__global__ void __launch_bounds__(256) colsoftmax_stats_generic_kernel(const __half* __restrict__ A, int N, int T,
-                                                                       float* __restrict__ partial, int nchunks) {
-  const int chunk = blockIdx.x, z = blockIdx.y;
-  const int r0 = chunk * CS_ROWS, r1 = min(N, r0 + CS_ROWS);
-  const __half* a = A + (long)z * N * T;
-  for (int t = threadIdx.x; t < T; t += blockDim.x) {
-    float m = -INFINITY, s = 0.f;
-    for (int r = r0; r < r1; ++r) {
-      const float v = __half2float(a[(long)r * T + t]);
-      const float m2 = fmaxf(m, v);
-      s = s * expf(m - m2) + expf(v - m2);
-      m = m2;
-    }
-    float* o = partial + (((long)z * nchunks + chunk) * 2) * T;
-    o[t] = m;
-    o[T + t] = s;
-  }
-}
-
-// T in {8, 16, .., 256} (power of two): a thread keeps 8 columns (one 16-byte vector) and walks the chunk 8 rows at a time:
-// 8 independent 16-byte loads in flight, block maximum first, then ONE exp per element (+ 8 rescales per 64 elements);
-// the 256 / (T/8) row groups of the CTA are merged through shared memory.
-__global__ void __launch_bounds__(256) colsoftmax_stats_kernel(const __half* __restrict__ A, int N, int T,
-                                                               float* __restrict__ partial, int nchunks) {
-  __shared__ float sm[2048], ss[2048];  // [row group][column]: groups * T == 2048 for every T
-  constexpr float L2E = 1.4426950408889634f;
-  const int chunk = blockIdx.x, z = blockIdx.y;
-  const int vpr = T >> 3;                 // vectors per row
-  const int groups = 256 / vpr;           // row groups of the CTA
-  const int g = threadIdx.x / vpr, c = (threadIdx.x % vpr) * 8;
-  const int r0 = chunk * CS_ROWS, r1 = min(N, r0 + CS_ROWS);
-  const __half* a = A + (long)z * N * T + c;
-  float m[8], sacc[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    m[i] = -INFINITY;
-    sacc[i] = 0.f;
-  }
-  for (int rb = r0 + g; rb < r1; rb += groups * 8) {
-    uint4 u[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int r = rb + j * groups;
-      // rows beyond the chunk: repeat the first row of the block (valid) and mask it out of the sum below
-      u[j] = *reinterpret_cast<const uint4*>(a + (long)(r < r1 ? r : rb) * T);
-    }
-    float bm[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) bm[i] = m[i];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        bm[2 * i] = fmaxf(bm[2 * i], f.x);
-        bm[2 * i + 1] = fmaxf(bm[2 * i + 1], f.y);
-      }
-    }
-    float nm[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      sacc[i] *= exp2f((m[i] - bm[i]) * L2E);  // m = -inf on the first block: exp2(-inf) = 0, sacc stays 0
-      m[i] = bm[i];
-      nm[i] = -bm[i] * L2E;
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      if (rb + j * groups < r1) {
-        const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 f = __half22float2(h[i]);
-          sacc[2 * i] += exp2f(fmaf(f.x, L2E, nm[2 * i]));
-          sacc[2 * i + 1] += exp2f(fmaf(f.y, L2E, nm[2 * i + 1]));
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    sm[g * T + c + i] = m[i];
-    ss[g * T + c + i] = sacc[i];
-  }
-  __syncthreads();
-  for (int t = threadIdx.x; t < T; t += blockDim.x) {
-    float mm = -INFINITY;
-    for (int k = 0; k < groups; ++k) mm = fmaxf(mm, sm[k * T + t]);
-    float s = 0.f;
-    for (int k = 0; k < groups; ++k)
-      if (sm[k * T + t] > -INFINITY) s += ss[k * T + t] * exp2f((sm[k * T + t] - mm) * L2E);
-    float* o = partial + (((long)z * nchunks + chunk) * 2) * T;
-    o[t] = mm;
-    o[T + t] = s;
-  }
-}
-
-// Fusion-tower special (T == 256): ONE pass over A [Z][N][256] that (a) accumulates the per-column (max, sum-exp) partials
-// exactly like colsoftmax_stats_kernel and (b) replaces every row by its masked softmax over the 256 tokens (the
-// image -> text probabilities, fuse_helper.py:277-287) in place.  With 32 vectors per row a warp owns whole rows, so the
-// row reductions are warp shuffles; every element is read once by the thread that overwrites it.
-__global__ void __launch_bounds__(256, 4) colstats_rowsoftmax256_kernel(__half* __restrict__ A, int N, float* __restrict__ partial,
-                                                                     int nchunks, const float* __restrict__ colmask,
-                                                                     int z_per_mask, float mask_value, float keep_add) {
-  constexpr int T = 256;
-  constexpr float L2E = 1.4426950408889634f;
-  __shared__ float sm[2048], ss[2048];
-  const int chunk = blockIdx.x, z = blockIdx.y;
-  const int g = threadIdx.x >> 5, lane = threadIdx.x & 31, c = lane * 8;
-  const int r0 = chunk * CS_ROWS, r1 = min(N, r0 + CS_ROWS);
-  __half* a = A + (long)z * N * T + c;
-  // additive mask of this thread's 8 columns as bits (1 = token in use) -> 1 register instead of 8
-  unsigned keep_bits = 0xffu;
-  float add_keep = 0.f, add_mask = 0.f;
-  if (colmask) {
-    const float* cm = colmask + (long)(z / z_per_mask) * T + c;
-    keep_bits = 0u;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) keep_bits |= (cm[i] != 0.f ? 1u : 0u) << i;
-    add_keep = keep_add;
-    add_mask = mask_value;
-  }
-  float m[8], sacc[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    m[i] = -INFINITY;
-    sacc[i] = 0.f;
-  }
-  constexpr int RB = 4;  // rows per thread per block: 4 x 16 B in flight, <= 64 registers -> 4 CTAs / SM
-  for (int rb = r0 + g; rb < r1; rb += 8 * RB) {
-    uint4 u[RB];
-#pragma unroll
-    for (int j = 0; j < RB; ++j) {
-      const int r = rb + j * 8;
-      u[j] = *reinterpret_cast<const uint4*>(a + (long)(r < r1 ? r : rb) * T);
-    }
-    // ---- column statistics (unmasked scores) ----
-    float bm[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) bm[i] = m[i];
-#pragma unroll
-    for (int j = 0; j < RB; ++j) {
-      const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        bm[2 * i] = fmaxf(bm[2 * i], f.x);
-        bm[2 * i + 1] = fmaxf(bm[2 * i + 1], f.y);
-      }
-    }
-    float nm[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      sacc[i] *= exp2f((m[i] - bm[i]) * L2E);
-      m[i] = bm[i];
-      nm[i] = -bm[i] * L2E;
-    }
-#pragma unroll
-    for (int j = 0; j < RB; ++j) {
-      const int r = rb + j * 8;
-      if (r >= r1) continue;  // warp-uniform
-      const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-      float v[8];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        v[2 * i] = f.x;
-        v[2 * i + 1] = f.y;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) sacc[i] += exp2f(fmaf(v[i], L2E, nm[i]));
-      // ---- masked row softmax, in place ----
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        v[i] += ((keep_bits >> i) & 1u) ? add_keep : add_mask;
-        mx = fmaxf(mx, v[i]);
-      }
-      mx = warp_max(mx);
-      const float ms = -mx * L2E;
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        v[i] = exp2f(fmaf(v[i], L2E, ms));
-        sum += v[i];
-      }
-      const float inv = 1.f / warp_sum(sum);
-      __half2 o[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) o[i] = __floats2half2_rn(v[2 * i] * inv, v[2 * i + 1] * inv);
-      *reinterpret_cast<uint4*>(a + (long)r * T) = *reinterpret_cast<uint4*>(o);
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    sm[g * T + c + i] = m[i];
-    ss[g * T + c + i] = sacc[i];
-  }
-  __syncthreads();
-  {
-    const int t = threadIdx.x;
-    float mm = -INFINITY;
-    for (int k = 0; k < 8; ++k) mm = fmaxf(mm, sm[k * T + t]);
-    float s = 0.f;
-    for (int k = 0; k < 8; ++k)
-      if (sm[k * T + t] > -INFINITY) s += ss[k * T + t] * exp2f((sm[k * T + t] - mm) * L2E);
-    float* o = partial + (((long)z * nchunks + chunk) * 2) * T;
-    o[t] = mm;
-    o[T + t] = s;
-  }
-}
-
-__global__ void colsoftmax_finish_kernel(const float* __restrict__ partial, int T, int nchunks, float* __restrict__ stat) {
-  const int z = blockIdx.x;
-  for (int t = threadIdx.x; t < T; t += blockDim.x) {
-    float m = -INFINITY;
-    for (int c = 0; c < nchunks; ++c) m = fmaxf(m, partial[(((long)z * nchunks + c) * 2) * T + t]);
-    float s = 0.f;
-    for (int c = 0; c < nchunks; ++c) {
-      const float* o = partial + (((long)z * nchunks + c) * 2) * T;
-      if (o[t] > -INFINITY) s += o[T + t] * expf(o[t] - m);
-    }
-    stat[((long)z * 2) * T + t] = m;
-    stat[((long)z * 2 + 1) * T + t] = 1.f / s;
-  }
-}
-
-// tile: 64 rows (n) x T columns -> P[z][t][n0..n0+63];  T <= 256, T % 8 == 0.
-// Row-major staging (16-byte conflict-free stores), then lane == column t reads 16 consecutive rows (2-byte loads,
-// consecutive lanes -> consecutive half-words) and writes one full 32-byte sector of P[t][n0+r0 .. +15].
-template <bool T256>
-__global__ void __launch_bounds__(256) colsoftmax_write_kernel(const __half* __restrict__ A, int N, int Np, int T,
-                                                               const float* __restrict__ stat, __half* __restrict__ P) {
-  __shared__ __align__(16) __half tile[64][256 + 8];
-  const int n0 = blockIdx.x * 64, z = blockIdx.y;
-  const __half* a = A + (long)z * N * T;
-  const float* mx = stat + ((long)z * 2) * T;
-  const float* inv = mx + T;
-  constexpr float L2E = 1.4426950408889634f;
-  if (T256) {
-    // T == 256: a thread keeps its 8 columns for all 8 of its rows; the 8 row loads are issued before any is used
-    const int c = (threadIdx.x & 31) * 8, rb = threadIdx.x >> 5;
-    float mxr[8], ivr[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      mxr[k] = -mx[c + k] * L2E;  // exp(v - m) = exp2(v * log2e - m * log2e)
-      ivr[k] = inv[c + k];
-    }
-    uint4 u[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int r = rb + 8 * j;
-      u[j] = (n0 + r < N) ? *reinterpret_cast<const uint4*>(a + (long)(n0 + r) * 256 + c) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int r = rb + 8 * j;
-      __half2 o[4];
-      if (n0 + r < N) {
-        const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float2 f = __half22float2(h[k]);
-          o[k] = __floats2half2_rn(exp2f(fmaf(f.x, L2E, mxr[2 * k])) * ivr[2 * k],
-                                   exp2f(fmaf(f.y, L2E, mxr[2 * k + 1])) * ivr[2 * k + 1]);
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) o[k] = __float2half2_rn(0.f);  // rows beyond N: zero padding of the K dimension of P.Vv
-      }
-      *reinterpret_cast<uint4*>(&tile[r][c]) = *reinterpret_cast<uint4*>(o);
-    }
-  } else {
-    const int vec_per_row = T / 8;
-    for (int i = threadIdx.x; i < 64 * vec_per_row; i += 256) {
-      const int r = i / vec_per_row, c = (i % vec_per_row) * 8;
-      __half2 o[4];
-      if (n0 + r < N) {
-        const uint4 u = *reinterpret_cast<const uint4*>(a + (long)(n0 + r) * T + c);
-        const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float2 f = __half22float2(h[k]);
-          o[k] = __floats2half2_rn(exp2f((f.x - mx[c + 2 * k]) * L2E) * inv[c + 2 * k],
-                                   exp2f((f.y - mx[c + 2 * k + 1]) * L2E) * inv[c + 2 * k + 1]);
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) o[k] = __float2half2_rn(0.f);
-      }
-      *reinterpret_cast<uint4*>(&tile[r][c]) = *reinterpret_cast<uint4*>(o);
-    }
-  }
-  __syncthreads();
-  __half* p = P + (long)z * T * Np;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tgroups = (T + 31) / 32;
-  for (int it = warp; it < tgroups * 4; it += 8) {
-    const int t = (it / 4) * 32 + lane, r0 = (it % 4) * 16;
-    if (t >= T) continue;
-    __align__(16) __half v[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] = tile[r0 + k][t];
-    __half* dst = p + (long)t * Np + n0 + r0;
-    if (n0 + r0 + 16 <= Np) {
-      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<uint4*>(&v[0]);
-      *reinterpret_cast<uint4*>(dst + 8) = *reinterpret_cast<uint4*>(&v[8]);
-    } else if (n0 + r0 + 8 <= Np) {
-      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<uint4*>(&v[0]);
-    }
-  }
 }
 
 // ContrastiveEmbed tail (groundingdino_new/models/GroundingDINO/utils.py:261-266): columns of padding tokens and the
@@ -1027,49 +543,25 @@ extern "C" int mqdet_softmax_rows(const void* x, int in_dtype, int64_t ldx, void
                                   int64_t n_pad, float scale, const float* colmask, int64_t rows_per_batch,
                                   float mask_value, float keep_add, void* stream) {
   MQ_REQUIRE(x && y && rows > 0 && n > 0 && n_pad >= n, "softmax_rows: bad args");
+  MQ_REQUIRE(in_dtype == MQDET_F32, "softmax_rows: fp32 scores required (in_dtype %d)", in_dtype);
   if (rows_per_batch <= 0) rows_per_batch = rows;
   const int wpb = 8;
-  dim3 grid(cdiv(rows, wpb));
   cudaStream_t st = (cudaStream_t)stream;
-  const bool vec = in_dtype == MQDET_F16 && (n % 8) == 0 && (n_pad % 8) == 0 && (ldx % 8) == 0 && (ldy % 8) == 0 &&
-                   ((uintptr_t)x % 16) == 0 && ((uintptr_t)y % 16) == 0 && (!colmask || ((uintptr_t)colmask % 16) == 0);
-  if (vec) {
-    const __half* xh = (const __half*)x;
-    __half* yh = (__half*)y;
-    if (n == 256 && n_pad == 256) {
-      constexpr int RW = 4;
-      softmax_rows256_kernel<RW><<<(unsigned)cdiv(rows, (long)wpb * RW), wpb * 32, 0, st>>>(xh, ldx, yh, ldy, rows, scale, colmask,
-                                                                                           rows_per_batch, mask_value, keep_add);
-    } else if (n_pad <= 256)
-      softmax_rows_f16v_kernel<1><<<grid, wpb * 32, 0, st>>>(xh, ldx, yh, ldy, rows, (int)n, (int)n_pad, scale, colmask,
-                                                            rows_per_batch, mask_value, keep_add);
-    else if (n_pad <= 1024)
-      softmax_rows_f16v_kernel<4><<<grid, wpb * 32, 0, st>>>(xh, ldx, yh, ldy, rows, (int)n, (int)n_pad, scale, colmask,
-                                                            rows_per_batch, mask_value, keep_add);
-    else
-      softmax_rows_f16v_kernel<0><<<grid, wpb * 32, 0, st>>>(xh, ldx, yh, ldy, rows, (int)n, (int)n_pad, scale, colmask,
-                                                            rows_per_batch, mask_value, keep_add);
-    return check_launch("softmax_rows_f16v_kernel");
-  }
-  if (in_dtype == MQDET_F32 && n == 256 && n_pad == 256 && (ldx % 4) == 0 && (ldy % 8) == 0 && ((uintptr_t)x % 16) == 0 &&
-      ((uintptr_t)y % 16) == 0 && (!colmask || ((uintptr_t)colmask % 16) == 0)) {
+  const float* xf = (const float*)x;
+  if (n == 256 && n_pad == 256 && (ldx % 4) == 0 && (ldy % 8) == 0 && ((uintptr_t)x % 16) == 0 && ((uintptr_t)y % 16) == 0 &&
+      (!colmask || ((uintptr_t)colmask % 16) == 0)) {
     constexpr int RW = 2;
     softmax_rows256_f32_kernel<RW><<<(unsigned)cdiv(rows, (long)wpb * RW), wpb * 32, 0, st>>>(
-        (const float*)x, ldx, (__half*)y, ldy, rows, scale, colmask, rows_per_batch, mask_value, keep_add);
+        xf, ldx, (__half*)y, ldy, rows, scale, colmask, rows_per_batch, mask_value, keep_add);
     return check_launch("softmax_rows256_f32_kernel");
   }
-  if (in_dtype == MQDET_F32 && n >= 4096 && rows <= 0x7fffffffL) {
-    softmax_longrows_f32_kernel<<<(unsigned)rows, 256, 0, st>>>((const float*)x, ldx, (__half*)y, ldy, (int)n, (int)n_pad, scale, colmask,
+  if (n >= 4096 && rows <= 0x7fffffffL) {
+    softmax_longrows_f32_kernel<<<(unsigned)rows, 256, 0, st>>>(xf, ldx, (__half*)y, ldy, (int)n, (int)n_pad, scale, colmask,
                                                                 rows_per_batch, mask_value, keep_add);
     return check_launch("softmax_longrows_f32_kernel");
   }
-  if (in_dtype == MQDET_F32)
-    softmax_rows_kernel<float><<<grid, wpb * 32, 0, st>>>((const float*)x, ldx, (__half*)y, ldy, rows, (int)n, (int)n_pad,
-                                                         scale, colmask, rows_per_batch, mask_value, keep_add);
-  else
-    softmax_rows_kernel<__half><<<grid, wpb * 32, 0, st>>>((const __half*)x, ldx, (__half*)y, ldy, rows, (int)n,
-                                                          (int)n_pad, scale, colmask, rows_per_batch, mask_value,
-                                                          keep_add);
+  softmax_rows_kernel<<<cdiv(rows, wpb), wpb * 32, 0, st>>>(xf, ldx, (__half*)y, ldy, rows, (int)n, (int)n_pad, scale, colmask,
+                                                           rows_per_batch, mask_value, keep_add);
   return check_launch("softmax_rows_kernel");
 }
 
@@ -1129,61 +621,4 @@ extern "C" int mqdet_cast_f16_f32(const void* x, float* y, int64_t n, void* stre
   if (blocks > 132 * 16) blocks = 132 * 16;
   cast_f16_f32_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)x, y, n);
   return check_launch("cast_f16_f32_kernel");
-}
-
-extern "C" int64_t mqdet_colsoftmax_workspace_floats(int64_t Z, int64_t N, int64_t T) {
-  const int64_t nchunks = (N + CS_ROWS - 1) / CS_ROWS;
-  return Z * nchunks * 2 * T + Z * 2 * T;
-}
-
-extern "C" int mqdet_colsoftmax_stats(const void* A, int64_t Z, int64_t N, int64_t T, float* workspace, void* stream) {
-  MQ_REQUIRE(A && workspace && Z > 0 && N > 0, "colsoftmax_stats: bad args");
-  MQ_REQUIRE(T > 0 && T <= 256 && (T % 8) == 0, "colsoftmax_stats: need T<=256, T%%8==0");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nchunks = (int)((N + CS_ROWS - 1) / CS_ROWS);
-  float* partial = workspace;
-  float* stat = workspace + Z * nchunks * 2 * T;
-  if ((T & (T - 1)) == 0 && ((uintptr_t)A % 16) == 0)
-    colsoftmax_stats_kernel<<<dim3(nchunks, (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)T, partial, nchunks);
-  else
-    colsoftmax_stats_generic_kernel<<<dim3(nchunks, (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)T, partial, nchunks);
-  colsoftmax_finish_kernel<<<(unsigned)Z, 256, 0, st>>>(partial, (int)T, nchunks, stat);
-  return check_launch("colsoftmax_stats");
-}
-
-extern "C" int mqdet_colstats_rowsoftmax(void* A, int64_t Z, int64_t N, int64_t T, const float* colmask, int64_t z_per_mask,
-                                         float mask_value, float keep_add, float* workspace, void* stream) {
-  MQ_REQUIRE(A && workspace && Z > 0 && N > 0, "colstats_rowsoftmax: bad args");
-  MQ_REQUIRE(T == 256, "colstats_rowsoftmax: T must be 256 (MODEL.LANGUAGE_BACKBONE.MAX_QUERY_LEN), got %ld", (long)T);
-  MQ_REQUIRE(((uintptr_t)A % 16) == 0 && (!colmask || z_per_mask >= 1), "colstats_rowsoftmax: A must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nchunks = (int)((N + CS_ROWS - 1) / CS_ROWS);
-  float* partial = workspace;
-  float* stat = workspace + Z * nchunks * 2 * T;
-  colstats_rowsoftmax256_kernel<<<dim3(nchunks, (unsigned)Z), 256, 0, st>>>((__half*)A, (int)N, partial, nchunks, colmask,
-                                                                           (int)(colmask ? z_per_mask : 1), mask_value, keep_add);
-  colsoftmax_finish_kernel<<<(unsigned)Z, 256, 0, st>>>(partial, (int)T, nchunks, stat);
-  return check_launch("colstats_rowsoftmax");
-}
-
-extern "C" int mqdet_colsoftmax_transposed(const void* A, int64_t Z, int64_t N, int64_t T, void* P, int64_t Np, float* workspace,
-                                           void* stream) {
-  MQ_REQUIRE(A && P && workspace && Z > 0 && N > 0, "colsoftmax_transposed: bad args");
-  MQ_REQUIRE(T > 0 && T <= 256 && (T % 8) == 0 && (Np % 8) == 0 && Np >= N, "colsoftmax_transposed: need T<=256, T%%8==0, Np%%8==0");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nchunks = (int)((N + CS_ROWS - 1) / CS_ROWS);
-  float* partial = workspace;
-  float* stat = workspace + Z * nchunks * 2 * T;
-  if ((T & (T - 1)) == 0 && ((uintptr_t)A % 16) == 0)
-    colsoftmax_stats_kernel<<<dim3(nchunks, (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)T, partial, nchunks);
-  else
-    colsoftmax_stats_generic_kernel<<<dim3(nchunks, (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)T, partial, nchunks);
-  colsoftmax_finish_kernel<<<(unsigned)Z, 256, 0, st>>>(partial, (int)T, nchunks, stat);
-  if (T == 256 && ((uintptr_t)A % 16) == 0)
-    colsoftmax_write_kernel<true><<<dim3((unsigned)((Np + 63) / 64), (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)Np,
-                                                                                             (int)T, stat, (__half*)P);
-  else
-    colsoftmax_write_kernel<false><<<dim3((unsigned)((Np + 63) / 64), (unsigned)Z), 256, 0, st>>>((const __half*)A, (int)N, (int)Np, (int)T,
-                                                                                       stat, (__half*)P);
-  return check_launch("colsoftmax_transposed");
 }

@@ -209,7 +209,8 @@ def add_layernorm(a, b, gamma, beta, eps, *, out16=True, out32=True, clamp=0.0):
 
 
 def softmax_rows(x, *, n=None, scale=1.0, colmask=None, rows_per_batch=0, mask_value=0.0, keep_add=0.0, out=None):
-    """Row softmax over the last dim of x [..., n_pad] (fp16/fp32, contiguous) -> fp16; cols >= n are zeroed."""
+    """Row softmax of fp32 scores over the last dim of x [..., n_pad] (contiguous) -> fp16; cols >= n are zeroed.  Other
+    dtypes raise MqdetError (mqdet_softmax_rows rejects them)."""
     global launch_count
     _need_cuda(x, colmask)
     n_pad = x.shape[-1]
@@ -338,66 +339,6 @@ def l2_normalize(x32, w=None, b0=None, eps=1e-12):
                                      _stream()), "l2norm_rowdot")
     launch_count += 1
     return e16, e32, dot
-
-
-def colsoftmax_transposed(A16, Np=None):
-    """A16 [..., N, T] fp16 -> P [..., T, Np] fp16 with P[t, n] = softmax over n of A[n, t] (zero for n >= N)."""
-    global launch_count
-    _need_cuda(A16)
-    N, T = A16.shape[-2], A16.shape[-1]
-    Z = A16.numel() // (N * T)
-    Np = (N + 7) // 8 * 8 if Np is None else Np
-    P = torch.empty(A16.shape[:-2] + (T, Np), dtype=torch.float16, device=A16.device)
-    ws = torch.empty((int(load().mqdet_colsoftmax_workspace_floats(Z, N, T)),), dtype=torch.float32, device=A16.device)
-    check(load().mqdet_colsoftmax_transposed(_ptr(A16), Z, N, T, _ptr(P), Np, _ptr(ws), _stream()), "colsoftmax_transposed")
-    launch_count += 3
-    return P
-
-
-def colsoftmax_stats(A16):
-    """A16 [..., N, T] fp16 -> stat [Z, 2, T] fp32 = (max over n, 1 / sum over n of exp(a - max)) per column."""
-    global launch_count
-    _need_cuda(A16)
-    N, T = A16.shape[-2], A16.shape[-1]
-    Z = A16.numel() // (N * T)
-    nws = int(load().mqdet_colsoftmax_workspace_floats(Z, N, T))
-    ws = torch.empty((nws,), dtype=torch.float32, device=A16.device)
-    check(load().mqdet_colsoftmax_stats(_ptr(A16), Z, N, T, _ptr(ws), _stream()), "colsoftmax_stats")
-    launch_count += 2
-    return ws[nws - Z * 2 * T:].view(Z, 2, T)  # the view keeps the workspace alive
-
-
-def colstats_rowsoftmax(A16, colmask, z_per_mask, mask_value, keep_add):
-    """T == 256.  One pass over A16 [..., N, 256] fp16: returns the column statistics [Z,2,T] of the scores (as
-    colsoftmax_stats) and overwrites every row with its masked softmax over the 256 tokens (as softmax_rows)."""
-    global launch_count
-    _need_cuda(A16, colmask)
-    N, T = A16.shape[-2], A16.shape[-1]
-    Z = A16.numel() // (N * T)
-    nws = int(load().mqdet_colsoftmax_workspace_floats(Z, N, T))
-    ws = torch.empty((nws,), dtype=torch.float32, device=A16.device)
-    check(load().mqdet_colstats_rowsoftmax(_ptr(A16), Z, N, T, _ptr(colmask), int(z_per_mask), float(mask_value),
-                                           float(keep_add), _ptr(ws), _stream()), "colstats_rowsoftmax")
-    launch_count += 2
-    return ws[nws - Z * 2 * T:].view(Z, 2, T)
-
-
-def biattn_text(kh, qh, vvT4, stat, clamp, out):
-    """Fused text->image attention: kh [B,H,T,d], qh [B,H,N,d], vvT4 [B,H,d,Np] fp16 (strided views), stat [B*H,2,T] fp32
-    (colsoftmax_stats of the clamped fp16 scores q.k^T), out [B,H,T,d] fp16 view <- softmax_n(scores)^T . Vv."""
-    global launch_count
-    _need_cuda(kh, qh, vvT4, stat, out)
-    B, H, T, d = kh.shape
-    N, Np = qh.shape[2], vvT4.shape[3]
-    for t in (kh, qh, vvT4, out):
-        if t.stride(3) != 1 or t.dtype != torch.float16:
-            raise _lib.MqdetError("biattn_text: fp16 operands with a contiguous last dimension required")
-    check(load().mqdet_biattn_text(_ptr(kh), kh.stride(2), kh.stride(1), kh.stride(0), _ptr(qh), qh.stride(2), qh.stride(1),
-                                   qh.stride(0), _ptr(vvT4), vvT4.stride(2), vvT4.stride(1), vvT4.stride(0), _ptr(stat),
-                                   float(clamp), _ptr(out), out.stride(2), out.stride(1), out.stride(0), H, B, T, N, Np, d,
-                                   _stream()), "biattn_text")
-    launch_count += 1
-    return out
 
 
 def biattn_image(vn16, gT, gbias, mT, bias, gamma, residual, mask, clamp, heads):

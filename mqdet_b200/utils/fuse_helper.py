@@ -60,11 +60,9 @@ class BiMultiHeadAttention(nn.Module):
         self.out_v_proj = nn.Linear(embed_dim, v_dim)
         self.out_l_proj = nn.Linear(embed_dim, l_dim)
         fc = cfg.MODEL.DYHEAD.FUSE_CONFIG if cfg is not None else None
-        self.fused_text_side = True  # False: column-softmax + GEMM path (kept for A/B checks, tests/test_fusion_gpu.py)
-        # "fused" (default): the product path; "f16": the score matrix A = q.k^T stored in fp16 (round-1 path, kept for
-        # A/B runs); "f32": diagnostic variant that keeps the
-        # scores in fp32 until both softmaxes have been taken, like the reference (fuse_helper.py:240-291) — twice the
-        # traffic, used by tests/test_parity_experiment_gpu.py to attribute the tower's end-to-end error
+        # "fused" (default): the product path (_attend_fused); "f32": the score matrices in fp32 in HBM until both softmaxes have
+        # been taken, like the reference (fuse_helper.py:240-291) — twice the traffic; the reference the product path is tested
+        # against, and the diagnostic mode of tests/test_parity_experiment_gpu.py.  Any other value is an error.
         self.score_precision = "fused"
         self.stable_softmax_2d = bool(fc.STABLE_SOFTMAX_2D if stable_softmax_2d is None else stable_softmax_2d)
         self.clamp_min_for_underflow = bool(fc.CLAMP_MIN_FOR_UNDERFLOW if clamp_min_for_underflow is None else clamp_min_for_underflow)
@@ -82,6 +80,25 @@ class BiMultiHeadAttention(nn.Module):
 
     SPLIT_K = 8
 
+    def _fused_applies(self, Cv, T):
+        """Whether the product path runs: ``score_precision == "fused"``, no STABLE_SOFTMAX_2D (its global maximum needs the
+        whole score tensor) and a shape inside the fused kernels' envelope (head dim 256, Cv = 256, T % 8 == 0, T <= 256,
+        H <= 8).  Everything else takes the explicit fp32-score path."""
+        if self.score_precision not in ("fused", "f32"):
+            raise ValueError(f"BiMultiHeadAttention.score_precision must be 'fused' or 'f32', got {self.score_precision!r}")
+        return (self.score_precision == "fused" and not self.stable_softmax_2d and self.head_dim == 256 and Cv == 256
+                and T % 8 == 0 and T <= 256 and self.num_heads <= 8)
+
+    def _score_clamp(self):
+        """The +-5e4 clamp of the scores (fuse_helper.py:245-252) as the kernels take it: 0 = none."""
+        return 50000.0 if (self.clamp_min_for_underflow or self.clamp_max_for_overflow) else 0.0
+
+    def _keys(self, ln16):
+        """k = LN(l) Wl^T + b  [B,T,H,d] fp16."""
+        B, T = ln16.shape[:2]
+        return ops.gemm(ln16.view(B * T, -1), w16(self.l_proj.weight), bias=f32(self.l_proj.bias)).view(B, T, self.num_heads,
+                                                                                                           self.head_dim)
+
     @torch.no_grad()
     def _attend(self, vn16, ln16, mask_l, v_epilogue=None, l_epilogue=None, mask_v=None):
         """vn16 [B,N,256] fp16, ln16 [B,T,768] fp16 (already layer-normed), mask_l [B,T] (1 keep / 0 padding) -> (dv, dl).
@@ -89,17 +106,16 @@ class BiMultiHeadAttention(nn.Module):
         ``mask_v`` [B,N] (1 keep / 0 padding; GroundingDINO's attention_mask_v) only on the explicit fp32-score path."""
         B, N, Cv = vn16.shape
         T = ln16.shape[1]
+        if self._fused_applies(Cv, T) and mask_v is None:
+            return self._attend_fused(vn16, ln16, mask_l, v_epilogue, l_epilogue)
         H, d, E = self.num_heads, self.head_dim, self.embed_dim
         dev = vn16.device
-        clamp = 50000.0 if (self.clamp_min_for_underflow or self.clamp_max_for_overflow) else 0.0
-        k = ops.gemm(ln16.view(B * T, -1), w16(self.l_proj.weight), bias=f32(self.l_proj.bias)).view(B, T, H, d)
+        k = self._keys(ln16)
         explicit = self.stable_softmax_2d or mask_v is not None
         # explicit path with many image tokens: the text-side P^T.V contracts over N with only B*H*T/128 output tiles, so it runs as
         # SPLIT_K K-slices (an extra GEMM batch dimension) -> N is padded to a multiple of 64 * SPLIT_K instead of 8
         split = self.SPLIT_K if (explicit and N >= 8192) else 1
         Np = (N + 64 * split - 1) // (64 * split) * (64 * split) if split > 1 else (N + 7) // 8 * 8
-        if not explicit and self.score_precision == "fused" and d == 256 and Cv == 256 and T % 8 == 0 and T <= 256 and H <= 8:
-            return self._attend_fused(vn16, ln16, k, mask_l, clamp, v_epilogue, l_epilogue)
         q = ops.gemm(vn16.view(B * N, Cv), w16(self.v_proj.weight), bias=f32(self.v_proj.bias), alpha=self.scale,
                      scale_after_bias=True).view(B, N, H, d)
         vvT = torch.empty((B, E, Np), dtype=torch.float16, device=dev)
@@ -110,37 +126,8 @@ class BiMultiHeadAttention(nn.Module):
         vlT = ops.gemm(w16(self.values_l_proj.weight), ln16, bias=f32(self.values_l_proj.bias), bias_mode=VEC_PER_ROW)
 
         qh, kh = q.permute(0, 2, 1, 3), k.permute(0, 2, 1, 3)
-        if self.score_precision == "f32" or explicit:
-            return self._finish(*self._attend_f32_scores(qh, kh, vvT, vlT, mask_l, clamp, B, N, T, Np, mask_v), v_epilogue,
-                                l_epilogue, B, N, T, Cv)
-        # scores A = clamp(Q_h K_h^T)  [B,H,N,T]  (ONE product serves both directions)
-        A = torch.empty((B, H, N, T), dtype=torch.float16, device=dev)
-        ops.gemm(qh, kh, out=A, clamp=clamp)
-        # text -> image direction first (A is normalised in place afterwards): softmax over all N locations, no mask.
-        ol = torch.empty((B, T, H, d), dtype=torch.float16, device=dev)
-        fused = self.fused_text_side and d == 256
-        cm = mask_l.float().contiguous() if mask_l is not None else None
-        if fused and T == 256:
-            # ONE pass over A: column statistics of the scores + the masked row softmax (image -> text probabilities) in
-            # place; then ONE fused kernel for the text -> image side: S^T = K Q^T recomputed on the tensor cores, exp,
-            # P.Vv -- the transposed probabilities [B,H,T,N] are never written
-            stat = ops.colstats_rowsoftmax(A, cm, H, -9e15, 1.0)
-            Pv = A
-            ops.biattn_text(kh, qh, vvT.view(B, H, d, Np), stat, clamp, ol.permute(0, 2, 1, 3))
-        else:
-            if fused:
-                stat = ops.colsoftmax_stats(A)
-                ops.biattn_text(kh, qh, vvT.view(B, H, d, Np), stat, clamp, ol.permute(0, 2, 1, 3))
-            else:
-                # unfused: probabilities written transposed [B,H,T,Np] so that P_l . Vv is a K-major x K-major product
-                Pl = ops.colsoftmax_transposed(A, Np)
-            # image -> text direction: softmax over the T tokens with the padding mask
-            Pv = ops.softmax_rows(A, colmask=cm, rows_per_batch=H * N, mask_value=-9e15, keep_add=1.0, out=A)
-        ov = torch.empty((B, N, H, d), dtype=torch.float16, device=dev)
-        ops.gemm(Pv, vlT.view(B, H, d, T), out=ov.permute(0, 2, 1, 3))
-        if not fused:
-            ops.gemm(Pl, vvT.view(B, H, d, Np), out=ol.permute(0, 2, 1, 3))
-        return self._finish(ov, ol, v_epilogue, l_epilogue, B, N, T, Cv)
+        return self._finish(*self._attend_f32_scores(qh, kh, vvT, vlT, mask_l, self._score_clamp(), B, N, T, Np, mask_v),
+                            v_epilogue, l_epilogue, B, N, T, Cv)
 
     def _query_fold_weights(self):
         """(scale * Wq)^T as fp16 [Cv, E] and scale * bq as fp16 [H, 8, d] (row 0 used), cached per parameter version: the B
@@ -155,7 +142,7 @@ class BiMultiHeadAttention(nn.Module):
             self._qfold = (key, wt, ops.cast_f16(bq))
         return self._qfold[1], self._qfold[2]
 
-    def _attend_fused(self, vn16, ln16, k, mask_l, clamp, v_epilogue, l_epilogue):
+    def _attend_fused(self, vn16, ln16, mask_l, v_epilogue, l_epilogue):
         """Product path: neither the queries q [B,N,E], the score matrix, its transpose, the per-head contexts nor the image-side
         value tensor reach HBM, and the scores stay fp32 until both softmaxes have been taken.  Three per-(image, head)
         operands of [256 x 256] fold the projections into the text side (tiny GEMMs over the T = 256 tokens):
@@ -166,10 +153,10 @@ class BiMultiHeadAttention(nn.Module):
           text side : ONE kernel = S^T recomputed from gT and the image tokens -> exp(. - column max) -> P^T . vn (the image
                       tokens themselves; the value projection follows as a small per-head GEMM because sum_n p[n] = 1) with
                       in-kernel column sums."""
-        dv, ctx = self._fused_image(vn16, ln16, k, mask_l, clamp, v_epilogue)
+        dv, ctx = self._fused_image(vn16, ln16, mask_l, v_epilogue)
         return dv, self._fused_text(ctx, l_epilogue)
 
-    def _fused_image(self, vn16, ln16, k, mask_l, clamp, v_epilogue):
+    def _fused_image(self, vn16, ln16, mask_l, v_epilogue):
         """Image side of the product path (see _attend_fused) -> (dv [B,N,Cv] fp16, context of the text side).  The text side
         only needs that context, so a caller may run it on another stream next to the visual branch (VLDyHead.forward_flat)."""
         B, N, Cv = vn16.shape
@@ -177,7 +164,8 @@ class BiMultiHeadAttention(nn.Module):
         H, d, E = self.num_heads, self.head_dim, self.embed_dim
         dev = vn16.device
         ve = v_epilogue or {}
-        kh = k.permute(0, 2, 1, 3)                                                     # [B,H,T,d]
+        clamp = self._score_clamp()
+        kh = self._keys(ln16).permute(0, 2, 1, 3)                                      # [B,H,T,d]
         wqT, bq8 = self._query_fold_weights()
         gT = torch.empty((B, H, T, Cv), dtype=torch.float16, device=dev)
         ops.gemm(kh, wqT.view(1, Cv, H, d).permute(0, 2, 1, 3), out=gT)                # gT[b,h,t,c] = sum_dd K[b,t,h,dd] scale Wq[h*d+dd, c]
@@ -305,18 +293,15 @@ class BiAttentionBlockForCheckpoint(nn.Module):
     def forward_flat_split(self, v16, l32, attention_mask_l):
         """forward_flat in two halves for two-stream execution: returns (v' fp16, ctx) after the image side; ``finish_text(ctx)``
         -> l' fp32 runs the text side (it depends on nothing the visual branch computes afterwards).  None when the product
-        path does not apply (A/B score precisions, unusual shapes)."""
+        path does not apply (score_precision "f32", unusual shapes)."""
         a = self.attn
         B, N, Cv = v16.shape
-        T = l32.shape[1]
-        if not (a.score_precision == "fused" and a.head_dim == 256 and Cv == 256 and T % 8 == 0 and T <= 256 and a.num_heads <= 8):
+        if not a._fused_applies(Cv, l32.shape[1]):
             return None
         nv, nl = self.layer_norm_v, self.layer_norm_l
         vn16 = ops.layernorm(v16, f32(nv.weight), f32(nv.bias), nv.eps)
         ln16, ln32 = ops.layernorm(l32, f32(nl.weight), f32(nl.bias), nl.eps, out16=True, out32=True)
-        clamp = 50000.0 if (a.clamp_min_for_underflow or a.clamp_max_for_overflow) else 0.0
-        k = ops.gemm(ln16.view(B * T, -1), w16(a.l_proj.weight), bias=f32(a.l_proj.bias)).view(B, T, a.num_heads, a.head_dim)
-        dv, ctx = a._fused_image(vn16, ln16, k, attention_mask_l, clamp, dict(gate=f32(self.gamma_v), residual=vn16))
+        dv, ctx = a._fused_image(vn16, ln16, attention_mask_l, dict(gate=f32(self.gamma_v), residual=vn16))
         ctx["ln32"] = ln32
         return dv.view(B, N, Cv), ctx
 

@@ -64,7 +64,7 @@ def add_layernorm(a, b, gamma, beta, eps, *, out16=True, out32=True, clamp=0.0):
     return y.half(), y
 ops.add_layernorm = add_layernorm
 def softmax_rows(x, *, n=None, scale=1.0, colmask=None, rows_per_batch=0, mask_value=0.0, keep_add=0.0, out=None):
-    assert x.is_contiguous()
+    assert x.is_contiguous() and x.dtype == torch.float32
     n_pad = x.shape[-1]; n = n_pad if n is None else n
     rows = x.numel() // n_pad
     v = x.float().reshape(rows, n_pad)[:, :n] * scale

@@ -57,7 +57,7 @@ def test_no_cpu_fallback():
         ops.layernorm(torch.zeros(2, 8), torch.ones(8), torch.zeros(8))
 
 
-def test_argument_validation_errors_without_gpu():
+def test_entry_points_reject_bad_arguments_without_gpu():
     """Every entry point validates its arguments BEFORE touching CUDA: a bad call returns a negative code and a message in
     mqdet_last_error() (mirrors the reference's AT_ERROR / TORCH_CHECK behaviour), also on a machine without a GPU."""
     import ctypes
@@ -81,8 +81,7 @@ def test_argument_validation_errors_without_gpu():
     g.K = g.lda = g.ldb = 16
     expect(lib.mqdet_gemm_f16(ctypes.byref(g), 7, nul), "unknown impl")
     expect(lib.mqdet_layernorm(nul, 0, 8, nul, nul, 1e-5, 1, 8, nul, nul, 8, 0, nul), "null pointer")
-    expect(lib.mqdet_colsoftmax_transposed(one, 1, 10, 12, one, 16, one, nul), "T%8")          # T % 8 != 0
-    expect(lib.mqdet_colstats_rowsoftmax(one, 1, 10, 128, nul, 1, 0.0, 0.0, one, nul), "T must be 256")
+    expect(lib.mqdet_softmax_rows(one, _lib.F16, 8, one, 8, 1, 8, 8, 1.0, nul, 0, 0.0, 0.0, nul), "fp32")   # fp16 scores
     expect(lib.mqdet_swin_window_attn(one, one, one, 1, 14, 14, 3, 8, 0, 1.0, one, nul), "window 7 (Swin-T) or 12 (Swin-L)")
     expect(lib.mqdet_biattn_image(one, 8, 8, one, 8, 8, 8, nul, 0, one, 8, 8, 8, nul, nul, nul, 0, 0, nul, 0.0, one, 8, 8, one,
                                   one, 1, 8, 100, 100, nul), "T % 8 == 0")
@@ -93,6 +92,4 @@ def test_argument_validation_errors_without_gpu():
     expect(lib.mqdet_dcn_conv(one, nul, 0, one, 5, 1, 128, 1, one, one, one, one, nul), "C must be 256")
     expect(lib.mqdet_dcn_conv(one, nul, 0, one, 5, 1, 256, 4, one, one, one, one, nul), "1..3 jobs")
     expect(lib.mqdet_conv3x3_small(one, one, one, one, 5, 1, 256, 40, one, 64, nul), "O <= 32")
-    expect(lib.mqdet_biattn_text(one, 8, 8, 8, one, 8, 8, 8, one, 8, 8, 8, one, 0.0, one, 8, 8, 8, 1, 1, 256, 100, 104, 128,
-                                 nul), "head dim must be 256")
     expect(lib.mqdet_contrastive_mask(one, one, 1, 1, 300, 256, nul), "bad args")                # Tmax < T

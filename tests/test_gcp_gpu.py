@@ -179,20 +179,6 @@ def test_preselect_vs_reference_golden(dev):
     assert err <= FP16_TOL * fx["vision_absmax"] + FP16_TOL, err
 
 
-def test_colsoftmax_transposed(dev):
-    """P[z][t][n] = softmax over n of A[z][n][t], zero-padded to a multiple of 8 along n (fuse_helper.py:257-268)."""
-    from mqdet_b200 import ops
-    g = torch.Generator().manual_seed(6)
-    for (Z, N, T) in [(3, 751, 256), (2, 1000, 64), (1, 70, 8)]:
-        A = (torch.randn(Z, N, T, generator=g) * 3).half()
-        P = ops.colsoftmax_transposed(A.to(dev))
-        Np = (N + 7) // 8 * 8
-        assert P.shape == (Z, T, Np)
-        ref = torch.softmax(A.float().transpose(1, 2), dim=-1)
-        assert_close(P[..., :N], ref, 1e-3, f"column softmax N={N} T={T}")
-        assert P[..., N:].abs().max().item() == 0 if Np > N else True
-
-
 def test_dense_cross_attention_flash_equals_unfused(dev):
     """PreSelect's dense MaskedCrossAttention: the flash-style kernel (online softmax over 64-token chunks, scores never in
     HBM) against the unfused GEMM / softmax_rows / GEMM path and plain torch, ragged query and key counts."""

@@ -5,8 +5,8 @@ layer on the GPU next to the fp32 CPU oracle, twice per attention-score precisio
   * free-running  : every GPU stage consumes the previous GPU stage's output -> the accumulated error after each stage;
   * teacher-forced: every GPU stage consumes the ORACLE's input of that stage (rounded to the stage's storage type) ->
                     the error each stage adds on its own.
-Score precisions (``BiMultiHeadAttention.score_precision``): "fused" = the product path, "f16" = the round-1 fp16-stored score
-matrix, "f32" = diagnostic fp32 score matrix in HBM.  Results go to parity_experiment.json in the run's output directory.
+Score precisions (``BiMultiHeadAttention.score_precision``): "fused" = the product path, "f32" = diagnostic fp32 score
+matrix in HBM.  Results go to parity_experiment.json in the run's output directory.
 """
 import json
 import os
@@ -26,7 +26,7 @@ def _mean_rel(out, ref):
     return (out - ref).abs().mean().item() / (ref.abs().mean().item() + 1e-12)
 
 
-def test_tower_error_attribution(dev):
+def test_tower_error_attribution_fused_and_f32(dev):
     from mqdet_b200 import ops
     from mqdet_b200.config import mq_glip_t_cfg
     from mqdet_b200.modeling.language_backbone.modeling_bert_new import BertLayer
@@ -45,7 +45,7 @@ def test_tower_error_attribution(dev):
     lv = ops.Levels(SIZES, dev)
     cm = masks.float().to(dev)
     report = {}
-    modes = ["fused", "f16", "f32"]
+    modes = ["fused", "f32"]
     for mode in modes:
         for i in range(0, len(head.dyhead_tower), 3):
             head.dyhead_tower[i].b_attn.attn.score_precision = mode

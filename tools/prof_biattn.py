@@ -1,7 +1,7 @@
-"""One BiAttention fusion layer at the bench size (B=8, N=22400 image tokens, T=256) for ncu captures of the fused
-text->image kernel (biattn_text_kernel), the one-pass statistics/softmax kernel and the z-batched GEMMs:
-    ncu --set full --import-source on --clock-control none -k regex:biattn_text -c 1 -o gpurun_out/r01_biattn python tools/prof_biattn.py
-Without ncu it prints CUDA-event times of the layer."""
+"""One BiAttention fusion layer (BiAttentionBlockForCheckpoint.forward_flat) at the bench size (B=8, N=22400 image tokens,
+T=256) on the product path: the layer norms, the small projection GEMMs, biattn_image_kernel and biattn_text_kernel.
+    python tools/prof_biattn.py [reps]
+runs the layer `reps` times (default 1) and, for reps > 1, prints its mean time per call from CUDA events."""
 import os
 import sys
 
