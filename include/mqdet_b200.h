@@ -488,6 +488,35 @@ int mqdet_atss_loss(const float* logits, const float* reg_ctr, const int32_t* ma
                     float gamma, float reg_weight, float token_weight, float* workspace, float* losses, float* d_logits, float* d_reg_ctr,
                     void* stream);
 
+/* ---- GroundingDINO Hungarian matching and set-prediction losses (groundingdino_new/models/GroundingDINO/matcher.py :49-86,
+ * loss.py SetCriterion :42-178) ---------------------------------------------------------------------------------------------
+ * Decoder outputs of L layers: logits f32 [L][B][Q][T] (raw, -inf outside the text mask), boxes f32 [L][B][Q][4] (sigmoid cxcywh).
+ * GTs come as a fixed-capacity pack: gt_boxes f32 [B][Gmax][4] (normalised cxcywh), gt_count i32 [B] (device; entries >= gt_count[b]
+ * are ignored), gt_tokens f32 [B][Gmax][T] (the positive-map rows).  1 <= Gmax <= Q.
+ *   mqdet_gdino_match_cost      : cost f32 [L][B][Q][Gmax] = cost_bbox * L1 + cost_class * focal class cost - cost_giou * GIoU
+ *                                 (0 for g >= gt_count[b]); norm f32 [1] (optional) = sum_b gt_count[b], the normaliser that
+ *                                 data-parallel ranks all-reduce (sum) before mqdet_gdino_set_loss.
+ *   mqdet_linear_sum_assignment : for each p < P, scipy.optimize.linear_sum_assignment of cost[p][:, :G] (cost f32 [P][Q][Gmax],
+ *                                 G = counts[p % ncounts]) -> match i32 [P][Q] = the column assigned to row q, or -1.  Index for
+ *                                 index scipy's result, ties included.  Q <= 4096; finite costs.
+ *                                 workspace: mqdet_linear_sum_assignment_workspace_bytes
+ *   mqdet_gdino_set_loss        : losses f32 [L][3] = (loss_ce, loss_bbox, loss_giou) per layer, each already multiplied by its
+ *                                 weight; d_logits f32 [L][B][Q][T] and d_boxes f32 [L][B][Q][4] = the gradient of their sum.
+ *                                 match i32 [L][B][Q]; text_mask f32 [B][T] (> 0 = in use) or NULL; world = number of ranks that
+ *                                 summed norm.  workspace: mqdet_gdino_set_loss_workspace_floats
+ * No host synchronisation; reductions are deterministic. */
+int mqdet_gdino_match_cost(const float* logits, const float* boxes, const float* gt_boxes, const int32_t* gt_count, const float* gt_tokens,
+                           int64_t L, int64_t B, int64_t Q, int64_t T, int64_t Gmax, float alpha, float cost_class, float cost_bbox,
+                           float cost_giou, float* cost, float* norm, void* stream);
+int64_t mqdet_linear_sum_assignment_workspace_bytes(int64_t P, int64_t Q, int64_t Gmax);
+int mqdet_linear_sum_assignment(const float* cost, const int32_t* counts, int64_t ncounts, int64_t P, int64_t Q, int64_t Gmax,
+                                void* workspace, int32_t* match, void* stream);
+int64_t mqdet_gdino_set_loss_workspace_floats(int64_t L, int64_t B, int64_t Q);
+int mqdet_gdino_set_loss(const float* logits, const float* boxes, const int32_t* match, const float* gt_boxes, const float* gt_tokens,
+                         int64_t L, int64_t B, int64_t Q, int64_t T, int64_t Gmax, const float* text_mask, const float* norm, float world,
+                         float alpha, float gamma, float w_ce, float w_bbox, float w_giou, float* workspace, float* losses, float* d_logits,
+                         float* d_boxes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -163,6 +163,14 @@ SIGNATURES = {
     "mqdet_atss_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                 c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_float, c_void_p,
                                 c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_gdino_match_cost": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
+                                       c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p]),
+    "mqdet_linear_sum_assignment_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
+    "mqdet_linear_sum_assignment": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
+    "mqdet_gdino_set_loss_workspace_floats": (c_int64, [c_int64, c_int64, c_int64]),
+    "mqdet_gdino_set_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
+                                     c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_float, c_float, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -78,7 +78,8 @@ def mq_groundingdino_t_cfg(**over):
         transformer_activation="relu", dec_pred_bbox_embed_share=True, embed_init_tgt=True, max_text_len=256,
         text_encoder_type="bert-base-uncased", use_text_enhancer=True, use_fusion_layer=True, use_checkpoint=False,
         use_transformer_ckpt=False, use_text_cross_attention=True, text_dropout=0.0, fusion_dropout=0.0, fusion_droppath=0.1,
-        sub_sentence_present=True, box_threshold=0.05)
+        sub_sentence_present=True, box_threshold=0.05, focal_alpha=0.25, loss_ce_coef=2.0, loss_bbox_coef=5.0, loss_giou_coef=2.0,
+        matcher=NS(matcher_type="HungarianMatcher", set_cost_class=1.0, set_cost_bbox=5.0, set_cost_giou=2.0, focal_alpha=0.25))
     for k, v in base.items():
         if k.startswith("GROUNDINGDINO."):
             setattr(cfg.GROUNDINGDINO, k.split(".", 1)[1], v)

@@ -9,6 +9,11 @@ that touches a TRAINABLE parameter.
                                                           ``parallel.all_reduce_loss_normalizers`` -> ``ops.atss_loss`` = losses +
                                                           d(logits), d(box / centerness output) on the device
       backward through the frozen fusion tower            NOT built (DESIGN.md §1 row f2) — the caller supplies dL/d(hidden)
+    GroundingDINO (config 4): out = decoder outputs,     ``GroundingDINO.decoder_outputs_flat`` (all layers, one MLP chain / one
+      SetCriterion(out, targets, text_mask, pos_map)      contrastive product) -> ``SetCriterion.forward_flat``: ``ops.gdino_match``
+      (HungarianMatcher + scipy, L1 / GIoU / token        (cost + on-device linear sum assignment) -> ``parallel.all_reduce_loss_
+      focal losses per decoder layer)                     normalizers`` -> ``ops.gdino_set_loss`` = losses + d(logits), d(boxes)
+                                                          of every layer on the device; the backward into the decoder: NOT built
     scaler.scale(losses).backward()                      ``QVBertModelTrain.backward(d_hidden)`` -> gradients of all 119 trainable tensors
     DDP gradient all-reduce                               ``parallel.all_reduce_gradients`` (ONE flat NCCL all-reduce, averaged)
     clip_grad_norm_ + AdamW per parameter group           ``FusedAdamW.step`` (norm, clip coefficient, updates: all on the device)

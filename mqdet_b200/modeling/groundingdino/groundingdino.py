@@ -1,6 +1,7 @@
 """MQ-GroundingDINO-T forward on sm_90a kernels, drop-in for groundingdino_new/models/GroundingDINO/groundingdino.py:93-709
 (``GroundingDINO``), backbone/backbone.py:155-221 (``Joiner`` of Swin-T + ``PositionEmbeddingSineHW``) and bertwarper.py:28-223
-(``BertModelWarper`` around the vision-conditioned ``QVBertModel``), inference only (BASELINE config 4).
+(``BertModelWarper`` around the vision-conditioned ``QVBertModel``), inference (BASELINE config 4), plus the decoder outputs of every
+layer and the set-prediction losses of the training branch (``decoder_outputs``, ``loss_evaluator``; groundingdino.py:590-641).
 
     images -> Swin-T (3 outputs) -> input_proj (1x1 conv + GroupNorm(32); one extra 3x3 stride-2 level) -> 4 levels of 256 channels
     prompt -> QuerySelector (vision queries) + token ids -> per-category text masks -> QVBertModel (PreSelect + GCP) -> feat_map
@@ -29,6 +30,8 @@ from ..language_backbone.modeling_bert_new import QVBertModel
 from ..query_selector.query_selector import QuerySelector
 from ..rpn.vldyhead import _conv_w16
 from .bertwarper import generate_masks_with_special_tokens_and_transfer_map
+from .loss import SetCriterion
+from .matcher import build_matcher
 from .transformer import Transformer
 from .utils import MLP, ContrastiveEmbed
 
@@ -134,6 +137,8 @@ class GroundingDINO(nn.Module):
                                  sampling_ratio=rb.POOLER_SAMPLING_RATIO, use_v2=True)
         self._prompt = None
         self._geo = None
+        # loss criterion (groundingdino.py:152); no parameters, so the state_dict keys are unchanged
+        self.loss_evaluator = SetCriterion(build_matcher(g.matcher), cfg)
 
     # ---- vision-query bank extraction (groundingdino.py:340-430) ------------------------------------------------------
     @torch.no_grad()
@@ -304,7 +309,41 @@ class GroundingDINO(nn.Module):
         return {"det_packed": packed, "det": packed[:, :nq], "num": packed[:, nq, 0], "pred_logits": logits, "pred_boxes": boxes,
                 "image_sizes": images.image_sizes, "hs": hs, "references": refs, "srcs": src32, "level_sizes": sizes,
                 "encoded_text": enc_text, "bert_hidden": h, "transformer": tr,
-                "vision_query_gates": bert["vision_query_gates"]}
+                "vision_query_gates": bert["vision_query_gates"], "valid_ratios": geo["valid_ratios"],
+                "text_token_mask": st["token_mask"]}
+
+    @torch.no_grad()
+    def decoder_outputs_flat(self, out):
+        """Class logits and boxes of EVERY decoder layer from ``forward_device(..., all_layers=True)`` (groundingdino.py:590-607)
+        -> (pred_logits fp32 [L, B, Q, 256], -inf outside the text mask; pred_boxes fp32 [L, B, Q, 4], sigmoid cxcywh, layer k =
+        sigmoid(bbox_embed(hs[k]) + inverse_sigmoid(references[k]))).  ``bbox_embed`` is shared across the layers and the text
+        operand of ``ContrastiveEmbed`` is the same for all of them, so the L layers' rows go through ONE MLP chain and ONE
+        contrastive product per image.  Layer L-1 equals ``out["pred_logits"]`` / ``out["pred_boxes"]`` bit for bit."""
+        hs, refs = out["hs"], out["references"]
+        L = len(hs)
+        if L != len(refs) - 1:
+            raise ValueError("decoder_outputs needs the hidden states of every layer: call forward_device(..., all_layers=True)")
+        B, nq, E = hs[0].shape
+        hs16 = ops.cast_f16(torch.stack(hs, 1).contiguous())                                 # [B, L, nq, E], rows (b, l, q)
+        delta = self.bbox_embed[-1](hs16.view(B * L * nq, E), out_dtype=torch.float32)
+        ref = torch.stack(refs[:L], 1).contiguous().view(B * L, nq, 4)
+        vr = out["valid_ratios"].repeat_interleave(L, dim=0)
+        boxes, _, _ = ops.box_refine_sine(ref, vr, delta=delta.view(B * L, nq, -1), want_sine=False)
+        tr = out["transformer"]
+        text_dict = {"encoded_text": tr["memory_text"], "encoded_text16": tr["memory_text16"], "text_token_mask": out["text_token_mask"]}
+        logits = self.class_embed[-1](hs16.view(B, L * nq, E), text_dict)                      # [B, L*nq, 256]
+        logits = logits.view(B, L, nq, -1).transpose(0, 1).contiguous()
+        boxes = boxes.view(B, L, nq, 4).transpose(0, 1).contiguous()
+        return logits, boxes
+
+    def decoder_outputs(self, out):
+        """The reference's training-branch ``out`` dict (groundingdino.py:609-611): {"pred_logits" [B, Q, 256], "pred_boxes"
+        [B, Q, 4] of the last layer, "aux_outputs": [{"pred_logits", "pred_boxes"} of layers 0..L-2]}, views of
+        ``decoder_outputs_flat``."""
+        logits, boxes = self.decoder_outputs_flat(out)
+        L = logits.shape[0]
+        return {"pred_logits": logits[L - 1], "pred_boxes": boxes[L - 1],
+                "aux_outputs": [{"pred_logits": logits[k], "pred_boxes": boxes[k]} for k in range(L - 1)]}
 
     @staticmethod
     def to_boxlists(packed, image_sizes):

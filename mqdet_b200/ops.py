@@ -864,6 +864,111 @@ def atss_loss(logits, reg_ctr, gt_boxes, gt_labels, gt_count, gt_tokens, levels,
     return losses, d_logits, d_reg_ctr
 
 
+def _gdino_gt_pack(gt_boxes, gt_count, gt_tokens, B, Q, T):
+    """Validates the GroundingDINO GT pack (``atss_targets`` convention, boxes normalised cxcywh) -> contiguous tensors + Gmax."""
+    _need_cuda(gt_boxes, gt_count, gt_tokens)
+    if gt_boxes.dim() != 3 or gt_boxes.shape[0] != B or gt_boxes.shape[2] != 4:
+        raise ValueError(f"gt_boxes must be [B={B}, Gmax, 4]; got {tuple(gt_boxes.shape)}")
+    G = gt_boxes.shape[1]
+    if tuple(gt_count.shape) != (B,) or tuple(gt_tokens.shape) != (B, G, T):
+        raise ValueError(f"gt_count must be [B] = ({B},) and gt_tokens [B, Gmax, T] = {(B, G, T)}; got {tuple(gt_count.shape)}, "
+                         f"{tuple(gt_tokens.shape)}")
+    if G < 1 or G > Q:
+        raise ValueError(f"GT capacity Gmax={G} must be in 1..Q={Q}")
+    return gt_boxes.float().contiguous(), gt_count.to(torch.int32).contiguous(), gt_tokens.float().contiguous(), G
+
+
+def _decoder_outputs(pred_logits, pred_boxes):
+    _need_cuda(pred_logits, pred_boxes)
+    if pred_logits.dim() != 4 or pred_boxes.dim() != 4 or pred_boxes.shape[:3] != pred_logits.shape[:3] or pred_boxes.shape[3] != 4:
+        raise ValueError(f"pred_logits [L, B, Q, T] and pred_boxes [L, B, Q, 4] required; got {tuple(pred_logits.shape)}, "
+                         f"{tuple(pred_boxes.shape)}")
+    for t in (pred_logits, pred_boxes):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise _lib.MqdetError("gdino: pred_logits / pred_boxes must be contiguous fp32")
+    return pred_logits.shape
+
+
+def linear_sum_assignment(cost, counts):
+    """``scipy.optimize.linear_sum_assignment`` of a batch of cost matrices on the device, index for index scipy's result (ties
+    included): cost fp32 [P, Q, Gmax], counts [P] (device) -> match int32 [P, Q] = the column (GT) assigned to row (query) q of
+    ``cost[p, :, :counts[p]]``, -1 for unassigned rows.  Requires counts[p] <= Gmax <= Q (rows >= columns) and finite costs."""
+    _need_cuda(cost, counts)
+    if cost.dim() != 3 or cost.dtype != torch.float32:
+        raise ValueError(f"cost must be fp32 [P, Q, Gmax]; got {cost.dtype} {tuple(cost.shape)}")
+    P, Q, G = cost.shape
+    if tuple(counts.shape) != (P,):
+        raise ValueError(f"counts must be [P] = ({P},); got {tuple(counts.shape)}")
+    if G < 1 or G > Q:
+        raise ValueError(f"Gmax={G} must be in 1..Q={Q}")
+    return _lsa(cost.contiguous(), counts.to(torch.int32).contiguous(), P, Q, G)
+
+
+def _lsa(cost, counts, P, Q, G):
+    global launch_count
+    ws = torch.empty((int(load().mqdet_linear_sum_assignment_workspace_bytes(P, Q, G)),), dtype=torch.uint8, device=cost.device)
+    match = torch.empty((P, Q), dtype=torch.int32, device=cost.device)
+    check(load().mqdet_linear_sum_assignment(_ptr(cost), _ptr(counts), counts.shape[0], P, Q, G, _ptr(ws), _ptr(match), _stream()),
+          "linear_sum_assignment")
+    launch_count += 2
+    return match
+
+
+def gdino_match(pred_logits, pred_boxes, gt_boxes, gt_count, gt_tokens, *, cost_class=1.0, cost_bbox=5.0, cost_giou=2.0,
+                focal_alpha=0.25):
+    """HungarianMatcher (matcher.py:49-86) of every decoder layer on the device: pred_logits fp32 [L, B, Q, T] (raw), pred_boxes fp32
+    [L, B, Q, 4] (sigmoid cxcywh), GT pack gt_boxes [B, Gmax, 4] (normalised cxcywh), gt_count [B], gt_tokens [B, Gmax, T] ->
+    dict(cost fp32 [L, B, Q, Gmax] (0 beyond gt_count), match int32 [L, B, Q] (matched GT or -1), norm fp32 [1] = sum of gt_count,
+    the normaliser data-parallel ranks all-reduce).  No host synchronisation: capturable in a CUDA graph at a fixed Gmax."""
+    global launch_count
+    L, B, Q, T = _decoder_outputs(pred_logits, pred_boxes)
+    gt_boxes, gt_count, gt_tokens, G = _gdino_gt_pack(gt_boxes, gt_count, gt_tokens, B, Q, T)
+    dev = pred_logits.device
+    cost = torch.empty((L, B, Q, G), dtype=torch.float32, device=dev)
+    norm = torch.empty((1,), dtype=torch.float32, device=dev)
+    with _Timed("gdino_match_cost", 2.0 * L * B * Q * T * G, 4.0 * L * B * Q * (T + G)):
+        check(load().mqdet_gdino_match_cost(_ptr(pred_logits), _ptr(pred_boxes), _ptr(gt_boxes), _ptr(gt_count), _ptr(gt_tokens), L, B, Q,
+                                            T, G, float(focal_alpha), float(cost_class), float(cost_bbox), float(cost_giou),
+                                            _ptr(cost), _ptr(norm), _stream()), "gdino_match_cost")
+    launch_count += 1
+    match = _lsa(cost.view(L * B, Q, G), gt_count, L * B, Q, G).view(L, B, Q)
+    return {"cost": cost, "match": match, "norm": norm}
+
+
+def gdino_set_loss(pred_logits, pred_boxes, gt_boxes, gt_count, gt_tokens, text_mask=None, *, targets=None, world=1, alpha=0.25,
+                   gamma=2.0, ce_coef=2.0, bbox_coef=5.0, giou_coef=2.0, cost_class=1.0, cost_bbox=5.0, cost_giou=2.0, focal_alpha=0.25):
+    """SetCriterion (loss.py:42-178) of every decoder layer on the device, with its gradients at the decoder outputs.
+
+    Inputs as ``gdino_match``, plus text_mask [B, T] (> 0 = token in use) or None.  ``targets``: the result of ``gdino_match``
+    (its ``norm`` summed over ``world`` ranks), else computed here for one rank.  -> (losses fp32 [L, 3] = (loss_ce, loss_bbox,
+    loss_giou) per layer, already weighted; d_logits fp32 [L, B, Q, T], d_boxes fp32 [L, B, Q, 4] = the gradient of their sum;
+    norm fp32 [1], the device-resident normaliser).  Row L-1 is the reference's un-suffixed keys, row k < L-1 its ``_k`` keys."""
+    global launch_count
+    L, B, Q, T = _decoder_outputs(pred_logits, pred_boxes)
+    gt_boxes, gt_count, gt_tokens, G = _gdino_gt_pack(gt_boxes, gt_count, gt_tokens, B, Q, T)
+    _need_cuda(text_mask)
+    if text_mask is not None and tuple(text_mask.shape) != (B, T):
+        raise ValueError(f"text_mask must be [B, T] = {(B, T)}; got {tuple(text_mask.shape)}")
+    if targets is None:
+        targets = gdino_match(pred_logits, pred_boxes, gt_boxes, gt_count, gt_tokens, cost_class=cost_class, cost_bbox=cost_bbox,
+                              cost_giou=cost_giou, focal_alpha=focal_alpha)
+    if tuple(targets["match"].shape) != (L, B, Q):
+        raise ValueError(f"targets['match'] must be [L, B, Q] = {(L, B, Q)}; got {tuple(targets['match'].shape)}")
+    dev = pred_logits.device
+    tm = None if text_mask is None else text_mask.float().contiguous()
+    ws = torch.empty((int(load().mqdet_gdino_set_loss_workspace_floats(L, B, Q)),), dtype=torch.float32, device=dev)
+    losses = torch.empty((L, 3), dtype=torch.float32, device=dev)
+    d_logits = torch.empty_like(pred_logits)
+    d_boxes = torch.empty_like(pred_boxes)
+    with _Timed("gdino_set_loss", 0.0, 8.0 * L * B * Q * T + 32.0 * L * B * Q):
+        check(load().mqdet_gdino_set_loss(_ptr(pred_logits), _ptr(pred_boxes), _ptr(targets["match"]), _ptr(gt_boxes), _ptr(gt_tokens),
+                                          L, B, Q, T, G, _ptr(tm), _ptr(targets["norm"]), float(world), float(alpha), float(gamma),
+                                          float(ce_coef), float(bbox_coef), float(giou_coef), _ptr(ws), _ptr(losses), _ptr(d_logits),
+                                          _ptr(d_boxes), _stream()), "gdino_set_loss")
+    launch_count += 3
+    return losses, d_logits, d_boxes, targets["norm"]
+
+
 def anchors(grid_h, grid_w, stride, size, img_w, img_h, device):
     """Anchors [H*W, 4] + visibility [H*W] of one level (anchor_generator.py:72-109)."""
     import numpy as np

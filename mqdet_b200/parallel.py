@@ -88,9 +88,13 @@ def all_gather_chunks(packed_local, num_chunks, group=None):
 
 
 def all_reduce_loss_normalizers(buf, group=None):
-    """The ATSS loss normalisers (number of positives, sum of centerness targets; loss.py:1149-1151, :1188) summed over the ranks
-    in place with ONE collective, between the target assignment and the losses: ``buf`` = ``ops.atss_targets(...)["norm"][:2]``
-    (a view: the rank-local copies in ``norm[2:]`` stay untouched).  Identity when no process group is initialised."""
+    """A device-resident loss-normaliser buffer summed over the ranks in place with ONE collective, between the target assignment
+    and the losses; the loss kernels then divide by ``world`` themselves.  Users:
+      * ATSS (number of positives, sum of centerness targets; rpn/loss.py:1149-1151, :1188): ``buf`` =
+        ``ops.atss_targets(...)["norm"][:2]`` (a view: the rank-local copies in ``norm[2:]`` stay untouched);
+      * GroundingDINO's SetCriterion (number of GT boxes, GroundingDINO/loss.py:132-136): ``buf`` = ``ops.gdino_match(...)["norm"]``;
+        ``ops.gdino_set_loss`` then uses max(sum / world, 1).
+    Identity when no process group is initialised."""
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return buf
     dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
