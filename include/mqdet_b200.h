@@ -353,12 +353,16 @@ int mqdet_ms_deform_attn(const void* value, const float* proj, int64_t proj_ld, 
 
 /* ---- GroundingDINO variant, small device ops (SURVEY.md §8 f1) --------------------------------------------------
  * STABLE_SOFTMAX_2D of BiMultiHeadAttention (groundingdino_new/models/GroundingDINO/fuse_modules.py:177-187): the global
- * maximum of the score tensor is subtracted before the +-5e4 clamps.
- *   mqdet_global_max_f32 : out[0] = max_i x[i] (two deterministic launches; workspace: mqdet_global_max_workspace_floats())
- *   mqdet_shift_clamp_f32: x[i] = clamp(x[i] - *shift, lo, hi) in place, shift a DEVICE scalar (no host sync) */
-int64_t mqdet_global_max_workspace_floats(void);
-int mqdet_global_max_f32(const float* x, int64_t n, float* out, float* workspace, void* stream);
-/* the same shift + clamps fused into the row softmax (one pass less over the scores): y = softmax_j(clamp(x - *shift_dev, lo, hi) + mask),
+ * maximum of the score tensor is subtracted before the +-5e4 clamps.  Prompt chunks batched as elements need that maximum per
+ * element (the reference runs one chunk per forward), hence the segments / per-shift strides (0 = one value for everything).
+ *   mqdet_global_max_f32 : out[s] = max of x[s * n / segments, (s + 1) * n / segments), n % segments == 0 (one pass over x + one
+ *                          tiny launch, deterministic; workspace: mqdet_global_max_workspace_floats(segments))
+ *   mqdet_shift_clamp_f32: x[i] = clamp(x[i] - shift[elems_per_shift ? i / elems_per_shift : 0], lo, hi) in place, shift on the
+ *                          DEVICE (no host sync) */
+int64_t mqdet_global_max_workspace_floats(int64_t segments);
+int mqdet_global_max_f32(const float* x, int64_t n, int64_t segments, float* out, float* workspace, void* stream);
+/* the same shift + clamps fused into the row softmax (one pass less over the scores):
+ * y[r] = softmax_j(clamp(x[r] - shift_dev[rows_per_shift ? r / rows_per_shift : 0], lo, hi) + mask),
  * fp32 rows of n == n_pad == 256 (image -> text side) or n >= 4096 (text -> image side); mask arguments as mqdet_softmax_rows */
 /* reduction of a split-K product whose K slices ran as an extra batch dimension of mqdet_gemm_f16: part f32 [nb2][nb1][S][R][C] ->
  * out16[z2 * o_s2 + z1 * o_s1 + r * ldo + c] = f16(sum_s part[z2][z1][s][r][c]); C % 4 == 0 */
@@ -366,9 +370,9 @@ int mqdet_sum_splits_cast(const float* part, int64_t nb2, int64_t nb1, int64_t S
                           int64_t ldo, void* stream);
 int mqdet_softmax_rows_shifted_supported(int64_t n, int64_t n_pad);
 int mqdet_softmax_rows_shifted(const float* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int64_t n, int64_t n_pad,
-                               const float* shift_dev, float lo, float hi, const float* colmask, int64_t rows_per_batch, float mask_value,
-                               float keep_add, void* stream);
-int mqdet_shift_clamp_f32(float* x, int64_t n, const float* shift, float lo, float hi, void* stream);
+                               const float* shift_dev, int64_t rows_per_shift, float lo, float hi, const float* colmask,
+                               int64_t rows_per_batch, float mask_value, float keep_add, void* stream);
+int mqdet_shift_clamp_f32(float* x, int64_t n, const float* shift, int64_t elems_per_shift, float lo, float hi, void* stream);
 /* Two-stage query selection (transformer.py:288-318): topk_logits = enc_outputs_class.max(-1)[0]; torch.topk(.., 900, dim=1);
  * torch.gather of the selected rows.
  *   mqdet_row_max_f32   : out[r] = max_j x[r*ld + j], j < D
@@ -394,8 +398,11 @@ int mqdet_gather_rows_f32(const float* src, const int64_t* idx, int64_t B, int64
  *                            sine16[b][q][512]  = gen_sineembed_for_position(ref_input[:, :, 0, :])  (utils.py:203-232), optional
  *                          delta [B*nq][ldd] f32 or NULL; ref_in / ref_out [B*nq][4]; valid_ratios [B][L][2]; ref_out optional.
  *   mqdet_gdino_detections: convert_groundingdino_to_glip_output (groundingdino.py:291-335) for raw class logits [B][nq][T] f32
- *                          (-inf on padding): sigmoid, per-class mean over its tokens (tokmap int32 [C][max_tok], -1 padded),
- *                          best class (lowest index on ties), keep if score > box_threshold, boxes cxcywh (normalised) -> xyxy in
+ *                          (-inf on padding): sigmoid, per-class mean over its tokens (tokmap int32 [C][max_tok], -1 padded;
+ *                          one table for the batch (tokmap_img_stride 0) or one per element, stride in int32 elements: prompt
+ *                          chunks batched as elements), best class (lowest column on ties; label = class_labels[column] of the
+ *                          element (labels_img_stride 0: shared [C]) with the columns in ascending label order, or column + 1
+ *                          when class_labels is NULL), keep if score > box_threshold, boxes cxcywh (normalised) -> xyxy in
  *                          pixels of img_wh[b] = (W, H), clipped to [0, W-1] x [0, H-1], boxes with a negative side dropped; kept rows in
  *                          query order -> out [B][max_out + 1][6] = (x1, y1, x2, y2, score, label), row max_out = (count, 0, ...);
  *                          workspace: mqdet_gdino_detections_workspace_floats. */
@@ -407,8 +414,8 @@ int mqdet_groupnorm_rows(const void* x, int x_dtype, int64_t B, int64_t HW, int6
 int mqdet_box_refine_sine(const float* delta, int64_t ldd, const float* ref_in, int ref_is_logit, const float* valid_ratios, int64_t B,
                           int64_t nq, int64_t L, float* ref_out, float* ref_input, void* sine16, void* stream);
 int64_t mqdet_gdino_detections_workspace_floats(int64_t B, int64_t nq);
-int mqdet_gdino_detections(const float* logits, int64_t T, const float* boxes, const int32_t* tokmap, int64_t C, int64_t max_tok,
-                           const float* img_wh, float box_threshold, int64_t B, int64_t nq, int64_t max_out, float* out,
+int mqdet_gdino_detections(const float* logits, int64_t T, const float* boxes, const int32_t* tokmap, int64_t tokmap_img_stride,
+                           const int32_t* class_labels, int64_t labels_img_stride, int64_t C, int64_t max_tok, const float* img_wh, float box_threshold, int64_t B, int64_t nq, int64_t max_out, float* out,
                            float* workspace, void* stream);
 
 /* ---- Training side of the modulated pre-training step (SURVEY.md §8 f2, BASELINE config 5): backward of the Gated Class-scalable

@@ -69,13 +69,13 @@ SIGNATURES = {
     "mqdet_contrastive_mask": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "mqdet_argsort_desc": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "mqdet_ml_nms_workspace_bytes": (c_int64, [c_int64]),
-    "mqdet_global_max_workspace_floats": (c_int64, []),
-    "mqdet_global_max_f32": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "mqdet_global_max_workspace_floats": (c_int64, [c_int64]),
+    "mqdet_global_max_f32": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "mqdet_sum_splits_cast": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
     "mqdet_softmax_rows_shifted_supported": (c_int, [c_int64, c_int64]),
-    "mqdet_softmax_rows_shifted": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_float, c_float,
-                                           c_void_p, c_int64, c_float, c_float, c_void_p]),
-    "mqdet_shift_clamp_f32": (c_int, [c_void_p, c_int64, c_void_p, c_float, c_float, c_void_p]),
+    "mqdet_softmax_rows_shifted": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int64, c_float,
+                                           c_float, c_void_p, c_int64, c_float, c_float, c_void_p]),
+    "mqdet_shift_clamp_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_float, c_float, c_void_p]),
     "mqdet_row_max_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_topk_desc": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_gather_rows_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p, c_void_p]),
@@ -130,8 +130,8 @@ SIGNATURES = {
     "mqdet_box_refine_sine": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
     "mqdet_gdino_detections_workspace_floats": (c_int64, [c_int64, c_int64]),
-    "mqdet_gdino_detections": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_float, c_int64, c_int64,
-                                       c_int64, c_void_p, c_void_p, c_void_p]),
+    "mqdet_gdino_detections": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p,
+                                       c_float, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "mqdet_transpose_cast": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_float, c_void_p, c_int64, c_void_p]),
     "mqdet_layernorm_bwd_workspace_floats": (c_int64, [c_int64, c_int64]),
     "mqdet_layernorm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int64, c_int64, c_void_p, c_int, c_void_p, c_void_p,

@@ -1,6 +1,7 @@
 // mqdet_b200 — small device ops of the GroundingDINO variant (SURVEY.md §8 f1) next to ms_deform_attn (msda.cu):
 //   * STABLE_SOFTMAX_2D of BiMultiHeadAttention (groundingdino_new/models/GroundingDINO/fuse_modules.py:177-187): the GLOBAL
-//     maximum of the score tensor is subtracted before the +-5e4 clamps                 -> global_max + shift_clamp
+//     maximum of the score tensor (of each batch element's, when prompt chunks share a batch) is subtracted before the +-5e4
+//     clamps                                                                            -> global_max + shift_clamp
 //   * two-stage query selection (transformer.py:288-318): max over the text tokens of the encoder class logits, top-900
 //     proposals per image, gathers of the selected rows                                -> row_max, topk_desc, gather_rows
 // All HBM-bound single-pass kernels; no host synchronisation.
@@ -20,44 +21,57 @@ __device__ __forceinline__ float block_max_256(float m, float* sh) {
   return r;  // valid in warp 0
 }
 
-__global__ void __launch_bounds__(256) global_max_partial_kernel(const float* __restrict__ x, long n, float* __restrict__ partial) {
+// Segment s = x[s * seg_len, (s + 1) * seg_len): blockIdx.y = segment, gridDim.x blocks per segment -> partial[s][blockIdx.x].
+// float4 loads where the segment starts 16-byte aligned (always for one segment, or seg_len % 4 == 0), scalar loads otherwise.
+__global__ void __launch_bounds__(256) global_max_partial_kernel(const float* __restrict__ x, long seg_len, float* __restrict__ partial) {
   __shared__ float sh[8];
   float m = -INFINITY;
-  const long n4 = n >> 2;
-  const float4* x4 = reinterpret_cast<const float4*>(x);
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long)gridDim.x * 256) {
-    const float4 v = __ldg(x4 + i);
-    m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
+  const long s = blockIdx.y;
+  const float* xs = x + s * seg_len;
+  const long stride = (long)gridDim.x * 256;
+  if (((s * seg_len) & 3) == 0) {
+    const long n4 = seg_len >> 2;
+    const float4* x4 = reinterpret_cast<const float4*>(xs);
+    for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n4; i += stride) {
+      const float4 v = __ldg(x4 + i);
+      m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
+    }
+    if (blockIdx.x == 0)
+      for (long i = (n4 << 2) + threadIdx.x; i < seg_len; i += 256) m = fmaxf(m, xs[i]);
+  } else {
+    for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < seg_len; i += stride) m = fmaxf(m, __ldg(xs + i));
   }
-  if (blockIdx.x == 0)
-    for (long i = (n4 << 2) + threadIdx.x; i < n; i += 256) m = fmaxf(m, x[i]);
   m = block_max_256(m, sh);
-  if (threadIdx.x == 0) partial[blockIdx.x] = m;
+  if (threadIdx.x == 0) partial[s * gridDim.x + blockIdx.x] = m;
 }
 
+// out[s] = max of partial[s][0 .. np): one CTA per segment
 __global__ void __launch_bounds__(256) global_max_final_kernel(const float* __restrict__ partial, int np, float* __restrict__ out) {
   __shared__ float sh[8];
   float m = -INFINITY;
-  for (int i = threadIdx.x; i < np; i += 256) m = fmaxf(m, partial[i]);
+  const float* p = partial + (long)blockIdx.x * np;
+  for (int i = threadIdx.x; i < np; i += 256) m = fmaxf(m, p[i]);
   m = block_max_256(m, sh);
-  if (threadIdx.x == 0) out[0] = m;
+  if (threadIdx.x == 0) out[blockIdx.x] = m;
 }
 
-__global__ void __launch_bounds__(256) shift_clamp_kernel(float* __restrict__ x, long n, const float* __restrict__ shift, float lo,
-                                                          float hi) {
+// x[i] = clamp(x[i] - shift[i / per_shift], lo, hi); per_shift = 0: shift[0] everywhere
+__global__ void __launch_bounds__(256) shift_clamp_kernel(float* __restrict__ x, long n, const float* __restrict__ shift, long per_shift,
+                                                          float lo, float hi) {
   const float s = __ldg(shift);
+  auto sh = [&](long i) { return per_shift ? __ldg(shift + i / per_shift) : s; };
   const long n4 = n >> 2;
   float4* x4 = reinterpret_cast<float4*>(x);
   for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long)gridDim.x * 256) {
     float4 v = x4[i];
-    v.x = fminf(fmaxf(v.x - s, lo), hi);
-    v.y = fminf(fmaxf(v.y - s, lo), hi);
-    v.z = fminf(fmaxf(v.z - s, lo), hi);
-    v.w = fminf(fmaxf(v.w - s, lo), hi);
+    v.x = fminf(fmaxf(v.x - sh(4 * i), lo), hi);
+    v.y = fminf(fmaxf(v.y - sh(4 * i + 1), lo), hi);
+    v.z = fminf(fmaxf(v.z - sh(4 * i + 2), lo), hi);
+    v.w = fminf(fmaxf(v.w - sh(4 * i + 3), lo), hi);
     x4[i] = v;
   }
   if (blockIdx.x == 0)
-    for (long i = (n4 << 2) + threadIdx.x; i < n; i += 256) x[i] = fminf(fmaxf(x[i] - s, lo), hi);
+    for (long i = (n4 << 2) + threadIdx.x; i < n; i += 256) x[i] = fminf(fmaxf(x[i] - sh(i), lo), hi);
 }
 
 // out[r] = max_j x[r][j], warp per row
@@ -188,23 +202,37 @@ __global__ void __launch_bounds__(1024) topk_desc_kernel(const float* __restrict
 
 using namespace mqdet;
 
-extern "C" int mqdet_global_max_f32(const float* x, int64_t n, float* out, float* workspace, void* stream) {
+// blocks per segment: GMAX_BLOCKS shared by the segments (at least one each), no more than the segment has float4 groups of 256
+static long gmax_blocks_per_segment(long seg_len, long segments) {
+  long cap = GMAX_BLOCKS / segments;
+  if (cap < 1) cap = 1;
+  long need = (seg_len / 4 + 255) / 256;
+  if (need < 1) need = 1;
+  return need < cap ? need : cap;
+}
+
+extern "C" int mqdet_global_max_f32(const float* x, int64_t n, int64_t segments, float* out, float* workspace, void* stream) {
   MQ_REQUIRE(x && out && workspace && n > 0, "global_max: null pointer / empty");
+  MQ_REQUIRE(segments >= 1 && segments <= 65535 && (n % segments) == 0, "global_max: %ld elements do not split into %ld equal segments (1..65535)",
+             (long)n, (long)segments);
   MQ_REQUIRE(((uintptr_t)x & 15) == 0, "global_max: x must be 16-byte aligned");
-  const int blocks = (int)((n / 4 + 255) / 256 < GMAX_BLOCKS ? ((n / 4 + 255) / 256 > 0 ? (n / 4 + 255) / 256 : 1) : GMAX_BLOCKS);
-  global_max_partial_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, n, workspace);
-  global_max_final_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(workspace, blocks, out);
+  const long seg_len = n / segments;
+  const long blocks = gmax_blocks_per_segment(seg_len, segments);
+  global_max_partial_kernel<<<dim3((unsigned)blocks, (unsigned)segments), 256, 0, (cudaStream_t)stream>>>(x, seg_len, workspace);
+  global_max_final_kernel<<<(unsigned)segments, 256, 0, (cudaStream_t)stream>>>(workspace, (int)blocks, out);
   return check_launch("global_max");
 }
 
-extern "C" int64_t mqdet_global_max_workspace_floats(void) { return GMAX_BLOCKS; }
+extern "C" int64_t mqdet_global_max_workspace_floats(int64_t segments) {
+  return segments < 1 ? 0 : segments * (GMAX_BLOCKS / segments > 0 ? GMAX_BLOCKS / segments : 1);
+}
 
-extern "C" int mqdet_shift_clamp_f32(float* x, int64_t n, const float* shift, float lo, float hi, void* stream) {
-  MQ_REQUIRE(x && shift && n > 0, "shift_clamp: null pointer / empty");
+extern "C" int mqdet_shift_clamp_f32(float* x, int64_t n, const float* shift, int64_t elems_per_shift, float lo, float hi, void* stream) {
+  MQ_REQUIRE(x && shift && n > 0 && elems_per_shift >= 0, "shift_clamp: null pointer / empty");
   MQ_REQUIRE(((uintptr_t)x & 15) == 0, "shift_clamp: x must be 16-byte aligned");
   const long blocks = (n / 4 + 255) / 256;
-  shift_clamp_kernel<<<(unsigned)(blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks)), 256, 0, (cudaStream_t)stream>>>(x, n, shift, lo,
-                                                                                                                        hi);
+  shift_clamp_kernel<<<(unsigned)(blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks)), 256, 0, (cudaStream_t)stream>>>(
+      x, n, shift, elems_per_shift, lo, hi);
   return check_launch("shift_clamp_kernel");
 }
 

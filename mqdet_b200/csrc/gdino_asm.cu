@@ -170,9 +170,10 @@ constexpr int GD_WARPS = 16;
 constexpr int GD_MAX_T = 256;
 
 __global__ void __launch_bounds__(GD_WARPS * 32) gdino_score_kernel(const float* __restrict__ logits, int T, const float* __restrict__ boxes,
-                                                                    const int* __restrict__ tokmap, int C, int max_tok,
-                                                                    const float* __restrict__ img_wh, float thr, int nq,
-                                                                    float* __restrict__ scratch) {
+                                                                    const int* __restrict__ tokmap, long tokmap_img_stride,
+                                                                    const int* __restrict__ class_labels, long labels_img_stride,
+                                                                    int C, int max_tok, const float* __restrict__ img_wh, float thr,
+                                                                    int nq, float* __restrict__ scratch) {
   __shared__ float prob[GD_WARPS][GD_MAX_T];
   const int b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q = blockIdx.x * GD_WARPS + warp;
@@ -185,7 +186,7 @@ __global__ void __launch_bounds__(GD_WARPS * 32) gdino_score_kernel(const float*
   float best = -1.f;
   int best_c = 0x7fffffff;
   for (int c = lane; c < C; c += 32) {
-    const int* tm = tokmap + (long)c * max_tok;
+    const int* tm = tokmap + b * tokmap_img_stride + (long)c * max_tok;
     float s = 0.f;
     int n = 0;
     for (int j = 0; j < max_tok; ++j) {
@@ -213,7 +214,9 @@ __global__ void __launch_bounds__(GD_WARPS * 32) gdino_score_kernel(const float*
     x2 = fminf(fmaxf(x2, 0.f), W - 1.f);
     y2 = fminf(fmaxf(y2, 0.f), H - 1.f);
     float* r = scratch + ((long)b * nq + q) * 7;
-    r[0] = x1; r[1] = y1; r[2] = x2; r[3] = y2; r[4] = best; r[5] = (float)(best_c + 1);
+    // columns of a per-element table are its classes in ascending label order, so the lowest column is also the lowest label
+    const int label = class_labels ? class_labels[b * labels_img_stride + best_c] : best_c + 1;
+    r[0] = x1; r[1] = y1; r[2] = x2; r[3] = y2; r[4] = best; r[5] = (float)label;
     // candidate_inds = max > box_threshold; remove_small_boxes(min_size=0): w = x2 - x1 + 1 >= 0 (boxlist_ops.py:78-92)
     r[6] = ((best > thr) && (x2 - x1 + 1.f >= 0.f) && (y2 - y1 + 1.f >= 0.f)) ? 1.f : 0.f;
   }
@@ -294,15 +297,20 @@ extern "C" int mqdet_box_refine_sine(const float* delta, int64_t ldd, const floa
 
 extern "C" int64_t mqdet_gdino_detections_workspace_floats(int64_t B, int64_t nq) { return B * nq * 7; }
 
-extern "C" int mqdet_gdino_detections(const float* logits, int64_t T, const float* boxes, const int32_t* tokmap, int64_t C,
+extern "C" int mqdet_gdino_detections(const float* logits, int64_t T, const float* boxes, const int32_t* tokmap,
+                                      int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride, int64_t C,
                                       int64_t max_tok, const float* img_wh, float box_threshold, int64_t B, int64_t nq,
                                       int64_t max_out, float* out, float* workspace, void* stream) {
   MQ_REQUIRE(logits && boxes && tokmap && img_wh && out && workspace, "gdino_detections: null pointer");
   MQ_REQUIRE(B > 0 && B <= 65535 && nq > 0 && T > 0 && T <= GD_MAX_T && C > 0 && max_tok > 0 && max_out > 0,
              "gdino_detections: bad shape (T <= 256)");
+  MQ_REQUIRE(tokmap_img_stride >= 0 && labels_img_stride >= 0 && (tokmap_img_stride == 0 || tokmap_img_stride >= C * max_tok) &&
+             (labels_img_stride == 0 || labels_img_stride >= C) && (class_labels || labels_img_stride == 0),
+             "gdino_detections: bad per-element table strides");
   cudaStream_t st = (cudaStream_t)stream;
   gdino_score_kernel<<<dim3((unsigned)((nq + GD_WARPS - 1) / GD_WARPS), (unsigned)B), GD_WARPS * 32, 0, st>>>(
-      logits, (int)T, boxes, tokmap, (int)C, (int)max_tok, img_wh, box_threshold, (int)nq, workspace);
+      logits, (int)T, boxes, tokmap, (long)tokmap_img_stride, class_labels, (long)labels_img_stride, (int)C, (int)max_tok, img_wh,
+      box_threshold, (int)nq, workspace);
   gdino_compact_kernel<<<(unsigned)B, 256, 0, st>>>(workspace, (int)nq, (int)max_out, out);
   return check_launch("gdino_detections");
 }

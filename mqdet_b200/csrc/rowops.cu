@@ -269,14 +269,15 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   }
 }
 
-// fp32 scores (the BERT self-attention products, [B*12*256, 256]): same single-read scheme with two float4 per lane.
-template <int RW>
+// fp32 scores (the BERT self-attention products, [B*12*256, 256]): same single-read scheme with two float4 per lane.  SHIFTED:
+// the stable-softmax shift + clamps (a template flag so that the per-row shift index costs the plain softmax no registers).
+template <int RW, bool SHIFTED = false>
 __global__ void __launch_bounds__(256) softmax_rows256_f32_kernel(const float* __restrict__ x, long ldx, __half* __restrict__ y,
                                                                   long ldy, long rows, float scale,
                                                                   const float* __restrict__ colmask, long rows_per_batch,
                                                                   float mask_value, float keep_add,
-                                                                  const float* __restrict__ shift = nullptr, float lo = -INFINITY,
-                                                                  float hi = INFINITY) {
+                                                                  const float* __restrict__ shift = nullptr, long rows_per_shift = 0,
+                                                                  float lo = -INFINITY, float hi = INFINITY) {
   const int lane = threadIdx.x & 31;
   const long r0 = ((long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * RW;
   if (r0 >= rows) return;
@@ -298,8 +299,9 @@ __global__ void __launch_bounds__(256) softmax_rows256_f32_kernel(const float* _
     if (row >= rows) break;
     float v[8] = {u[j][0].x * scale, u[j][0].y * scale, u[j][0].z * scale, u[j][0].w * scale,
                   u[j][1].x * scale, u[j][1].y * scale, u[j][1].z * scale, u[j][1].w * scale};
-    if (shift) {  // STABLE_SOFTMAX_2D: v = clamp(v - global max, lo, hi) fused here instead of a pass of its own over the scores
-      const float sh = __ldg(shift);
+    if (SHIFTED) {  // STABLE_SOFTMAX_2D: v = clamp(v - global max, lo, hi) fused here instead of a pass of its own over the scores
+      // one maximum per batch element, or one for all (rows < 2^31: checked by the entry point)
+      const float sh = __ldg(shift + (rows_per_shift ? (unsigned)row / (unsigned)rows_per_shift : 0u));
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = fminf(fmaxf(v[i] - sh, lo), hi);
     }
@@ -336,8 +338,8 @@ __global__ void __launch_bounds__(256) softmax_rows256_f32_kernel(const float* _
 __global__ void __launch_bounds__(256) softmax_longrows_f32_kernel(const float* __restrict__ x, long ldx, __half* __restrict__ y, long ldy,
                                                                    int n, int n_pad, float scale, const float* __restrict__ colmask,
                                                                    long rows_per_batch, float mask_value, float keep_add,
-                                                                   const float* __restrict__ shift = nullptr, float lo = -INFINITY,
-                                                                   float hi = INFINITY) {
+                                                                   const float* __restrict__ shift = nullptr, long rows_per_shift = 0,
+                                                                   float lo = -INFINITY, float hi = INFINITY) {
   __shared__ float red[8];
   __shared__ float bcast;
   const long row = blockIdx.x;
@@ -345,7 +347,7 @@ __global__ void __launch_bounds__(256) softmax_longrows_f32_kernel(const float* 
   __half* yr = y + row * ldy;
   const float* cm = colmask ? colmask + (row / rows_per_batch) * n : nullptr;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const float sh = shift ? __ldg(shift) : 0.f;
+  const float sh = shift ? __ldg(shift + (rows_per_shift ? row / rows_per_shift : 0)) : 0.f;
   auto val = [&](int i) {
     float v = xr[i] * scale;
     if (shift) v = fminf(fmaxf(v - sh, lo), hi);
@@ -568,23 +570,24 @@ extern "C" int mqdet_softmax_rows(const void* x, int in_dtype, int64_t ldx, void
 extern "C" int mqdet_softmax_rows_shifted_supported(int64_t n, int64_t n_pad) { return (n == 256 && n_pad == 256) || n >= 4096; }
 
 extern "C" int mqdet_softmax_rows_shifted(const float* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int64_t n, int64_t n_pad,
-                                          const float* shift_dev, float lo, float hi, const float* colmask, int64_t rows_per_batch,
-                                          float mask_value, float keep_add, void* stream) {
-  MQ_REQUIRE(x && y && shift_dev && rows > 0 && n > 0 && n_pad >= n, "softmax_rows_shifted: bad args");
+                                          const float* shift_dev, int64_t rows_per_shift, float lo, float hi, const float* colmask,
+                                          int64_t rows_per_batch, float mask_value, float keep_add, void* stream) {
+  MQ_REQUIRE(x && y && shift_dev && rows > 0 && n > 0 && n_pad >= n && rows_per_shift >= 0, "softmax_rows_shifted: bad args");
   MQ_REQUIRE(mqdet_softmax_rows_shifted_supported(n, n_pad), "softmax_rows_shifted: n == n_pad == 256 or n >= 4096 only");
   if (rows_per_batch <= 0) rows_per_batch = rows;
   cudaStream_t st = (cudaStream_t)stream;
+  MQ_REQUIRE(rows <= 0x7fffffffL && rows_per_shift <= 0x7fffffffL, "softmax_rows_shifted: too many rows");
   if (n == 256) {
     MQ_REQUIRE((ldx % 4) == 0 && (ldy % 8) == 0 && ((uintptr_t)x % 16) == 0 && ((uintptr_t)y % 16) == 0 &&
                    (!colmask || ((uintptr_t)colmask % 16) == 0), "softmax_rows_shifted: 16-byte aligned rows required for n = 256");
     constexpr int RW = 2;
-    softmax_rows256_f32_kernel<RW><<<(unsigned)cdiv(rows, 8L * RW), 256, 0, st>>>(x, ldx, (__half*)y, ldy, rows, 1.f, colmask,
-                                                                                  rows_per_batch, mask_value, keep_add, shift_dev, lo, hi);
+    softmax_rows256_f32_kernel<RW, true><<<(unsigned)cdiv(rows, 8L * RW), 256, 0, st>>>(x, ldx, (__half*)y, ldy, rows, 1.f, colmask,
+                                                                                  rows_per_batch, mask_value, keep_add, shift_dev, rows_per_shift,
+                                                                                  lo, hi);
     return check_launch("softmax_rows256_f32_kernel");
   }
-  MQ_REQUIRE(rows <= 0x7fffffffL, "softmax_rows_shifted: too many rows");
   softmax_longrows_f32_kernel<<<(unsigned)rows, 256, 0, st>>>(x, ldx, (__half*)y, ldy, (int)n, (int)n_pad, 1.f, colmask, rows_per_batch,
-                                                              mask_value, keep_add, shift_dev, lo, hi);
+                                                              mask_value, keep_add, shift_dev, rows_per_shift, lo, hi);
   return check_launch("softmax_longrows_f32_kernel");
 }
 

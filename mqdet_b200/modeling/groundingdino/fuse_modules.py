@@ -5,7 +5,9 @@ encoder, transformer.py:171-180).
 Same parameters (``state_dict`` keys) and arithmetic as the reference; it differs from the GLIP block (utils/fuse_helper.py) in
 three places, all handled by the shared implementation:
   * ``stable_softmax_2d = True``: the GLOBAL maximum of the score tensor is subtracted before the +-5e4 clamps (:177-187) —
-    ``mqdet_global_max_f32`` + ``mqdet_shift_clamp_f32`` on the fp32 scores, the maximum never leaves the device;
+    ``mqdet_global_max_f32`` + ``mqdet_shift_clamp_f32`` on the fp32 scores, the maximum never leaves the device; batched prompt
+    chunks (``GroundingDINO.forward_chunked_device``) take one maximum per batch element, since the reference sees one chunk per
+    forward;
   * masks are boolean with True = padding and are filled with -inf (:201-214), for the text tokens AND for the image tokens;
   * the block takes / returns flat ``[B, N, C]`` tensors (no FPN-level lists).
 The scores are materialised in fp32 here (the global maximum is needed before either softmax), i.e. this is the explicit path,
@@ -52,9 +54,10 @@ class BiAttentionBlock(nn.Module):
         self.gamma_l = nn.Parameter(init_values * torch.ones((l_dim)), requires_grad=True)
 
     @torch.no_grad()
-    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None, keep_v=None, keep_l=None):
+    def forward(self, v, l, attention_mask_v=None, attention_mask_l=None, keep_v=None, keep_l=None, per_element_max=False):
         """v [B,N,v_dim], l [B,T,l_dim] fp32 -> (v', l') fp32:  x' = LN(x) + gamma * delta  (residual on the NORMALISED inputs,
-        :286-296).  ``keep_v`` / ``keep_l``: the masks already as fp32 1 keep / 0 padding (the assembly builds them once)."""
+        :286-296).  ``keep_v`` / ``keep_l``: the masks already as fp32 1 keep / 0 padding (the assembly builds them once).
+        ``per_element_max``: the stable-softmax maximum of each batch element alone (batched prompt chunks)."""
         if not v.is_cuda:
             raise MqdetError("BiAttentionBlock: CUDA tensors required (no CPU fallback)")
         nv, nl = self.layer_norm_v, self.layer_norm_l
@@ -63,7 +66,7 @@ class BiAttentionBlock(nn.Module):
         a = self.attn
         keep_l = a._keep(attention_mask_l) if keep_l is None else keep_l
         keep_v = a._keep(attention_mask_v) if keep_v is None else keep_v
-        dv, dl = a._attend(vn16, ln16, keep_l, mask_v=keep_v,
+        dv, dl = a._attend(vn16, ln16, keep_l, mask_v=keep_v, per_element_max=per_element_max,
                            v_epilogue=dict(gate=f32(self.gamma_v), residual=vn32, out_dtype=torch.float32),
                            l_epilogue=dict(gate=f32(self.gamma_l), residual=ln32))
         return dv, dl

@@ -13,7 +13,8 @@ Same module / parameter names as the reference (``backbone.0.*``, ``input_proj.N
 checkpoints load unchanged.  Differences from the reference's inference path, all outside the arithmetic: string captions need an
 attached tokenizer (pre-tokenised ``{"input_ids", "attention_mask"}`` are accepted, no vocabulary offline); batches larger than 1 are
 supported when the images share one prompt (the reference asserts B == 1, groundingdino.py:543); everything that depends only on
-the prompt or on the padding geometry is cached (``_prompt_state`` / ``_geometry``).
+the prompt or on the padding geometry is cached (``_prompt_state`` / ``_geometry``).  Many-category vocabularies (LVIS) run
+through ``forward_chunked``: the backbone once per image batch, the prompt chunks as batch elements.
 """
 import math
 
@@ -227,21 +228,29 @@ class GroundingDINO(nn.Module):
         self._geo = None
         return self._prompt
 
-    @torch.no_grad()
-    def _geometry(self, image_sizes, padded_hw, level_hw, B, dev, st):
-        """Padding masks per level (backbone.py:103-111, groundingdino.py:513-516), position embeddings, encoder reference points,
-        valid ratios, anchor proposals, text position embeddings: functions of the image sizes and the prompt only."""
+    def _image_key(self, image_sizes, padded_hw, level_hw):
         le = self.transformer.level_embed   # folded into the cached level position embeddings: a reloaded checkpoint invalidates them
-        key = (tuple(tuple(int(v) for v in s) for s in image_sizes), tuple(padded_hw), tuple(level_hw), st["key"], le.data_ptr(), le._version)
-        if self._geo is not None and self._geo["key"] == key:
-            return self._geo
+        return (tuple(tuple(int(v) for v in s) for s in image_sizes), tuple(padded_hw), tuple(level_hw), le.data_ptr(), le._version)
+
+    @torch.no_grad()
+    def _level_masks(self, image_sizes, padded_hw, level_hw, B, dev):
+        """Padding masks per level (backbone.py:103-111, groundingdino.py:513-516) and their position embeddings."""
         Hp, Wp = padded_hw
         m = torch.zeros((B, Hp, Wp), dtype=torch.float32, device=dev)
         for b, (h, w) in enumerate(image_sizes):
             m[b, int(h):, :] = 1
             m[b, :, int(w):] = 1
         masks = [torch.nn.functional.interpolate(m[None], size=hw).to(torch.bool)[0] for hw in level_hw]
-        poss = [self.backbone[1](mk) for mk in masks]
+        return masks, [self.backbone[1](mk) for mk in masks]
+
+    @torch.no_grad()
+    def _geometry(self, image_sizes, padded_hw, level_hw, B, dev, st):
+        """Padding masks per level, position embeddings, encoder reference points, valid ratios, anchor proposals, text position
+        embeddings: functions of the image sizes and the prompt only."""
+        key = self._image_key(image_sizes, padded_hw, level_hw) + (st["key"],)
+        if self._geo is not None and self._geo["key"] == key:
+            return self._geo
+        masks, poss = self._level_masks(image_sizes, padded_hw, level_hw, B, dev)
         geo = self.transformer.prepare(masks, poss, st["token_mask"], st["position_ids"], st["self_mask"])
         geo["key"] = key
         geo["levels"] = ops.get_levels(list(level_hw), dev)
@@ -299,18 +308,179 @@ class GroundingDINO(nn.Module):
         tr = self.transformer.forward_flat(src32, geo, enc_text, all_layers=all_layers, proposals=proposals)
         hs, refs = tr["hs"], tr["references"]
         nq = hs[-1].shape[1]
-        # deformable-detr-like anchor update of the LAST layer on the normed hidden state (groundingdino.py:618-627)
-        hs16 = ops.cast_f16(hs[-1])
-        delta = self.bbox_embed[-1](hs16.view(B * nq, -1), out_dtype=torch.float32)
-        boxes, _, _ = ops.box_refine_sine(refs[-2], geo["valid_ratios"], delta=delta.view(B, nq, -1), want_sine=False)
-        text_dict = {"encoded_text": tr["memory_text"], "encoded_text16": tr["memory_text16"], "text_token_mask": st["token_mask"]}
-        logits = self.class_embed[-1](hs16, text_dict)
+        logits, boxes = self._last_layer_heads(tr, geo["valid_ratios"], st["token_mask"])
         packed = ops.gdino_detections(logits, boxes, st["tokmap"], geo["img_wh"], self.box_threshold)
         return {"det_packed": packed, "det": packed[:, :nq], "num": packed[:, nq, 0], "pred_logits": logits, "pred_boxes": boxes,
                 "image_sizes": images.image_sizes, "hs": hs, "references": refs, "srcs": src32, "level_sizes": sizes,
                 "encoded_text": enc_text, "bert_hidden": h, "transformer": tr,
                 "vision_query_gates": bert["vision_query_gates"], "valid_ratios": geo["valid_ratios"],
                 "text_token_mask": st["token_mask"]}
+
+    def _last_layer_heads(self, tr, valid_ratios, token_mask):
+        """Class logits [B, nq, 256] and boxes [B, nq, 4] of the last decoder layer: deformable-detr-like anchor update on the
+        normed hidden state (groundingdino.py:618-627) and the contrastive class head."""
+        h = tr["hs"][-1]
+        B, nq = h.shape[:2]
+        hs16 = ops.cast_f16(h)
+        delta = self.bbox_embed[-1](hs16.view(B * nq, -1), out_dtype=torch.float32)
+        boxes, _, _ = ops.box_refine_sine(tr["references"][-2], valid_ratios, delta=delta.view(B, nq, -1), want_sine=False)
+        text_dict = {"encoded_text": tr["memory_text"], "encoded_text16": tr["memory_text16"], "text_token_mask": token_mask}
+        return self.class_embed[-1](hs16, text_dict), boxes
+
+    # ---- many-category prompts: chunked evaluation (LVIS) --------------------------------------------------------------
+    CHUNK_STATE_CAPACITY = 4096    # distinct chunk prompts kept (LVIS: 31)
+    CHUNK_GROUP_CAPACITY = 16      # passes of one image geometry kept (LVIS at 8 chunks per pass: 4)
+
+    @torch.no_grad()
+    def _chunk_state(self, captions, positive_map, dev):
+        """Per-chunk prompt state, cached by content like ``_prompt_state``: token ids, attention mask, per-category self-attention
+        mask and restarted position ids (bertwarper.py:271-320), selected vision queries + their token mask, and the chunk's
+        classes in ascending label order with their token lists (its score columns)."""
+        from ..detector.generalized_vl_rcnn_new import GeneralizedVLRCNN_New
+        bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
+        key = GeneralizedVLRCNN_New._prompt_key(captions, positive_map, 1, bank_version)
+        cache = self.__dict__.setdefault("_chunk_cache", {})
+        st = cache.get(key)
+        if st is not None:
+            return st
+        ids, am = self._tokenize(captions)
+        ids, am = ids[:1, : self.max_text_len].cpu(), am[:1, : self.max_text_len].cpu()
+        sam, pid, _ = generate_masks_with_special_tokens_and_transfer_map({"input_ids": ids}, self.specical_tokens, self.tokenizer)
+        vision = vmask = None
+        if self.cfg.VISION_QUERY.ENABLED and self.query_selector is not None and self.query_selector.query_bank is not None:
+            labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
+            vision, vmask, _ = self.query_selector([labels], [all_map], None)
+            vision, vmask = vision[0].float().to(dev).contiguous(), vmask[0].float().to(dev).contiguous()
+        cols = sorted(int(k) for k in positive_map)
+        toks = [([positive_map[c]] if isinstance(positive_map[c], int) else list(positive_map[c])) for c in cols]
+        if len(cache) >= self.CHUNK_STATE_CAPACITY:
+            cache.clear()
+        st = cache[key] = dict(key=key, ids=ids.to(dev), token_mask=am.bool().to(dev), self_mask=sam.to(dev), position_ids=pid.to(dev),
+                               vision=vision, vmask=vmask, cols=cols, toks=toks)
+        return st
+
+    @torch.no_grad()
+    def _chunk_pass_state(self, image_sizes, padded_hw, level_hw, B, dev, sts):
+        """Everything one pass of ``forward_chunked_device`` needs besides the image features, for elements e = chunk * B + image:
+        the image half of the geometry (computed once per image geometry, repeated per chunk), the text half and the BERT inputs
+        of the chunks, the vision queries zero-padded to the pass's largest count (the pad_sequence padding of
+        QuerySelector.forward, query_selector.py:112-116), and the per-element class tables.  Cached per (image geometry, chunk
+        group); the cache holds the passes of the current image geometry only."""
+        ikey = self._image_key(image_sizes, padded_hw, level_hw)
+        cache = self.__dict__.get("_chunk_pass_cache")
+        if cache is None or cache["ikey"] != ikey:
+            masks, poss = self._level_masks(image_sizes, padded_hw, level_hw, B, dev)
+            img_geo = self.transformer.prepare_image(masks, poss)
+            img_geo["levels"] = ops.get_levels(list(level_hw), dev)
+            img_geo["img_wh"] = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32, device=dev)
+            cache = self._chunk_pass_cache = dict(ikey=ikey, img_geo=img_geo, passes={})
+        gkey = tuple(st["key"] for st in sts)
+        ps = cache["passes"].get(gkey)
+        if ps is not None:
+            return ps
+        G = len(sts)
+
+        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...], element e = chunk * B + image
+            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
+
+        img_geo = cache["img_geo"]
+        ps = Transformer.repeat_image_geometry(img_geo, G)
+        ps["levels"] = img_geo["levels"]
+        ps["img_wh"] = img_geo["img_wh"].repeat(G, 1).contiguous()
+        token_mask = per_element([st["token_mask"] for st in sts])
+        self_mask, position_ids = per_element([st["self_mask"] for st in sts]), per_element([st["position_ids"] for st in sts])
+        ps.update(self.transformer.prepare_text(token_mask, position_ids, self_mask))
+        ps["per_element_max"] = True   # each chunk's fusion scores are shifted by their own maximum (one chunk per reference forward)
+        ps["ids"], ps["bert_mask"], ps["position_ids"] = per_element([st["ids"] for st in sts]), self_mask.float().contiguous(), position_ids
+        ps["vision"] = ps["vmask"] = None
+        if sts[0]["vision"] is not None:
+            Vmax = max(st["vision"].shape[0] for st in sts)
+            vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
+            vmask = torch.zeros((G, Vmax, sts[0]["vmask"].shape[1]), dtype=torch.float32, device=dev)
+            for g, st in enumerate(sts):
+                vision[g, :st["vision"].shape[0]] = st["vision"]
+                vmask[g, :st["vmask"].shape[0]] = st["vmask"]
+            ps["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
+            ps["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
+        Cmax = max(max(len(st["cols"]) for st in sts), 1)
+        mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
+        tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
+        lab_h = torch.zeros((G, Cmax), dtype=torch.int32)
+        for g, st in enumerate(sts):
+            for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
+                tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
+                lab_h[g, j] = c
+        ps["tokmap"] = tok_h.to(dev).repeat_interleave(B, dim=0).contiguous()
+        ps["class_labels"] = lab_h.to(dev).repeat_interleave(B, dim=0).contiguous()
+        if len(cache["passes"]) >= self.CHUNK_GROUP_CAPACITY:
+            cache["passes"].clear()
+        cache["passes"][gkey] = ps
+        return ps
+
+    @torch.no_grad()
+    def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
+        """Chunked evaluation of a many-category vocabulary (LVIS: 1203 classes as 31 prompts of 40 classes,
+        maskrcnn_benchmark/engine/inference.py:600-660 with TEST.CHUNKED_EVALUATION).  The reference runs the WHOLE model once per
+        chunk and image; here Swin-T + ``input_proj`` run ONCE per image batch and the chunks travel as extra batch elements
+        (element e = chunk * B + image) through the vision-conditioned BERT, ``feat_map``, the transformer and the heads,
+        ``chunks_per_pass`` chunks at a time.  The stable-softmax maximum of the fusion layers is taken per element, so a chunk's
+        detections do not depend on which chunks share its pass.  Score columns of a chunk are its classes in ascending label
+        order; the emitted labels are the global class ids (ties to the lowest label, as the reference's ``topk(1)`` over the
+        zero-filled full-vocabulary scores).  ``chunk_ids``: the subset of chunks THIS rank evaluates, default all.
+        Returns {"det_packed": [n_chunks_local, B, num_queries + 1, 6] device tensor, "chunks": [chunk index ...], ...}."""
+        if self.training:
+            raise NotImplementedError("training is SURVEY.md §8(f2)")
+        if int(chunks_per_pass) < 1:
+            raise ValueError(f"chunks_per_pass must be >= 1, got {chunks_per_pass}")
+        chunks_per_pass = int(chunks_per_pass)
+        images = to_image_list(images, self.cfg.DATALOADER.SIZE_DIVISIBILITY)
+        x = images.tensors
+        if not x.is_cuda:
+            raise MqdetError("GroundingDINO: CUDA images required (no CPU fallback)")
+        if len(chunk_captions) != len(chunk_positive_maps):
+            raise ValueError("one positive map per chunk caption required")
+        B, dev = x.shape[0], x.device
+        chunk_ids = list(range(len(chunk_captions))) if chunk_ids is None else [int(c) for c in chunk_ids]
+        src32, src16, sizes = self.visual_features(x)     # ONCE per image batch, shared by all chunks
+        nq = self.num_queries
+        packed = torch.empty((len(chunk_ids), B, nq + 1, 6), dtype=torch.float32, device=dev)
+        pooled = None
+        for p0 in range(0, len(chunk_ids), chunks_per_pass):
+            group = chunk_ids[p0:p0 + chunks_per_pass]
+            G = len(group)
+            sts = [self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in group]
+            ps = self._chunk_pass_state(images.image_sizes, tuple(x.shape[-2:]), tuple(sizes), B, dev, sts)
+            if ps["vision"] is not None and pooled is None:
+                pooled = ops.avgpool2_levels(src16, ps["levels"])   # flatten_fpn_features (:432-434)
+            bert = self.bert(input_ids=ps["ids"], attention_mask=ps["bert_mask"], position_ids=ps["position_ids"], vision=ps["vision"],
+                             images=pooled.repeat(G, 1, 1) if ps["vision"] is not None else None,
+                             vision_attention_mask=ps["vmask"], batched_pos_category_map=None)
+            h = bert["last_hidden_state"]
+            E, T = h.shape[:2]
+            enc_text = ops.gemm(ops.cast_f16(h).view(E * T, -1), w16(self.feat_map.weight), bias=f32(self.feat_map.bias),
+                                out_dtype=torch.float32).view(E, T, self.hidden_dim)
+            tr = self.transformer.forward_flat(src32.repeat(G, 1, 1) if G > 1 else src32, ps, enc_text)
+            logits, boxes = self._last_layer_heads(tr, ps["valid_ratios"], ps["text_token_mask"])
+            det = ops.gdino_detections(logits, boxes, ps["tokmap"], ps["img_wh"], self.box_threshold, class_labels=ps["class_labels"])
+            packed[p0:p0 + G] = det.view(G, B, nq + 1, 6)
+        return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "srcs": src32}
+
+    def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
+        """-> list[BoxList] (mode xyxy, fields labels / scores): per image, the per-chunk detections concatenated in chunk order
+        with their global labels (``BoxList.concate_box_list``, engine/inference.py:704-706)."""
+        from ...structures.bounding_box import BoxList
+        out = self.forward_chunked_device(images, chunk_captions, chunk_positive_maps, chunks_per_pass, chunk_ids)
+        pk = out["det_packed"].cpu()
+        nq = pk.shape[2] - 1
+        res = []
+        for b, (h, w) in enumerate(out["image_sizes"]):
+            parts = [pk[g, b, :int(pk[g, b, nq, 0])] for g in range(pk.shape[0])]
+            d = torch.cat(parts) if parts else torch.zeros((0, 6))
+            bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
+            bl.add_field("labels", d[:, 5].long())
+            bl.add_field("scores", d[:, 4].clone())
+            res.append(bl)
+        return res
 
     @torch.no_grad()
     def decoder_outputs_flat(self, out):

@@ -212,7 +212,8 @@ class TransformerEncoder(nn.Module):
         t32, t16 = text32, None
         for i, layer in enumerate(self.layers):
             if len(self.fusion_layers):
-                out32, t32 = self.fusion_layers[i](out32, t32, keep_v=geo["keep_mem2d"], keep_l=geo["text_keep"])
+                out32, t32 = self.fusion_layers[i](out32, t32, keep_v=geo["keep_mem2d"], keep_l=geo["text_keep"],
+                                                   per_element_max=geo.get("per_element_max", False))
                 out16 = t16 = None
             if len(self.text_layers):
                 t16 = ops.cast_f16(t32) if t16 is None else t16
@@ -320,6 +321,14 @@ class Transformer(nn.Module):
         utils.py:59-107): cached by the caller per input geometry.  masks: list of bool [B,h,w] (True = padding); pos_embeds: list
         of [B,C,h,w]; text_token_mask bool [B,T] (True = token in use); position_ids int64 [B,T]; text_self_attention_masks bool
         [B,T,T] (True = may attend)."""
+        return {**self.prepare_image(masks, pos_embeds), **self.prepare_text(text_token_mask, position_ids, text_self_attention_masks)}
+
+    IMAGE_GEOMETRY_KEYS = ("mask_flat", "pos", "valid_ratios", "ref_enc", "keep_mem2d", "output_proposals")
+
+    @torch.no_grad()
+    def prepare_image(self, masks, pos_embeds):
+        """The image half of ``prepare``: level masks, level position embeddings, valid ratios, encoder reference points, anchor
+        proposals.  Batched tensors are under ``IMAGE_GEOMETRY_KEYS`` (plus the flat views ``keep_mem`` / ``proposal_keep``)."""
         dev = masks[0].device
         shapes = [tuple(int(x) for x in m.shape[-2:]) for m in masks]
         mask_flat = torch.cat([m.flatten(1) for m in masks], 1)
@@ -327,14 +336,29 @@ class Transformer(nn.Module):
                          for l, p in enumerate(pos_embeds)], 1).contiguous()
         valid_ratios = torch.stack([self.get_valid_ratio(m) for m in masks], 1).float().contiguous()
         ref_enc = TransformerEncoder.get_reference_points(shapes, valid_ratios, dev).contiguous()
-        pos_text = get_sine_pos_embed(position_ids[..., None].float(), num_pos_feats=256, exchange_xy=False).contiguous()
         valid, proposals = gen_encoder_output_proposals(mask_flat, shapes)
         keep = (~mask_flat).float().contiguous()
         return {"spatial_shapes": shapes, "mask_flat": mask_flat, "pos": pos, "valid_ratios": valid_ratios, "ref_enc": ref_enc,
-                "pos_text": pos_text, "text_keep": text_token_mask.float().contiguous(), "text_token_mask": text_token_mask,
-                "text_self_mask": text_self_attention_masks.float().contiguous(), "keep_mem": keep.reshape(-1),
-                "keep_mem2d": keep, "proposal_keep": (valid & ~mask_flat).float().reshape(-1).contiguous(),
-                "output_proposals": proposals.contiguous()}
+                "keep_mem": keep.reshape(-1), "keep_mem2d": keep,
+                "proposal_keep": (valid & ~mask_flat).float().reshape(-1).contiguous(), "output_proposals": proposals.contiguous()}
+
+    @staticmethod
+    def repeat_image_geometry(img_geo, times):
+        """``prepare_image`` output for a batch that holds the same images ``times`` times over (element e = k * B + image)."""
+        out = dict(img_geo)
+        for k in Transformer.IMAGE_GEOMETRY_KEYS:
+            t = img_geo[k]
+            out[k] = t.repeat(times, *([1] * (t.dim() - 1))).contiguous()
+        out["keep_mem"] = out["keep_mem2d"].reshape(-1)
+        out["proposal_keep"] = img_geo["proposal_keep"].repeat(times).contiguous()
+        return out
+
+    @torch.no_grad()
+    def prepare_text(self, text_token_mask, position_ids, text_self_attention_masks):
+        """The prompt half of ``prepare``: text position embeddings, token and self-attention masks."""
+        pos_text = get_sine_pos_embed(position_ids[..., None].float(), num_pos_feats=256, exchange_xy=False).contiguous()
+        return {"pos_text": pos_text, "text_keep": text_token_mask.float().contiguous(), "text_token_mask": text_token_mask,
+                "text_self_mask": text_self_attention_masks.float().contiguous()}
 
     @torch.no_grad()
     def forward_flat(self, src32, geo, text32, all_layers=False, proposals=None):

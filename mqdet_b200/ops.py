@@ -240,47 +240,67 @@ def sum_splits_cast(part32, out16):
     return out16
 
 
-def softmax_rows_shifted(x32, shift, lo, hi, *, n=None, colmask=None, rows_per_batch=0, mask_value=0.0, keep_add=0.0):
-    """softmax over the last dim of clamp(x - shift[0], lo, hi) (+ mask) for contiguous fp32 [..., n_pad] -> fp16; ``shift`` is a device
-    scalar.  Fused where the kernel supports the row length, else ``shift_clamp_`` (in place!) followed by ``softmax_rows``."""
+def softmax_rows_shifted(x32, shift, lo, hi, *, n=None, colmask=None, rows_per_batch=0, mask_value=0.0, keep_add=0.0,
+                         rows_per_shift=0):
+    """softmax over the last dim of clamp(x - shift[r // rows_per_shift], lo, hi) (+ mask) for contiguous fp32 [..., n_pad] -> fp16;
+    ``shift`` is on the device: one value per ``rows_per_shift`` rows (one per batch element), or ``rows_per_shift = 0`` = shift[0]
+    for every row.  Fused where the kernel supports the row length, else ``shift_clamp_`` (in place!) followed by ``softmax_rows``."""
     global launch_count
     _need_cuda(x32, shift, colmask)
     n_pad = x32.shape[-1]
     n = n_pad if n is None else n
     if x32.dtype != torch.float32 or not x32.is_contiguous():
         raise _lib.MqdetError("softmax_rows_shifted: contiguous fp32 tensor required")
-    if not load().mqdet_softmax_rows_shifted_supported(n, n_pad):
-        shift_clamp_(x32, shift, lo, hi)
-        return softmax_rows(x32, n=n, colmask=colmask, rows_per_batch=rows_per_batch, mask_value=mask_value, keep_add=keep_add)
     rows = x32.numel() // n_pad
+    _check_shift(shift, rows, rows_per_shift, "softmax_rows_shifted")
+    if not load().mqdet_softmax_rows_shifted_supported(n, n_pad):
+        shift_clamp_(x32, shift, lo, hi, rows_per_shift=rows_per_shift)
+        return softmax_rows(x32, n=n, colmask=colmask, rows_per_batch=rows_per_batch, mask_value=mask_value, keep_add=keep_add)
     out = torch.empty(x32.shape, dtype=torch.float16, device=x32.device)
-    check(load().mqdet_softmax_rows_shifted(_ptr(x32), n_pad, _ptr(out), n_pad, rows, n, n_pad, _ptr(shift), float(lo), float(hi),
-                                            _ptr(colmask), int(rows_per_batch), float(mask_value), float(keep_add), _stream()),
+    check(load().mqdet_softmax_rows_shifted(_ptr(x32), n_pad, _ptr(out), n_pad, rows, n, n_pad, _ptr(shift), int(rows_per_shift),
+                                            float(lo), float(hi), _ptr(colmask), int(rows_per_batch), float(mask_value),
+                                            float(keep_add), _stream()),
           "softmax_rows_shifted")
     launch_count += 1
     return out
 
 
-def global_max(x32):
-    """max over ALL elements of a contiguous fp32 tensor -> device scalar [1] (no host sync)."""
+def _check_shift(shift, rows, rows_per_shift, what):
+    """The shift vector must cover every row group: rows_per_shift divides rows and shift holds rows // rows_per_shift values."""
+    if rows_per_shift < 0 or (rows_per_shift and (rows % rows_per_shift or shift.numel() < rows // rows_per_shift)):
+        raise ValueError(f"{what}: rows_per_shift={rows_per_shift} does not split {rows} rows over {shift.numel()} shifts")
+    if shift.dtype != torch.float32 or not shift.is_contiguous():
+        raise _lib.MqdetError(f"{what}: contiguous fp32 shift required")
+
+
+def global_max(x32, *, segments=1):
+    """Maximum of each of ``segments`` equal contiguous segments of a contiguous fp32 tensor -> device fp32 [segments] (no host
+    sync); ``segments = 1`` is the maximum over all elements.  One pass over x, deterministic."""
     global launch_count
     _need_cuda(x32)
     if x32.dtype != torch.float32 or not x32.is_contiguous():
         raise _lib.MqdetError("global_max: contiguous fp32 tensor required")
-    out = torch.empty((1,), dtype=torch.float32, device=x32.device)
-    ws = torch.empty((int(load().mqdet_global_max_workspace_floats()),), dtype=torch.float32, device=x32.device)
-    check(load().mqdet_global_max_f32(_ptr(x32), x32.numel(), _ptr(out), _ptr(ws), _stream()), "global_max")
+    segments = int(segments)
+    if segments < 1 or x32.numel() % segments:
+        raise ValueError(f"global_max: {x32.numel()} elements do not split into {segments} equal segments")
+    out = torch.empty((segments,), dtype=torch.float32, device=x32.device)
+    ws = torch.empty((int(load().mqdet_global_max_workspace_floats(segments)),), dtype=torch.float32, device=x32.device)
+    check(load().mqdet_global_max_f32(_ptr(x32), x32.numel(), segments, _ptr(out), _ptr(ws), _stream()), "global_max")
     launch_count += 2
     return out
 
 
-def shift_clamp_(x32, shift, lo, hi):
-    """x = clamp(x - shift[0], lo, hi) in place over the whole (contiguous fp32) buffer; ``shift`` is a device scalar."""
+def shift_clamp_(x32, shift, lo, hi, *, rows_per_shift=0):
+    """x = clamp(x - shift[r // rows_per_shift], lo, hi) in place over the whole (contiguous fp32) buffer, r = the row of the last
+    dim; ``shift`` is on the device (``rows_per_shift = 0``: shift[0] for every element)."""
     global launch_count
     _need_cuda(x32, shift)
     if x32.dtype != torch.float32 or not x32.is_contiguous():
         raise _lib.MqdetError("shift_clamp_: contiguous fp32 tensor required")
-    check(load().mqdet_shift_clamp_f32(_ptr(x32), x32.numel(), _ptr(shift), float(lo), float(hi), _stream()), "shift_clamp")
+    n_row = x32.shape[-1] if x32.dim() else 1
+    _check_shift(shift, x32.numel() // n_row, rows_per_shift, "shift_clamp_")
+    check(load().mqdet_shift_clamp_f32(_ptr(x32), x32.numel(), _ptr(shift), int(rows_per_shift) * n_row, float(lo), float(hi),
+                                       _stream()), "shift_clamp")
     launch_count += 1
     return x32
 
@@ -1161,19 +1181,31 @@ def box_refine_sine(ref_in, valid_ratios, *, delta=None, ref_is_logit=False, wan
     return ref, ref_input, sine
 
 
-def gdino_detections(logits, boxes, tokmap, img_wh, box_threshold, max_out=None):
+def gdino_detections(logits, boxes, tokmap, img_wh, box_threshold, max_out=None, *, class_labels=None):
     """Raw class logits fp32 [B, nq, T] + boxes fp32 [B, nq, 4] (cxcywh, normalised) -> packed [B, max_out + 1, 6]
-    (x1, y1, x2, y2, score, label; last row = count).  tokmap int32 [C, max_tok]; img_wh fp32 [B, 2] = (W, H)."""
+    (x1, y1, x2, y2, score, label; last row = count).  tokmap int32 [C, max_tok] (shared; column c = label c + 1) or
+    [B, C, max_tok] (one table per element: batched prompt chunks); class_labels int32 [C] / [B, C] = the label of each column,
+    columns in ascending label order (ties go to the lowest label), or None (label c + 1); img_wh fp32 [B, 2] = (W, H)."""
     global launch_count
-    _need_cuda(logits, boxes, tokmap, img_wh)
+    _need_cuda(logits, boxes, tokmap, img_wh, class_labels)
     B, nq, T = logits.shape
-    C, max_tok = tokmap.shape
+    C, max_tok = tokmap.shape[-2:]
+    if tokmap.dtype != torch.int32 or not tokmap.is_contiguous() or tokmap.dim() not in (2, 3) or \
+            (tokmap.dim() == 3 and tokmap.shape[0] != B):
+        raise ValueError("gdino_detections: tokmap must be contiguous int32 [C, max_tok] or [B, C, max_tok]")
+    tm_stride = C * max_tok if tokmap.dim() == 3 else 0
+    lab_stride = 0
+    if class_labels is not None:
+        if class_labels.dtype != torch.int32 or not class_labels.is_contiguous() or class_labels.shape[-1] != C or \
+                class_labels.dim() not in (1, 2) or (class_labels.dim() == 2 and class_labels.shape[0] != B):
+            raise ValueError("gdino_detections: class_labels must be contiguous int32 [C] or [B, C]")
+        lab_stride = C if class_labels.dim() == 2 else 0
     max_out = nq if max_out is None else int(max_out)
     out = torch.empty((B, max_out + 1, 6), dtype=torch.float32, device=logits.device)
     ws = torch.empty((int(load().mqdet_gdino_detections_workspace_floats(B, nq)),), dtype=torch.float32, device=logits.device)
-    check(load().mqdet_gdino_detections(_ptr(logits.float().contiguous()), T, _ptr(boxes.float().contiguous()), _ptr(tokmap), C,
-                                        max_tok, _ptr(img_wh.float().contiguous()), float(box_threshold), B, nq, max_out,
-                                        _ptr(out), _ptr(ws), _stream()), "gdino_detections")
+    check(load().mqdet_gdino_detections(_ptr(logits.float().contiguous()), T, _ptr(boxes.float().contiguous()), _ptr(tokmap),
+                                        tm_stride, _ptr(class_labels), lab_stride, C, max_tok, _ptr(img_wh.float().contiguous()),
+                                        float(box_threshold), B, nq, max_out, _ptr(out), _ptr(ws), _stream()), "gdino_detections")
     launch_count += 2
     return out
 

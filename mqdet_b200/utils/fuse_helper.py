@@ -100,10 +100,11 @@ class BiMultiHeadAttention(nn.Module):
                                                                                                            self.head_dim)
 
     @torch.no_grad()
-    def _attend(self, vn16, ln16, mask_l, v_epilogue=None, l_epilogue=None, mask_v=None):
+    def _attend(self, vn16, ln16, mask_l, v_epilogue=None, l_epilogue=None, mask_v=None, per_element_max=False):
         """vn16 [B,N,256] fp16, ln16 [B,T,768] fp16 (already layer-normed), mask_l [B,T] (1 keep / 0 padding) -> (dv, dl).
         ``*_epilogue`` = dict(gate=gamma, residual=normed input) fuses the layer-scale + residual into the out-proj.
-        ``mask_v`` [B,N] (1 keep / 0 padding; GroundingDINO's attention_mask_v) only on the explicit fp32-score path."""
+        ``mask_v`` [B,N] (1 keep / 0 padding; GroundingDINO's attention_mask_v) only on the explicit fp32-score path.
+        ``per_element_max``: STABLE_SOFTMAX_2D subtracts each batch element's own maximum instead of the batch-wide one."""
         B, N, Cv = vn16.shape
         T = ln16.shape[1]
         if self._fused_applies(Cv, T) and mask_v is None:
@@ -126,8 +127,8 @@ class BiMultiHeadAttention(nn.Module):
         vlT = ops.gemm(w16(self.values_l_proj.weight), ln16, bias=f32(self.values_l_proj.bias), bias_mode=VEC_PER_ROW)
 
         qh, kh = q.permute(0, 2, 1, 3), k.permute(0, 2, 1, 3)
-        return self._finish(*self._attend_f32_scores(qh, kh, vvT, vlT, mask_l, self._score_clamp(), B, N, T, Np, mask_v),
-                            v_epilogue, l_epilogue, B, N, T, Cv)
+        return self._finish(*self._attend_f32_scores(qh, kh, vvT, vlT, mask_l, self._score_clamp(), B, N, T, Np, mask_v,
+                                                     per_element_max), v_epilogue, l_epilogue, B, N, T, Cv)
 
     def _query_fold_weights(self):
         """(scale * Wq)^T as fp16 [Cv, E] and scale * bq as fp16 [H, 8, d] (row 0 used), cached per parameter version: the B
@@ -199,9 +200,11 @@ class BiMultiHeadAttention(nn.Module):
                       residual=le["residual"].view(B * T, -1) if le else None)
         return dl.view(B, T, -1)
 
-    def _attend_f32_scores(self, qh, kh, vvT, vlT, mask_l, clamp, B, N, T, Np, mask_v=None):
+    def _attend_f32_scores(self, qh, kh, vvT, vlT, mask_l, clamp, B, N, T, Np, mask_v=None, per_element_max=False):
         """Both score matrices in fp32 (A and its transpose as two products), softmaxes on the fp32 values: the diagnostic
-        variant of the GLIP path and THE path of STABLE_SOFTMAX_2D / an image-token mask (GroundingDINO)."""
+        variant of the GLIP path and THE path of STABLE_SOFTMAX_2D / an image-token mask (GroundingDINO).
+        ``per_element_max``: the STABLE_SOFTMAX_2D maximum is taken per batch element (batched prompt chunks: each chunk's
+        scores are shifted by its own maximum, as in the reference's one-chunk forwards) instead of over the whole batch."""
         H, d = self.num_heads, self.head_dim
         dev = qh.device
         cm = mask_l.float().contiguous() if mask_l is not None else None
@@ -209,10 +212,14 @@ class BiMultiHeadAttention(nn.Module):
         lim = clamp if clamp > 0 else float("inf")
         A32 = torch.empty((B, H, N, T), dtype=torch.float32, device=dev)
         ops.gemm(qh, kh, out=A32, clamp=0.0 if stable else clamp)
+        # per element: shift rows r of element r // (rows of one element) by that element's maximum; 0 = one maximum for all
+        per = per_element_max and B > 1
         if stable:  # attn_weights - attn_weights.max(), then the clamps; the maximum stays on the device, the shift + clamps ride in
-            gmax = ops.global_max(A32)  # the softmax kernels (no pass of their own over the 183 MB score tensors)
+            # the softmax kernels (no pass of their own over the 183 MB score tensors)
+            gmax = ops.global_max(A32, segments=B) if per else ops.global_max(A32)
+            kw = dict(rows_per_shift=H * N) if per else {}
             Pv = ops.softmax_rows_shifted(A32, gmax, -lim, lim, colmask=cm, rows_per_batch=H * N, mask_value=self.mask_fill[0],
-                                          keep_add=self.mask_fill[1])
+                                          keep_add=self.mask_fill[1], **kw)
         else:
             Pv = ops.softmax_rows(A32, colmask=cm, rows_per_batch=H * N, mask_value=self.mask_fill[0], keep_add=self.mask_fill[1])
         del A32
@@ -225,7 +232,7 @@ class BiMultiHeadAttention(nn.Module):
         mv = mask_v.float().contiguous() if mask_v is not None else None
         mkw = dict(colmask=mv, rows_per_batch=H * T, mask_value=float("-inf"), keep_add=0.0) if mv is not None else {}
         if stable:
-            Pl = ops.softmax_rows_shifted(AT32, gmax, -lim, lim, n=N, **mkw)
+            Pl = ops.softmax_rows_shifted(AT32, gmax, -lim, lim, n=N, **mkw, **(dict(rows_per_shift=H * T) if per else {}))
         else:
             Pl = ops.softmax_rows(AT32, n=N, **mkw)
         del AT32
