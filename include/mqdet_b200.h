@@ -524,6 +524,35 @@ int mqdet_gdino_set_loss(const float* logits, const float* boxes, const int32_t*
                          float alpha, float gamma, float w_ce, float w_bbox, float w_giou, float* workspace, float* losses, float* d_logits,
                          float* d_boxes, void* stream);
 
+/* ---- multi-scale / flip test-time augmentation (box_aug.py): the cross-pass merge on the device (bbox_aug.cu) ----
+ *   mqdet_hflip_pad        : in f32 [planes][h][w] -> out f32 [planes][H][W]: every row reversed within the width w, zeros to
+ *                            the right of w and below h.
+ *   mqdet_bbox_aug_collect : appends one pass's candidates (cand_* of mqdet_atss_candidates: rows of S per image, cand_totals
+ *                            on the device) to the merged per-image buffers boxes f32 [B][cap][4], scores f32 [B][cap],
+ *                            labels i32 [B][cap] behind count[b] (device-resident, updated in place).  Per candidate, in this
+ *                            order: flip != 0: x1' = pass_w - x2 - 1, x2' = pass_w - x1 - 1; has_range != 0: kept only if
+ *                            lo2 < (x2 - x1 + 1)(y2 - y1 + 1) < hi2; x *= ratio_x, y *= ratio_y.  Survivors keep the candidate
+ *                            order.  What does not fit in cap is counted in overflow[b], not written.  cap <= 131072.
+ *   mqdet_nms_by_class     : merge_result_from_multi_scales for the whole batch.  classes = sorted i32 [C] (boxes of any other
+ *                            label are dropped).  Per (image, class): order by score descending, equal scores by ascending
+ *                            merged index; vote == 0: greedy suppression of later boxes with IoU > thresh (+1 box convention),
+ *                            survivors by ascending merged index; vote == 1: every box joins the first survivor it overlaps
+ *                            with IoU >= thresh, a cluster of several becomes sum(score * box) / sum(score) with the highest
+ *                            score, clusters in score order; thresh <= 0 keeps every box.  Then, if more than top_n > 0
+ *                            remain in the image, only scores >= the top_n-th largest stay.  out f32 [B][max_out + 1][6] rows
+ *                            (x1, y1, x2, y2, score, label), classes ascending; row max_out = (count, overflow[b] or 0, 0...):
+ *                            count may exceed max_out (rows beyond are not written).  Sums in a fixed order: reruns are
+ *                            bit-identical.  workspace: mqdet_nms_by_class_workspace_bytes, linear in B * cap. */
+int mqdet_hflip_pad(const float* in, int64_t planes, int64_t h, int64_t w, int64_t H, int64_t W, float* out, void* stream);
+int mqdet_bbox_aug_collect(const float* cand_boxes, const float* cand_scores, const float* cand_labels, const int32_t* cand_totals,
+                           int64_t B, int64_t S, int flip, float pass_w, int has_range, float lo2, float hi2, float ratio_x,
+                           float ratio_y, float* boxes, float* scores, int32_t* labels, int64_t cap, int32_t* count,
+                           int32_t* overflow, void* stream);
+int64_t mqdet_nms_by_class_workspace_bytes(int64_t B, int64_t cap, int64_t C);
+int mqdet_nms_by_class(const float* boxes, const float* scores, const int32_t* labels, const int32_t* count, const int32_t* overflow,
+                       int64_t B, int64_t cap, const int32_t* classes, int64_t C, float thresh, int vote, int64_t top_n,
+                       int64_t max_out, float* out, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -171,6 +171,13 @@ SIGNATURES = {
     "mqdet_gdino_set_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
                                      c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_float, c_float, c_void_p, c_void_p,
                                      c_void_p, c_void_p, c_void_p]),
+    "mqdet_hflip_pad": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    "mqdet_bbox_aug_collect": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_float, c_int, c_float,
+                                       c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                       c_void_p]),
+    "mqdet_nms_by_class_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
+    "mqdet_nms_by_class": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float,
+                                   c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -36,7 +36,12 @@ def mq_glip_t_cfg(**over):
                         SHARE_KV=False, NUM_QUERY_PER_CLASS=5, SELECT_FPN_LEVEL=True, QUERY_BANK_PATH="",
                         LEARNABLE_BANK=False, ADD_VISION_LAYER=False, PURE_TEXT_RATE=0.0, RANDOM_KSHOT=False,
                         EXPAND_RATIO=1.5, MAX_QUERY_NUMBER=5000, SIMILARITY_THRESHOLD=0.85),
-        TEST=NS(MDETR_STYLE_AGGREGATE_CLASS_NUM=-1, USE_MULTISCALE=False),
+        # multi-scale / flip test-time augmentation (engine/bbox_aug.py), the values of config/defaults.py:856-867
+        TEST=NS(MDETR_STYLE_AGGREGATE_CLASS_NUM=-1, USE_MULTISCALE=False,
+                SCALES=(400, 500, 600, 640, 700, 900, 1000, 1100, 1200, 1300, 1400, 1800),
+                RANGES=((96, 10000), (96, 10000), (64, 10000), (64, 10000), (64, 10000), (0, 10000), (0, 10000), (0, 256),
+                        (0, 256), (0, 192), (0, 192), (0, 96)),
+                MAX_SIZE=2500, FLIP=True, SPECIAL_NMS="none", TH=0.6, PRE_NMS_TOP_N=1000, NUM_CLASSES=81, SELECT_CLASSES=()),
         INPUT=NS(PIXEL_MEAN=[103.530, 116.280, 123.675], PIXEL_STD=[57.375, 57.120, 58.395]),
         DATALOADER=NS(SIZE_DIVISIBILITY=32),
     )

@@ -561,6 +561,97 @@ def ml_nms(boxes, scores, labels, thresh):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# Multi-scale / flip test-time augmentation: the cross-pass merge (csrc/bbox_aug.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+BBOX_AUG_MAX_CAP = 1 << 17
+
+
+def hflip_pad(images, out_hw):
+    """fp32 [B, C, h, w] -> [B, C, H, W]: every row reversed within the width w, zeros to the right and below (the
+    horizontally flipped batch after SIZE_DIVISIBILITY padding; flipping the normalised tensor equals flipping the image before
+    ToTensor / Normalize, both being per-pixel)."""
+    global launch_count
+    _need_cuda(images)
+    if images.dim() != 4 or images.dtype != torch.float32 or not images.is_contiguous():
+        raise _lib.MqdetError("hflip_pad: contiguous fp32 [B, C, h, w] required")
+    B, C, h, w = images.shape
+    H, W = int(out_hw[0]), int(out_hw[1])
+    out = torch.empty((B, C, H, W), dtype=torch.float32, device=images.device)
+    check(load().mqdet_hflip_pad(_ptr(images), B * C, h, w, H, W, _ptr(out), _stream()), "hflip_pad")
+    launch_count += 1
+    return out
+
+
+class MergedBoxes:
+    """The per-image union of the candidates of every augmentation pass, device-resident: boxes fp32 [B, cap, 4] (original
+    image coordinates), scores fp32 [B, cap], labels int32 [B, cap], count int32 [B] (rows in use), overflow int32 [B]
+    (candidates that did not fit)."""
+
+    def __init__(self, B, cap, device):
+        if not 0 < cap <= BBOX_AUG_MAX_CAP:
+            raise _lib.MqdetError(f"bbox_aug: 1 <= cap <= {BBOX_AUG_MAX_CAP} merged boxes per image (got {cap})")
+        self.B, self.cap = int(B), int(cap)
+        self.boxes = torch.zeros((B, cap, 4), dtype=torch.float32, device=device)
+        self.scores = torch.zeros((B, cap), dtype=torch.float32, device=device)
+        self.labels = torch.zeros((B, cap), dtype=torch.int32, device=device)
+        self.count = torch.zeros((B,), dtype=torch.int32, device=device)
+        self.overflow = torch.zeros((B,), dtype=torch.int32, device=device)
+
+
+def bbox_aug_collect(merged, cand_boxes, cand_scores, cand_labels, cand_totals, pass_size, orig_size, *, flip=False,
+                     keep_range=None):
+    """Append one pass's candidates (``cand_*`` of ``atss_postprocess``) to ``merged``: un-flip about the pass's image width
+    (BoxList.transpose), drop boxes whose area is outside ``keep_range`` = (lo, hi), both bounds strict (remove_boxes), scale
+    from ``pass_size`` to ``orig_size`` (both (width, height); BoxList.resize), in that order.  Candidate order is kept and
+    the running count stays on the device."""
+    import numpy as np
+    global launch_count
+    _need_cuda(cand_boxes, cand_scores, cand_labels, cand_totals)
+    B, S = cand_scores.shape
+    for t, dt in ((cand_boxes, torch.float32), (cand_scores, torch.float32), (cand_labels, torch.float32), (cand_totals, torch.int32)):
+        if t.dtype != dt or not t.is_contiguous():
+            raise _lib.MqdetError("bbox_aug_collect: contiguous fp32 boxes / scores / labels and int32 totals required")
+    if B != merged.B or tuple(cand_boxes.shape) != (B, S, 4):
+        raise _lib.MqdetError(f"bbox_aug_collect: candidates {tuple(cand_boxes.shape)} do not match a merged buffer of {merged.B} images")
+    rx, ry = float(orig_size[0]) / float(pass_size[0]), float(orig_size[1]) / float(pass_size[1])
+    rx32, ry32 = float(np.float32(rx)), float(np.float32(ry))      # tensor * python_float multiplies by the fp32 ratio
+    lo2 = hi2 = 0.0
+    if keep_range is not None:
+        lo2, hi2 = float(np.float32(keep_range[0] * keep_range[0])), float(np.float32(keep_range[1] * keep_range[1]))
+    check(load().mqdet_bbox_aug_collect(_ptr(cand_boxes), _ptr(cand_scores), _ptr(cand_labels), _ptr(cand_totals), B, S, int(bool(flip)),
+                                        float(pass_size[0]), int(keep_range is not None), lo2, hi2, rx32, ry32, _ptr(merged.boxes),
+                                        _ptr(merged.scores), _ptr(merged.labels), merged.cap, _ptr(merged.count),
+                                        _ptr(merged.overflow), _stream()), "bbox_aug_collect")
+    launch_count += 1
+    return merged
+
+
+def nms_by_class(boxes, scores, labels, count, classes, thresh, *, mode="nms", top_n=0, max_out, overflow=None):
+    """merge_result_from_multi_scales for a batch: boxes fp32 [B, cap, 4], scores fp32 [B, cap], labels int32 [B, cap], count
+    int32 [B]; classes = sorted int32 table of the labels considered.  mode "nms" | "vote".  -> packed fp32 [B, max_out + 1, 6]
+    rows (x1, y1, x2, y2, score, label), last row = (count, overflow, 0...).  See include/mqdet_b200.h for the exact rules."""
+    global launch_count
+    _need_cuda(boxes, scores, labels, count, classes, overflow)
+    if mode not in ("nms", "vote"):
+        raise NotImplementedError(f"nms_by_class: mode {mode!r} (only 'nms' and 'vote' are implemented)")
+    B, cap = scores.shape
+    for t, dt in ((boxes, torch.float32), (scores, torch.float32), (labels, torch.int32), (count, torch.int32), (classes, torch.int32)):
+        if t.dtype != dt or not t.is_contiguous():
+            raise _lib.MqdetError("nms_by_class: contiguous fp32 boxes / scores and int32 labels / count / classes required")
+    if tuple(boxes.shape) != (B, cap, 4) or tuple(labels.shape) != (B, cap) or count.numel() != B or classes.dim() != 1:
+        raise _lib.MqdetError("nms_by_class: boxes [B, cap, 4], scores / labels [B, cap], count [B], classes [C] required")
+    C = classes.numel()
+    out = torch.zeros((B, max_out + 1, 6), dtype=torch.float32, device=boxes.device)
+    ws = torch.empty((int(load().mqdet_nms_by_class_workspace_bytes(B, cap, C)),), dtype=torch.uint8, device=boxes.device)
+    check(load().mqdet_nms_by_class(_ptr(boxes), _ptr(scores), _ptr(labels), _ptr(count), _ptr(overflow), B, cap, _ptr(classes), C,
+                                    float(thresh), int(mode == "vote"), int(top_n), int(max_out), _ptr(out), _ptr(ws), _stream()),
+          "nms_by_class")
+    passes = max(0, (max(cap - 1, 1) // 2048).bit_length())
+    launch_count += 6 + 2 * passes
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # DyHead vision path
 # ----------------------------------------------------------------------------------------------------------------------
 class Levels:
