@@ -1504,3 +1504,77 @@ def adamw_step_(param, grad, exp_avg, exp_avg_sq, step, lr, betas=(0.9, 0.999), 
                                   float(betas[1]), float(eps), float(weight_decay), int(step), _ptr(grad_scale), _stream()), "adamw_step")
     launch_count += 1
     return param
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# LVIS box AP (csrc/lvis_eval.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+class LvisPool:
+    """Device-resident detection pool of the LVIS evaluator: score fp32 [cap], box fp32 xywh [cap, 4], img / cat int32 [cap]
+    (indices into the sorted GT image / category ids; cat -1 = empty slot), seq int64 [cap] (arrival number)."""
+
+    def __init__(self, cap, device):
+        self.cap = int(cap)
+        self.score = torch.zeros((cap,), dtype=torch.float32, device=device)
+        self.box = torch.zeros((cap, 4), dtype=torch.float32, device=device)
+        self.img = torch.full((cap,), -1, dtype=torch.int32, device=device)
+        self.cat = torch.full((cap,), -1, dtype=torch.int32, device=device)
+        self.seq = torch.zeros((cap,), dtype=torch.int64, device=device)
+
+    def fields(self):
+        return self.score, self.box, self.img, self.cat, self.seq
+
+
+def lvis_collect(pool, base, seq_base, packed, img_idx, ratios, cat_ids, *, label_map=None, need_img, bad):
+    """Append packed detector rows fp32 [G, B, M + 1, 6] to ``pool`` at slots base + (b * G + g) * M + r (rule 1 conversion with
+    ratios fp32 [B, 2]; img_idx int32 [B]; cat_ids = sorted int32 GT category ids; label_map int32 [L] label -> category id)."""
+    global launch_count
+    _need_cuda(packed, img_idx, ratios, cat_ids, label_map, bad)
+    G, B, M1, six = packed.shape
+    if six != 6 or packed.dtype != torch.float32 or not packed.is_contiguous():
+        raise _lib.MqdetError("lvis_collect: contiguous fp32 [G, B, max_out + 1, 6] required")
+    if base + G * B * (M1 - 1) > pool.cap:
+        raise _lib.MqdetError("lvis_collect: pool full")
+    check(load().mqdet_lvis_collect(_ptr(packed), G, B, M1 - 1, _ptr(img_idx), _ptr(ratios), _ptr(label_map),
+                                    0 if label_map is None else label_map.numel(), _ptr(cat_ids), cat_ids.numel(), int(bool(need_img)),
+                                    *[_ptr(t) for t in pool.fields()], int(base), int(seq_base), _ptr(bad), _stream()), "lvis_collect")
+    launch_count += 1
+
+
+def lvis_cut(src, n, dst, *, by_image, n_groups, k):
+    """The first k rows per category (by_image=False) or image, by score descending then arrival, from src[:n] to dst.
+    -> int32 [1] device count of rows written."""
+    global launch_count
+    count = torch.zeros((1,), dtype=torch.int32, device=src.score.device)
+    ws = torch.empty((load().mqdet_lvis_cut_workspace_bytes(n, n_groups),), dtype=torch.uint8, device=src.score.device)
+    check(load().mqdet_lvis_cut(*[_ptr(t) for t in src.fields()], int(n), int(bool(by_image)), int(n_groups), int(k),
+                                *[_ptr(t) for t in dst.fields()], _ptr(count), _ptr(ws), _stream()), "lvis_cut")
+    launch_count += 1
+    return count
+
+
+def lvis_evaluate(pool, n, gt, *, want_match=False):
+    """Federated filter, greedy matching and accumulation of pool[:n] against an ``LvisGroundTruth``.
+    -> dict(precision fp64 [10, 101, K, 4], recall fp64 [10, K, 4], n_paired int32 [1], order int32 [n], tp_bits / ig_bits int64 [n],
+    match_gt int32 [n, 40] when want_match)."""
+    global launch_count
+    dev = pool.score.device
+    K = len(gt.cat_ids)
+    out = {"precision": torch.full((10, 101, K, 4), -1.0, dtype=torch.float64, device=dev),
+           "recall": torch.full((10, K, 4), -1.0, dtype=torch.float64, device=dev),
+           "n_paired": torch.zeros((1,), dtype=torch.int32, device=dev),
+           "order": torch.empty((max(n, 1),), dtype=torch.int32, device=dev),
+           "tp_bits": torch.empty((max(n, 1),), dtype=torch.int64, device=dev),
+           "ig_bits": torch.empty((max(n, 1),), dtype=torch.int64, device=dev),
+           "match_gt": torch.zeros((max(n, 1), 40), dtype=torch.int32, device=dev) if want_match else None}
+    t = gt.dev
+    ws = torch.empty((load().mqdet_lvis_evaluate_workspace_bytes(n, t["gt_pair"].numel()),), dtype=torch.uint8, device=dev)
+    check(load().mqdet_lvis_evaluate(*[_ptr(x) for x in pool.fields()], int(n), K, _ptr(t["pos_pairs"]), t["pos_pairs"].numel(),
+                                     _ptr(t["neg_pairs"]), t["neg_pairs"].numel(), _ptr(t["nel_pairs"]), t["nel_pairs"].numel(),
+                                     _ptr(t["gt_pair"]), _ptr(t["gt_box"]), _ptr(t["gt_area"]), _ptr(t["gt_ignore"]), _ptr(t["gt_id"]),
+                                     t["gt_pair"].numel(), _ptr(t["num_gt"]), _ptr(t["iou_thrs"]), _ptr(t["rec_thrs"]),
+                                     _ptr(t["area_rng"]), _ptr(out["precision"]), _ptr(out["recall"]), _ptr(out["n_paired"]),
+                                     _ptr(out["order"]), _ptr(out["tp_bits"]), _ptr(out["ig_bits"]), _ptr(out["match_gt"]), _ptr(ws),
+                                     _stream()), "lvis_evaluate")
+    launch_count += 1
+    return out

@@ -51,6 +51,23 @@ def all_gather_packed(packed, group=None, out=None):
     return out
 
 
+def all_gather_rows(rows, head, group=None):
+    """Rows of a different count per rank: rows [n, C] and a small int64 ``head`` [H] (whose entry 0 is n) per rank ->
+    (list of each rank's rows [n_r, C], list of each rank's head) in rank order.  Two collectives: the heads, then the rows
+    padded to the largest n.  Identity when no process group of several ranks is initialised."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return [rows], [head]
+    world = dist.get_world_size(group)
+    heads = [torch.empty_like(head) for _ in range(world)]
+    dist.all_gather(heads, head.contiguous(), group=group)
+    m = max(int(h[0]) for h in heads)
+    pad = torch.zeros((m,) + tuple(rows.shape[1:]), dtype=rows.dtype, device=rows.device)
+    pad[:rows.shape[0]] = rows
+    outs = [torch.empty_like(pad) for _ in range(world)]
+    dist.all_gather(outs, pad, group=group)
+    return [o[:int(h[0])] for o, h in zip(outs, heads)], heads
+
+
 def unshard(det_all, num_all, num_images, world):
     """rank-major gathered rows -> original image order for images sharded with ``shard_indices``."""
     per = det_all.shape[0] // world
