@@ -10,8 +10,8 @@
 //                         V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile): the value
 //                         projection is applied AFTER the token reduction (sum_n p[n] = 1), and the column sums are
 //                         accumulated in-kernel, so the [B, E, N] value tensor of the image side is never built.
-// Each CTA is one warpgroup; a 64-row tile keeps a 64 x 256 fp32 accumulator in its registers (128 per thread).  Operands arrive
-// by TMA (128B swizzle) through a two-stage ring; accumulator fragment: row / column of element i of thread t = wg_row / wg_col.
+// Each MMA warpgroup keeps a 64 x 256 fp32 accumulator in its registers (128 per thread).  Operands arrive by TMA (128B swizzle);
+// accumulator fragment: row / column of element i of thread t = wg_row / wg_col.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/mqdet_b200.h"
@@ -42,7 +42,8 @@ __device__ __forceinline__ float quad_sum(float v) {
 // =====================================================================================================================
 // Fused text -> image side of the bi-directional attention (BiMultiHeadAttention, fuse_helper.py:257-275, 289-291):
 //     out[t, :] = sum_n softmax_n(clamp(k_t . q_n + rowbias_t)) * vn[n, :]   per (image, head), t = text token, n = image token
-// One CTA per (z, 64 text tokens).  The transposed probabilities [T, N] never reach HBM.  Per step of 64 image tokens:
+// One CTA (one warpgroup, two-stage ring) per (z, 64 text tokens).  The transposed probabilities [T, N] never reach HBM.
+// Per step of 64 image tokens:
 //     S^T   = K_tile (64 x 256, resident) . Q_step^T           16 wgmma 64x64x16
 //     P     = exp(clamp(S^T + rowbias) - colmax_t)             in the accumulator fragments -> fp16 A operand (registers)
 //     O    += P . vn_step                                        4 wgmma 64x256x16, O (64 x 256) in registers
@@ -199,23 +200,39 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
 //                              (image, head) by a tiny GEMM — (P V_l,h) W_h^T == P (V_l,h W_h^T), so the per-head context O never
 //                              exists and a head costs two tensor-core products instead of three
 //   out[B][N][256] fp16
-// One CTA per (image, 64-token tile); per tile the heads run back to back:
-//   S (64 x 256 t)   = vn . gT_h^T (+ gbias_h)   16 wgmma 64x256x16, gT_h streamed as [256 x 64] k-blocks
-//   P                = softmax_t(clamp(S) + mask) in the fragments (a row lives in one quad of threads); the column maxima of
-//                      the clamped scores over the tile's valid rows go to colmax_part[b][h][tile][t] (reduced by
-//                      colmax_reduce_kernel) — the text side needs them as the softmax shift
-//   D (64 x 256 o)  += P . mT_h^T                 P from registers; the head sum is kept in thread-private shared memory
-//   out              = res + gamma * (D + bias)
+// One CTA per (image, 64-token tile), 384 threads; per tile the heads run back to back:
+//   warpgroup 0      : producer.  One thread loads the image-token tile once, then streams per head the 4 k-blocks of gT_h and
+//                      the 4 of mT_h ([256 x 64] each, 32 KB) through a STAGES-deep ring with a full and an empty mbarrier per
+//                      stage, so up to STAGES - 1 k-blocks are in flight while the consumers compute.
+//   warpgroups 1, 2  : consumers; warpgroup w owns the text tokens t and the output columns o in [128 w, 128 w + 128):
+//     S_w (64 x 128)  = vn . gT_h[t]^T            16 wgmma 64x128x16 (rows 128 w.. of each gT stage)
+//     column maxima of the clamped scores over the tile's valid rows -> colmax_part[b][h][tile][t] (reduced by
+//                       colmax_reduce_kernel): the text side needs them as the softmax shift
+//     P               = softmax_t(clamp(S) + mask): row max and row sum combined over the two halves in shared memory; both
+//                       halves of P are written to shared memory as one 128B-swizzled [64 x 256 t] A operand
+//     D_h,w (64 x 128) = P . mT_h[o]^T            16 wgmma 64x128x16 over all T (rows 128 w.. of each mT stage)
+//     Dsum_w          += D_h,w                     the head sum, in registers
+//   out[:, o] = res + gamma * (Dsum_w + bias).
+// Every sum runs in the order of a single warpgroup walking the whole row (the row sum continues warpgroup 0's per-thread partial,
+// each D_h element is one K = T chain, and the head sum adds one D_h per head), so the result is bit-identical to computing a
+// tile in one warpgroup.
 // =====================================================================================================================
 struct BiCfg {
+  static constexpr int STAGES = 4;
   static constexpr int VN_BYTES = 4 * KB_BYTES;     // image-token tile [64 x 256 c]
   static constexpr int STAGE_BYTES = 256 * BK * 2;  // one [256 x 64] k-block of gT_h or mT_h
+  static constexpr int P_BYTES = 4 * KB_BYTES;      // probabilities [64 x 256 t] fp16, the A operand of P . mT_h
   static constexpr int MAX_HEADS = 8;
-  static constexpr int D_BYTES = 128 * 128 * 4;     // head sum: [128 fragment elements][128 threads] fp32
-  static constexpr int EXTRA_BYTES = (4 * 256 + MAX_HEADS * 256) * 4;  // cmx, gk
-  static constexpr int SMEM_BYTES = VN_BYTES + 2 * STAGE_BYTES + D_BYTES + EXTRA_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int GK_BYTES = MAX_HEADS * 256 * 4;  // additive row-softmax term per (head, token)
+  static constexpr int GC_BYTES = MAX_HEADS * 256 * 4;  // folded query bias per (head, token) for the column maxima
+  static constexpr int CMX_BYTES = 2 * 4 * 128 * 4;     // column-max partials [consumer warpgroup][warp][128 tokens]
+  static constexpr int XCH_BYTES = (2 * BM + BM + 2 * 128) * 4;  // row max halves, row sums, warpgroup 0's row-sum partials
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int SMEM_BYTES = VN_BYTES + STAGES * STAGE_BYTES + P_BYTES + GK_BYTES + GC_BYTES + CMX_BYTES + XCH_BYTES +
+                                    BAR_BYTES + 1024 /*align*/;
 };
 static_assert(BiCfg::SMEM_BYTES <= 232448, "biattn_image: dynamic shared memory above the 227 KB per-CTA limit");
+static_assert((1 + 2 * BiCfg::STAGES) * 8 <= BiCfg::BAR_BYTES, "biattn_image: barrier space");
 struct BiP {
   const float* mask;   // [B][T] 1 keep / 0 padding, or nullptr
   const float* bias;   // [256] out-projection bias
@@ -231,158 +248,227 @@ struct BiP {
   int B, H, T, N, tiles_per_img;
 };
 
-__global__ void __launch_bounds__(128, 1) biattn_image_kernel(const __grid_constant__ CUtensorMap tma_q,
+__global__ void __launch_bounds__(384, 1) biattn_image_kernel(const __grid_constant__ CUtensorMap tma_q,
                                                               const __grid_constant__ CUtensorMap tma_k,
                                                               const __grid_constant__ CUtensorMap tma_m, const BiP p) {
+  constexpr int STAGES = BiCfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* vnt = smem;
   uint8_t* ring = vnt + BiCfg::VN_BYTES;
-  float* dsum = reinterpret_cast<float*>(ring + 2 * BiCfg::STAGE_BYTES);
-  float* cmx = dsum + 128 * 128;  // [4 warps][256 tokens] column maxima
-  float* gk = cmx + 4 * 256;      // [H][256] additive row-softmax term per (head, token): folded query bias + mask (0 / -inf)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(gk + BiCfg::MAX_HEADS * 256);
+  uint8_t* pt = ring + STAGES * BiCfg::STAGE_BYTES;
+  float* gk = reinterpret_cast<float*>(pt + BiCfg::P_BYTES);  // [H][256]: folded query bias + mask (0 / -inf)
+  float* gc = gk + BiCfg::MAX_HEADS * 256;  // [H][256]: folded query bias, unmasked
+  float* cmx = gc + BiCfg::MAX_HEADS * 256;
+  float* xmax = cmx + 2 * 4 * 128;  // [warpgroup][64 rows]
+  float* xsum = xmax + 2 * BM;      // [64 rows]
+  float* xpart = xsum + BM;         // [128 threads][2 rows]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xpart + 2 * 128);
   uint64_t* vn_full = bars;
-  uint64_t* full = bars + 1;  // [2]
+  uint64_t* full = bars + 1;        // [STAGES]
+  uint64_t* empty = full + STAGES;  // [STAGES]
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int H = p.H;
   const int b = blockIdx.x / p.tiles_per_img, ti = blockIdx.x - b * p.tiles_per_img, m0 = ti * BM;
   const int nq = 8 * H;  // ring sequence: per head 4 k-blocks of gT_h, then 4 of mT_h
-  auto issue = [&](int q) {
-    const int h = q >> 3, kb = q & 3;
-    uint64_t* bar = &full[q & 1];
-    mbar_expect_tx(bar, BiCfg::STAGE_BYTES);
-    tma_load_4d(ring + (q & 1) * BiCfg::STAGE_BYTES, (q & 4) ? &tma_m : &tma_k, bar, kb * BK, 0, h, b);
-  };
-  if (tid == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_k);
     tma_prefetch_desc(&tma_m);
     mbar_init(vn_full, 1);
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 256);  // both consumer warpgroups read every stage
+    }
     fence_mbar_init();
-    mbar_expect_tx(vn_full, BiCfg::VN_BYTES);
-    for (int kb = 0; kb < 4; ++kb) tma_load_4d(vnt + kb * KB_BYTES, &tma_q, vn_full, kb * BK, m0, b, 0);
-    issue(0);
-    issue(1);
   }
+  __syncthreads();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (tid == 0) {
+      mbar_expect_tx(vn_full, BiCfg::VN_BYTES);
+      for (int kb = 0; kb < 4; ++kb) tma_load_4d(vnt + kb * KB_BYTES, &tma_q, vn_full, kb * BK, m0, b, 0);
+      for (int q = 0; q < nq; ++q) {
+        const int s = q % STAGES;
+        mbar_wait(&empty[s], ((q / STAGES) & 1) ^ 1);
+        mbar_expect_tx(&full[s], BiCfg::STAGE_BYTES);
+        tma_load_4d(ring + s * BiCfg::STAGE_BYTES, (q & 4) ? &tma_m : &tma_k, &full[s], (q & 3) * BK, 0, q >> 3, b);
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int w = wg - 1, warp = tid >> 5, lane = tid & 31;
+  const int t0 = 128 * w;  // first text token and first output column of this warpgroup
   constexpr float L2E = 1.4426950408889634f;
   const float NEG_INF = __int_as_float(0xff800000);
   const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
-  for (int t = tid; t < 256; t += 128) {
+  {
+    const int t = threadIdx.x - 128;
     const bool kept = t < p.T && (!p.mask || p.mask[(long)b * p.T + t] != 0.f);
-    for (int hh = 0; hh < H; ++hh)
-      gk[hh * 256 + t] = !kept ? NEG_INF : (p.gbias ? p.gbias[(((long)b * H + hh) * p.T + t) * p.gb_ld] : 0.f);
+    for (int hh = 0; hh < H; ++hh) {
+      const float gb = p.gbias && t < p.T ? p.gbias[(((long)b * H + hh) * p.T + t) * p.gb_ld] : 0.f;
+      gc[hh * 256 + t] = gb;
+      gk[hh * 256 + t] = kept ? gb : NEG_INF;
+    }
   }
-  __syncthreads();
+  named_bar_sync(1, 256);
   bool valid[2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) valid[h] = m0 + wg_row(tid, 2 * h) < p.N;
-  const uint32_t vn_addr = smem_u32(vnt);
-  int q = 0;
-  auto ring_wait = [&](int qq) { mbar_wait(&full[qq & 1], (qq >> 1) & 1); };
-  auto ring_release = [&](int qq) {  // every wgmma of the warpgroup has read stage qq & 1
-    __syncthreads();
-    if (tid == 0 && qq + 2 < nq) issue(qq + 2);
-  };
+  for (int r = 0; r < 2; ++r) valid[r] = m0 + wg_row(tid, 2 * r) < p.N;
+  const int row0 = wg_row(tid, 0);  // this thread's rows: row0 and row0 + 8
+  const uint32_t vn_addr = smem_u32(vnt), ring_addr = smem_u32(ring), pt_addr = smem_u32(pt);
+  float* cw = cmx + w * 512;
+  auto stage_wait = [&](int q) { mbar_wait(&full[q % STAGES], (q / STAGES) & 1); };
+  float dsum[64];
   mbar_wait(vn_full, 0);
   for (int h = 0; h < H; ++h) {
-    // ================= S = vn . gT_h^T =================
-    float sc[128];
+    const int qh = 8 * h;
+    // ================= S_w = vn . gT_h[t0 .. t0 + 127]^T; each k-block's stage is released once its MMAs have retired =========
+    float sc[64];
 #pragma unroll
-    for (int j = 0; j < 128; ++j) sc[j] = 0.f;
-    for (int kb = 0; kb < 4; ++kb, ++q) {
-      ring_wait(q);
-      const uint32_t b0 = smem_u32(ring + (q & 1) * BiCfg::STAGE_BYTES);
-      wgmma_fence_acc(sc);
+    for (int j = 0; j < 64; ++j) sc[j] = 0.f;
+    wgmma_fence_acc(sc);
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb) {
+      stage_wait(qh + kb);
       wgmma_fence();
+      // rows 128 w.. of the [256 x 64] stage: 16 KB further, a multiple of the 1 KB swizzle atom
+      const uint32_t b0 = ring_addr + ((qh + kb) % STAGES) * BiCfg::STAGE_BYTES + w * (128 * 128);
 #pragma unroll
       for (int k = 0; k < 4; ++k)
-        wgmma_ss_m64n256_kk(sc, wg_desc_k_sw128(vn_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(b0 + k * 32), 1);
+        wgmma_ss_m64n128_kk(sc, wg_desc_k_sw128(vn_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(b0 + k * 32), 1);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_acc(sc);
-      ring_release(q);
+      if (kb > 0) {
+        wgmma_wait<1>();
+        mbar_arrive(&empty[(qh + kb - 1) % STAGES]);
+      }
     }
+    wgmma_wait<0>();
+    wgmma_fence_acc(sc);
+    mbar_arrive(&empty[(qh + 3) % STAGES]);
     // ---- column maxima over the tile's valid rows (for the text side): two rows per thread, then the 8 row groups of the warp,
-    //      then the 4 warps through shared memory.  The +-5e4 clamp (fuse_helper.py:245-252) is applied to the REDUCED values
-    //      (clamp is monotonic) ----
+    //      then the 4 warps of the warpgroup through shared memory.  The +-5e4 clamp (fuse_helper.py:245-252) is applied to the
+    //      REDUCED values (clamp is monotonic) ----
 #pragma unroll
-    for (int j = 0; j < 128; j += 4) {
+    for (int j = 0; j < 64; j += 4) {
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         float m = fmaxf(valid[0] ? sc[j + c] : NEG_INF, valid[1] ? sc[j + 2 + c] : NEG_INF);
         m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
         m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
         m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-        if (lane < 4) cmx[warp * 256 + wg_col(tid, j + c)] = m;
+        if (lane < 4) cw[warp * 128 + wg_col(tid, j + c)] = m;
       }
     }
-    __syncthreads();
-    for (int t = tid; t < p.T; t += 128) {
-      float c4 = fmaxf(fmaxf(cmx[t], cmx[256 + t]), fmaxf(cmx[512 + t], cmx[768 + t]));
-      if (p.gbias) c4 += p.gbias[(((long)b * H + h) * p.T + t) * p.gb_ld];  // the text side sees the full score, no mask
-      c4 = fminf(fmaxf(c4, -clampv), clampv);
-      p.colmax_part[(((long)b * H + h) * p.tiles_per_img + ti) * p.T + t] = c4;
-    }
-    // ---- row softmax over the T tokens; `kk` carries the folded query bias and the token mask as an additive 0 / -inf ----
-    const float* kl = gk + h * 256;
+    // ---- row softmax over the T tokens; `kk` carries the folded query bias and the token mask as an additive 0 / -inf.
+    //      Each warpgroup holds half of a row; the halves meet in xmax / xpart / xsum ----
+    const float* kl = gk + h * 256 + t0;
     float mr[2] = {NEG_INF, NEG_INF};
 #pragma unroll
-    for (int j = 0; j < 128; ++j) mr[(j >> 1) & 1] = fmaxf(mr[(j >> 1) & 1], sc[j] + kl[wg_col(tid, j)]);
-    float ml2[2];
-    bool uniform[2];
+    for (int j = 0; j < 64; ++j) {
+      sc[j] += kl[wg_col(tid, j)];  // from here on sc holds S + kk (-inf for masked tokens)
+      mr[(j >> 1) & 1] = fmaxf(mr[(j >> 1) & 1], sc[j]);
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float m_raw = quad_max(mr[r]);
-      // every token masked: the reference's fp32 sum A + (-9e15) swallows A and the softmax is uniform over the T tokens
-      uniform[r] = (m_raw == NEG_INF);
-      ml2[r] = uniform[r] ? 0.f : fminf(fmaxf(m_raw, -clampv), clampv) * L2E;  // max over the kept tokens of the CLAMPED scores
+      mr[r] = quad_max(mr[r]);
+      if ((lane & 3) == 0) xmax[w * BM + row0 + 8 * r] = mr[r];
     }
-    float ls[2] = {0.f, 0.f};
+    named_bar_sync(1, 256);  // cw and xmax written; the previous head's P . mT MMAs have retired in both warpgroups
+    {
+      const int t = t0 + tid;
+      if (t < p.T) {
+        float c4 = fmaxf(fmaxf(cw[tid], cw[128 + tid]), fmaxf(cw[256 + tid], cw[384 + tid]));
+        if (p.gbias) c4 += gc[h * 256 + t];  // the text side sees the full score, no mask
+        c4 = fminf(fmaxf(c4, -clampv), clampv);
+        p.colmax_part[(((long)b * H + h) * p.tiles_per_img + ti) * p.T + t] = c4;
+      }
+    }
+    float ml2[2];
 #pragma unroll
-    for (int j = 0; j < 128; ++j) {
-      const int r = (j >> 1) & 1, c = wg_col(tid, j);
-      const float kk = kl[c];
-      float ev = (kk == NEG_INF) ? 0.f : ex2_approx(fmaf(fminf(fmaxf(sc[j] + kk, -clampv), clampv), L2E, -ml2[r]));
-      if (uniform[r]) ev = (c < p.T) ? 1.f : 0.f;
+    for (int r = 0; r < 2; ++r) {
+      const float m_raw = fmaxf(xmax[row0 + 8 * r], xmax[BM + row0 + 8 * r]);
+      ml2[r] = fminf(fmaxf(m_raw, -clampv), clampv) * L2E;  // max over the kept tokens of the CLAMPED scores
+    }
+    const bool uniform = xmax[row0] == NEG_INF && xmax[BM + row0] == NEG_INF;
+#pragma unroll
+    for (int j = 0; j < 64; ++j) {
+      const int r = (j >> 1) & 1;
+      float ev = (sc[j] == NEG_INF) ? 0.f : ex2_approx(fmaf(fminf(fmaxf(sc[j], -clampv), clampv), L2E, -ml2[r]));
+      // every token of the image masked (the row maximum is -inf for every row of the tile): the reference's fp32 sum
+      // A + (-9e15) swallows A and the softmax is uniform over the T tokens
+      if (uniform) ev = (t0 + wg_col(tid, j) < p.T) ? 1.f : 0.f;
       sc[j] = ev;
-      ls[r] += ev;
     }
-    const float inv[2] = {1.f / quad_sum(ls[0]), 1.f / quad_sum(ls[1])};
+    // row sum: the thread of warpgroup 1 continues the sequential sum of the same thread of warpgroup 0 (the same rows, the
+    // columns 128 further), then the four threads of a row combine
+    float ls[2] = {0.f, 0.f};
+    if (w == 0) {
 #pragma unroll
-    for (int j = 0; j < 128; ++j) sc[j] *= inv[(j >> 1) & 1];
-    uint32_t pa[16][4];
+      for (int j = 0; j < 64; ++j) ls[(j >> 1) & 1] += sc[j];
+      xpart[2 * tid] = ls[0];
+      xpart[2 * tid + 1] = ls[1];
+    }
+    named_bar_sync(1, 256);  // xpart written; cw and xmax have been read
+    if (w == 1) {
+      ls[0] = xpart[2 * tid];
+      ls[1] = xpart[2 * tid + 1];
 #pragma unroll
-    for (int kk = 0; kk < 16; ++kk) acc_to_a(sc, kk, pa[kk]);
-    // ================= D_h = P . mT_h^T, added to the head sum =================
-    float d[128];
+      for (int j = 0; j < 64; ++j) ls[(j >> 1) & 1] += sc[j];
 #pragma unroll
-    for (int j = 0; j < 128; ++j) d[j] = 0.f;
-    for (int kb = 0; kb < 4; ++kb, ++q) {
-      ring_wait(q);
-      const uint32_t b0 = smem_u32(ring + (q & 1) * BiCfg::STAGE_BYTES);
-      wgmma_fence_acc(d);
+      for (int r = 0; r < 2; ++r) {
+        ls[r] = quad_sum(ls[r]);
+        if ((lane & 3) == 0) xsum[row0 + 8 * r] = ls[r];
+      }
+    }
+    named_bar_sync(1, 256);  // xsum written; xpart has been read
+    float inv[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) inv[r] = 1.f / xsum[row0 + 8 * r];
+    // P (fp16) -> this warpgroup's two [64 x 64 t] k-blocks of the swizzled A tile: row r, 16-byte chunk c at chunk c ^ (r & 7)
+#pragma unroll
+    for (int j = 0; j < 64; j += 2) {
+      const int r = wg_row(tid, j), kc = wg_col(tid, j) & 63;
+      const uint32_t a = pt_addr + (2 * w + (j >> 5)) * KB_BYTES + r * 128 + ((((kc >> 3) ^ (r & 7))) << 4) + (kc & 7) * 2;
+      sts32(a, pack_half2(sc[j] * inv[(j >> 1) & 1], sc[j + 1] * inv[(j >> 1) & 1]));
+    }
+    fence_proxy_async();     // the A tile's generic-proxy writes are visible to wgmma
+    named_bar_sync(1, 256);  // both halves of P written; xsum has been read
+    // ================= D_h,w = P . mT_h[t0 .. t0 + 127 (o)]^T over the T tokens, added to the head sum =================
+    float dh[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) dh[j] = 0.f;
+    wgmma_fence_acc(dh);
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb) {
+      stage_wait(qh + 4 + kb);
       wgmma_fence();
+      const uint32_t b0 = ring_addr + ((qh + 4 + kb) % STAGES) * BiCfg::STAGE_BYTES + w * (128 * 128);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_rs_m64n256_kk(d, pa[kb * 4 + k], wg_desc_k_sw128(b0 + k * 32), 1);
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss_m64n128_kk(dh, wg_desc_k_sw128(pt_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(b0 + k * 32), 1);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_acc(d);
-      ring_release(q);
+      if (kb > 0) {
+        wgmma_wait<1>();
+        mbar_arrive(&empty[(qh + 4 + kb - 1) % STAGES]);
+      }
     }
+    wgmma_wait<0>();
+    wgmma_fence_acc(dh);
+    mbar_arrive(&empty[(qh + 7) % STAGES]);
 #pragma unroll
-    for (int j = 0; j < 128; ++j) dsum[j * 128 + tid] = (h == 0 ? 0.f : dsum[j * 128 + tid]) + d[j];
+    for (int j = 0; j < 64; ++j) dsum[j] = (h == 0 ? 0.f : dsum[j]) + dh[j];
   }
-  // ================= epilogue: out = res + gamma * (D + bias) =================
-#pragma unroll 4
-  for (int j = 0; j < 128; j += 2) {
+  // ================= epilogue: out = res + gamma * (Dsum + bias) on this warpgroup's 128 columns =================
+#pragma unroll
+  for (int j = 0; j < 64; j += 2) {
     const long row = m0 + wg_row(tid, j);
-    const int c = wg_col(tid, j);
+    const int c = t0 + wg_col(tid, j);
     if (row >= p.N) continue;
-    float o0 = dsum[j * 128 + tid], o1 = dsum[(j + 1) * 128 + tid];
+    float o0 = dsum[j], o1 = dsum[j + 1];
     const float g0 = p.gamma ? p.gamma[c] : 1.f, g1 = p.gamma ? p.gamma[c + 1] : 1.f;
     const float b0 = p.bias ? p.bias[c] : 0.f, b1 = p.bias ? p.bias[c + 1] : 0.f;
     o0 = (o0 + b0) * g0;  // gamma * (D + bias)
@@ -498,7 +584,7 @@ extern "C" int mqdet_biattn_image(const void* vn, int64_t vn_ld, int64_t vn_b, c
   p.tiles_per_img = (int)((N + BM - 1) / BM);
   rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_image_kernel), BiCfg::SMEM_BYTES);
   if (rc) return rc;
-  biattn_image_kernel<<<(unsigned)(p.tiles_per_img * B), 128, BiCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mq, mk, mm, p);
+  biattn_image_kernel<<<(unsigned)(p.tiles_per_img * B), 384, BiCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mq, mk, mm, p);
   rc = check_launch("biattn_image_kernel");
   if (rc) return rc;
   colmax_reduce_kernel<<<(unsigned)(B * H), 256, 0, (cudaStream_t)stream>>>(workspace, p.tiles_per_img, (int)T, colmax);
