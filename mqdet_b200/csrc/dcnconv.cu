@@ -8,14 +8,18 @@
 //
 // A_j is the bilinearly sampled, mask-modulated column matrix of dyhead.cu's dcn_cols_kernel — here it only ever exists as
 // 64x64 fp16 tiles in shared memory.  Persistent, one CTA (384 threads) per SM walks the 64-row tiles of ALL jobs of the launch:
-//   * warps 8-11 (gather): per tile, every (pixel, tap) gets ONE sampling record in shared memory (four corner offsets, four
-//     corner weights with the modulation mask folded in; 18 KB); then, per k-block (tap, 64 channels), two threads per pixel
-//     fetch 64 contiguous bytes of each corner row (four 128-bit loads), blend in fp32, round once to fp16 and store straight
-//     into the 128B-swizzled K-major A stage; the loads of k-block kb+1 are issued before k-block kb is stored;
-//   * warp 0: the [256 x 64] weight tile of the k-block by TMA;
+//   * warps 0-3 and 8-11 (gather): per tile, every (pixel, tap) gets ONE sampling record in shared memory (four corner
+//     offsets, four corner weights with the modulation mask folded in; 18 KB); then, per k-block (tap, 64 channels), four
+//     threads per pixel fetch 32 contiguous bytes of each corner row (two 128-bit loads), blend in fp32, round once to fp16
+//     and store straight into the 128B-swizzled K-major A stage; the loads of k-block kb+1 are issued before k-block kb is
+//     stored.  Gather thread 0 also requests the [256 x 64] weight tile of the k-block by TMA, one ring slot ahead of the
+//     stores;
 //   * warps 4-7 (one warpgroup): four wgmma.m64n256k16 per k-block, fp32 accumulator in registers (128 per thread), then
 //     +bias -> fp16 -> global stores straight from the accumulator fragments.
-// 64-row tiles keep the 64 x 256 accumulator in one warpgroup's registers next to the gather warps.
+// The corner gathers, not the weight stream, bound the kernel: with two gather warps per scheduler instead of one, each
+// warp's load latency is hidden behind the other's blends.  64-row tiles keep the 64 x 256 accumulator in one warpgroup's
+// registers: 128-row tiles need a second MMA warpgroup, and 384 threads then leave one gather warp per scheduler doing twice
+// the work (measured 40 % slower), while 512 threads cap every thread at 128 registers, below what the m64n256 chain needs.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/mqdet_b200.h"
@@ -27,9 +31,10 @@ constexpr int DC_STAGES = 4;
 constexpr int DC_A_BYTES = DC_BM * DC_BK * 2;  // 8 KB
 constexpr int DC_B_BYTES = DC_BN * DC_BK * 2;  // 32 KB
 constexpr int DC_KB = DC_TAPS * DC_C / DC_BK;  // 36 k-blocks: tap = kb / 4, channels (kb % 4) * 64 ..
-constexpr int DC_GATHER_WARPS = 4;
-constexpr int DC_GATHER_THREADS = DC_GATHER_WARPS * 32;  // two per pixel
-constexpr int DC_THREADS = 256 + DC_GATHER_THREADS;      // warp 0 TMA, warps 4-7 MMA + epilogue, warps 8-11 gather
+constexpr int DC_GATHER_WARPS = 8;
+constexpr int DC_GATHER_THREADS = DC_GATHER_WARPS * 32;  // four per pixel
+constexpr int DC_THREADS = 128 + DC_GATHER_THREADS;      // warps 4-7 MMA + epilogue, warps 0-3 and 8-11 gather
+static_assert(DC_GATHER_THREADS == 4 * DC_BM, "dcn_conv: four gather threads per pixel, two 16-byte chunks each");
 constexpr int DC_COORD_BYTES = DC_TAPS * DC_BM * 32;     // per (tap, row): 4 corner offsets + 4 corner weights
 constexpr int DC_SMEM_BYTES = DC_STAGES * (DC_A_BYTES + DC_B_BYTES) + DC_COORD_BYTES + 1024 /*align*/ + 256 /*barriers*/ +
                               DC_BN * 4 /*bias row*/;
@@ -107,21 +112,7 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
     return j;
   };
 
-  if (warp == 0) {
-    // ---- weight tiles by TMA ------------------------------------------------------------------------------------------
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int j = job_of(tile);
-        for (int kb = 0; kb < DC_KB; ++kb, ++it) {
-          const int s = it % DC_STAGES;
-          mbar_wait(&empty[s], ((it / DC_STAGES) & 1) ^ 1);
-          mbar_expect_tx(&b_full[s], DC_B_BYTES);
-          tma_load_4d(smem_b + s * DC_B_BYTES, &p.map_w[j], &b_full[s], kb * DC_BK, 0, 0, 0);
-        }
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
+  if (warp >= 4 && warp < 8) {
     // ---- MMA + epilogue: registers -> (+bias) -> fp16 -> global ---------------------------------------------------------
     const int tid = threadIdx.x - 128;
     uint32_t it = 0;
@@ -168,19 +159,27 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
           *reinterpret_cast<__half2*>(y + row * DC_BN + col) = __floats2half2_rn(acc[i] + s_bias[col], acc[i + 1] + s_bias[col + 1]);
       }
     }
-  } else if (warp >= 8) {
-    // ---- gather: 2 threads per output pixel, 4 x 8 channels each per k-block -------------------------------------------
-    const int pt = threadIdx.x - 256, rl = pt >> 1, q = pt & 1;
+  } else {
+    // ---- gather: 4 threads per output pixel, 2 x 8 channels each per k-block -------------------------------------------
+    const int pt = warp < 4 ? threadIdx.x : threadIdx.x - 128, rl = pt >> 2, q = pt & 3;
     const int sw = rl & 7;
-    // thread q of a row owns the adjacent 16-byte chunks 4q .. 4q+3 of the 128-byte swizzled row
+    // thread q of a row owns the adjacent 16-byte chunks 2q, 2q+1 of the 128-byte swizzled row
     const uint32_t a_row = smem_u32(smem_a) + rl * 128;
     const uint32_t my_coords = smem_u32(coords) + rl * 32;
     const LevelTable& L = p.lt;
-    const __half* const xa = p.x + q * 32;
+    const __half* const xa = p.x + q * 16;
+    // weight k-block kb of job j into the ring slot of iteration i, once the MMA warpgroup has released it
+    auto load_w = [&](uint32_t i, int j, int kb) {
+      const int s = i % DC_STAGES;
+      mbar_wait(&empty[s], ((i / DC_STAGES) & 1) ^ 1);
+      mbar_expect_tx(&b_full[s], DC_B_BYTES);
+      tma_load_4d(smem_b + s * DC_B_BYTES, &p.map_w[j], &b_full[s], kb * DC_BK, 0, 0, 0);
+    };
+    if (pt == 0) load_w(0, job_of(blockIdx.x), 0);
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int j = job_of(tile);
-      // -- sampling records of the tile: thread pt works out (row pt % 64, taps pt / 64 + 2 i): four corner offsets
+      // -- sampling records of the tile: thread pt works out (row pt % 64, taps pt / 64 + 4 i): four corner offsets
       //    (elements from x) and four corner weights with the modulation mask folded in
       {
         const int branch = p.branch[j];
@@ -247,13 +246,13 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
       //    k-block kb is stored
       uint4 o = lds128u(my_coords);
       float4 w = lds128f(my_coords + 16);
-      uint4 c[4][4];
+      uint4 c[4][2];
       auto load = [&](int ch) {
         const uint32_t off[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
         for (int cr = 0; cr < 4; ++cr)
 #pragma unroll
-          for (int h = 0; h < 4; ++h) c[cr][h] = __ldg(reinterpret_cast<const uint4*>(xa + off[cr] + ch) + h);
+          for (int h = 0; h < 2; ++h) c[cr][h] = __ldg(reinterpret_cast<const uint4*>(xa + off[cr] + ch) + h);
       };
       load(0);
 #pragma unroll 1
@@ -266,17 +265,21 @@ __global__ void __launch_bounds__(DC_THREADS, 1) dcn_conv_kernel(const __grid_co
           o = lds128u(rec);
           w = lds128f(rec + 16);
         }
-        uint4 ob[4];
+        uint4 ob[2];
 #pragma unroll
-        for (int h = 0; h < 4; ++h) ob[h] = blend8(c[0][h], c[1][h], c[2][h], c[3][h], wc.x, wc.y, wc.z, wc.w);
+        for (int h = 0; h < 2; ++h) ob[h] = blend8(c[0][h], c[1][h], c[2][h], c[3][h], wc.x, wc.y, wc.z, wc.w);
         if (nk < DC_KB) load((nk & 3) * DC_BK);
         mbar_wait(&empty[s], ((it / DC_STAGES) & 1) ^ 1);
         const uint32_t dst = a_row + s * DC_A_BYTES;
 #pragma unroll
-        for (int h = 0; h < 4; ++h) sts128(dst + (uint32_t)(((4 * q + h) ^ sw) << 4), ob[h].x, ob[h].y, ob[h].z, ob[h].w);
+        for (int h = 0; h < 2; ++h) sts128(dst + (uint32_t)(((2 * q + h) ^ sw) << 4), ob[h].x, ob[h].y, ob[h].z, ob[h].w);
         fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_full[s]);
+        if (pt == 0) {  // the weight k-block of the next iteration, possibly the first of the next tile
+          if (nk < DC_KB) load_w(it + 1, j, nk);
+          else if (tile + (int)gridDim.x < total_tiles) load_w(it + 1, job_of(tile + gridDim.x), 0);
+        }
       }
       asm volatile("bar.sync 2, %0;" ::"n"(DC_GATHER_THREADS) : "memory");  // every record of this tile has been read
     }
