@@ -553,39 +553,47 @@ int mqdet_nms_by_class(const float* boxes, const float* scores, const int32_t* l
                        int64_t B, int64_t cap, const int32_t* classes, int64_t C, float thresh, int vote, int64_t top_n,
                        int64_t max_out, float* out, void* workspace, void* stream);
 
-/* ---- LVIS box AP (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval), both protocols, on the device (lvis_eval.cu) ----
+/* ---- Box AP on the device (lvis_eval.cu): LVIS (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval, both protocols) and COCO
+ *      (od_eval.py + pycocotools COCOeval, bbox).  Where the protocols differ the rule is an argument, never a protocol switch.
  *   mqdet_lvis_collect : packed f32 [G][B][M + 1][6] detector rows (row M = (count, ...)) -> pool slots base + (b * G + g) * M + r:
- *                        score f32, box f32 xywh (x * ratios[b][0], y * ratios[b][1], then x2 - x1 / y2 - y1, IEEE fp32),
- *                        img i32 = img_idx[b] (-1: not in the GT file), cat i32 = position of the label (through label_map
- *                        [n_labels] when non-null) in the sorted cat_ids [K], -2 when absent, -1 for empty slots and for rows
- *                        the protocol never counts (need_img = 0: cat -2; need_img = 1: img -1), seq i64 = seq_base + slot - base.
- *                        A count row that is not an integer in [0, M] adds 1 to *bad.  Pools hold at most 2^30 rows.
- *   mqdet_lvis_cut     : keeps, per group (by_image = 0: category, 1: image; n_groups groups), the first k rows by score
- *                        descending, then seq ascending; rows with cat = -1 are dropped.  Writes them to the o_* pool in (group,
- *                        score desc, seq) order and their number to *count (device).  workspace: mqdet_lvis_cut_workspace_bytes.
- *   mqdet_lvis_evaluate: the federated filter (img >= 0, cat >= 0, 0 < w * h < inf in fp64, (img << 32 | cat) in pos_pairs or
- *                        neg_pairs, all sorted i64), the greedy matching per (image, category) pair against the GTs (gt_pair
- *                        sorted i64 keys in annotation order, gt_box f64 xywh, gt_area f64, gt_ignore i32, gt_id i64 >= 1) for
- *                        iou_thrs f64 [10] x area_rng f64 [4][2], and the accumulation per category into precision f64
- *                        [10][101][K][4] and recall f64 [10][K][4] (both pre-filled with -1 by the caller; num_gt i32 [K][4] =
- *                        regular GTs per category and range, 0 leaves -1).  Per paired detection i (pairing order: image,
- *                        category, score desc, seq): order[i] = its pool row (-1 past *n_paired), tp_bits / ig_bits bit v =
- *                        matched / ignored at threshold v % 10 in range v / 10, match_gt [i][v] = matched GT id or 0 (optional).
- *                        workspace: mqdet_lvis_evaluate_workspace_bytes. */
+ *                        score f32, box f32 xywh (x * ratios[b][0], y * ratios[b][1], then x2 - x1 / y2 - y1, plus 1 when
+ *                        wh_plus_one, IEEE fp32), img i32 = img_idx[b] (-1: not in the GT file), cat i32 = position of the label
+ *                        (through label_map [n_labels] when non-null) in the sorted cat_ids [K], -2 when absent, -1 for empty
+ *                        slots and for rows the protocol never counts (drop bit 0: cat -2; drop bit 1: img -1), seq i64 =
+ *                        seq_base + slot - base.  A count row that is not an integer in [0, M] adds 1 to *bad.  *bad_img (when
+ *                        non-null) counts the detections on images with img -1, except those the label_map drops (a label outside
+ *                        it, or one it maps to a negative id); without a label_map every detection counts.  Pools hold at most
+ *                        2^30 rows.
+ *   mqdet_lvis_cut     : keeps, per group (group = 0: category, 1: image, 2: (image, category) pair, index img * n_cat + cat;
+ *                        n_groups groups), the first k rows by score descending, then seq ascending; rows with cat = -1 (and, for
+ *                        the pair grouping, img < 0) are dropped.  Writes them to the o_* pool in (group, score desc, seq) order
+ *                        and their number to *count (device).  workspace: mqdet_lvis_cut_workspace_bytes.
+ *   mqdet_lvis_evaluate: pairs the detections with img >= 0 and cat >= 0 (area_filter: only 0 < w * h < inf in fp64; federated: only
+ *                        (img << 32 | cat) in pos_pairs or neg_pairs, all sorted i64), matches them greedily per (image, category)
+ *                        pair against the GTs (gt_pair sorted i64 keys in annotation order, gt_box f64 xywh, gt_area f64, gt_ignore
+ *                        i32, gt_crowd i32 or null: IoU = inter / detection area and never used up, gt_id i64; a match to id 0
+ *                        uses the GT up but is no match) for iou_thrs f64 [10] x area_rng f64 [4][2], and accumulates per category
+ *                        into precision f64 [10][101][K][4][n_max_dets] and recall f64 [10][K][4][n_max_dets] (both pre-filled
+ *                        with -1 by the caller; num_gt i32 [K][4] = regular GTs per category and range, 0 leaves -1; entry m counts
+ *                        a detection when its rank in its pair is below max_dets[m], i32 device [n_max_dets]; null: one entry, no
+ *                        bound).  Per paired detection i (pairing order: image, category, score desc, seq): order[i] = its pool row
+ *                        (-1 past *n_paired), tp_bits / ig_bits bit v = matched / ignored at threshold v % 10 in range v / 10,
+ *                        match_gt [i][v] = matched GT id or 0 (optional).  workspace: mqdet_lvis_evaluate_workspace_bytes. */
 int mqdet_lvis_collect(const float* packed, int64_t G, int64_t B, int64_t M, const int32_t* img_idx, const float* ratios,
-                       const int32_t* label_map, int64_t n_labels, const int32_t* cat_ids, int64_t K, int need_img, float* score,
-                       float* box, int32_t* img, int32_t* cat, int64_t* seq, int64_t base, int64_t seq_base, int32_t* bad,
-                       void* stream);
+                       const int32_t* label_map, int64_t n_labels, const int32_t* cat_ids, int64_t K, int drop, int wh_plus_one,
+                       float* score, float* box, int32_t* img, int32_t* cat, int64_t* seq, int64_t base, int64_t seq_base, int32_t* bad,
+                       int32_t* bad_img, void* stream);
 int64_t mqdet_lvis_cut_workspace_bytes(int64_t n, int64_t n_groups);
 int mqdet_lvis_cut(const float* score, const float* box, const int32_t* img, const int32_t* cat, const int64_t* seq, int64_t n,
-                   int by_image, int64_t n_groups, int64_t k, float* o_score, float* o_box, int32_t* o_img, int32_t* o_cat,
+                   int group, int64_t n_groups, int64_t n_cat, int64_t k, float* o_score, float* o_box, int32_t* o_img, int32_t* o_cat,
                    int64_t* o_seq, int32_t* count, void* workspace, void* stream);
 int64_t mqdet_lvis_evaluate_workspace_bytes(int64_t n, int64_t n_gt);
 int mqdet_lvis_evaluate(const float* score, const float* box, const int32_t* img, const int32_t* cat, const int64_t* seq, int64_t n,
-                        int64_t K, const int64_t* pos_pairs, int64_t n_pos, const int64_t* neg_pairs, int64_t n_neg,
-                        const int64_t* nel_pairs, int64_t n_nel, const int64_t* gt_pair, const double* gt_box, const double* gt_area,
-                        const int32_t* gt_ignore, const int64_t* gt_id, int64_t n_gt, const int32_t* num_gt, const double* iou_thrs,
-                        const double* rec_thrs, const double* area_rng, double* precision, double* recall, int32_t* n_paired,
+                        int64_t K, int federated, const int64_t* pos_pairs, int64_t n_pos, const int64_t* neg_pairs, int64_t n_neg,
+                        const int64_t* nel_pairs, int64_t n_nel, int area_filter, const int64_t* gt_pair, const double* gt_box,
+                        const double* gt_area, const int32_t* gt_ignore, const int32_t* gt_crowd, const int64_t* gt_id, int64_t n_gt,
+                        const int32_t* num_gt, const double* iou_thrs, const double* rec_thrs, const double* area_rng,
+                        const int32_t* max_dets, int64_t n_max_dets, double* precision, double* recall, int32_t* n_paired,
                         int32_t* order, int64_t* tp_bits, int64_t* ig_bits, int32_t* match_gt, void* workspace, void* stream);
 
 #ifdef __cplusplus

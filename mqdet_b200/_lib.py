@@ -179,15 +179,16 @@ SIGNATURES = {
     "mqdet_nms_by_class": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float,
                                    c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "mqdet_lvis_collect": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
-                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+                                   c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
+                                   c_void_p]),
     "mqdet_lvis_cut_workspace_bytes": (c_int64, [c_int64, c_int64]),
-    "mqdet_lvis_cut": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int64, c_void_p, c_void_p,
-                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_lvis_cut": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int64, c_int64, c_void_p,
+                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mqdet_lvis_evaluate_workspace_bytes": (c_int64, [c_int64, c_int64]),
-    "mqdet_lvis_evaluate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p,
-                                    c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
-                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                    c_void_p, c_void_p]),
+    "mqdet_lvis_evaluate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64,
+                                    c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

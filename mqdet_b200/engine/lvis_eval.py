@@ -55,17 +55,6 @@ class LvisGroundTruth:
                 if int(a["id"]) < 1:
                     raise ValueError(f"annotation id {a['id']}: LVIS match arrays use 0 for 'unmatched', ids must be >= 1")
                 rows.append((self.img_pos[a["image_id"]], cat_pos[a["category_id"]], a))
-        order = sorted(range(len(rows)), key=lambda j: (rows[j][0], rows[j][1], j))
-        rows = [rows[j] for j in order]
-        gi = np.array([r[0] for r in rows], np.int64)
-        gc = np.array([r[1] for r in rows], np.int64)
-        box = np.array([r[2]["bbox"] for r in rows], np.float64).reshape(-1, 4)
-        area = np.array([r[2]["area"] for r in rows], np.float64)
-        ign = np.array([1 if r[2].get("ignore", 0) else 0 for r in rows], np.int32)
-        num_gt = np.zeros((len(self.cat_ids), 4), np.int32)
-        for a, (lo, hi) in enumerate(AREA_RNG):
-            ok = (ign == 0) & (area >= lo) & (area <= hi)
-            np.add.at(num_gt[:, a], gc[ok], 1)
         neg, nel = [], []
         for im in annotations["images"]:
             k = self.img_pos[im["id"]]
@@ -76,16 +65,34 @@ class LvisGroundTruth:
             p = np.unique(np.array(p, np.int64).reshape(-1, 2), axis=0) if len(p) else np.zeros((0, 2), np.int64)
             return torch.from_numpy(np.sort(_pairs(p[:, 0], p[:, 1]))).to(dev)
 
-        gt_pair = _pairs(gi, gc)
-        self.dev = {"cat_ids": torch.from_numpy(self.cat_ids.astype(np.int32)).to(dev),
-                    "gt_pair": torch.from_numpy(gt_pair).to(dev), "gt_box": torch.from_numpy(box).to(dev),
-                    "gt_area": torch.from_numpy(area).to(dev), "gt_ignore": torch.from_numpy(ign).to(dev),
-                    "gt_id": torch.tensor([int(r[2]["id"]) for r in rows], dtype=torch.int64).to(dev),
-                    "pos_pairs": torch.from_numpy(np.unique(gt_pair)).to(dev), "neg_pairs": table(neg), "nel_pairs": table(nel),
-                    "num_gt": torch.from_numpy(num_gt).to(dev), "iou_thrs": torch.from_numpy(IOU_THRS).to(dev),
-                    "rec_thrs": torch.from_numpy(REC_THRS).to(dev),
-                    "area_rng": torch.tensor(AREA_RNG, dtype=torch.float64).to(dev)}
+        self.dev = gt_tables(rows, len(self.cat_ids), lambda a: a.get("ignore", 0), dev)
+        self.dev.update({"cat_ids": torch.from_numpy(self.cat_ids.astype(np.int32)).to(dev),
+                         "pos_pairs": torch.unique(self.dev["gt_pair"]), "neg_pairs": table(neg), "nel_pairs": table(nel)})
         self.device = dev
+        self.det_area_filter = True
+
+
+def gt_tables(rows, n_cat, ignore, dev):
+    """The GT side of the device evaluation, shared by the LVIS and COCO ground truths.  rows: (image index, category index,
+    annotation dict) of the GTs that take part; ``ignore(annotation)`` -> its ignore flag.  -> device tables: gt_pair (image << 32 |
+    category, sorted, annotation order within a pair), gt_box fp64 xywh, gt_area fp64 (the ``area`` field), gt_ignore, gt_id,
+    num_gt int32 [K, 4] (GTs not ignored per category and area range), and the IoU / recall thresholds and area ranges."""
+    order = sorted(range(len(rows)), key=lambda j: (rows[j][0], rows[j][1], j))
+    rows = [rows[j] for j in order]
+    gi = np.array([r[0] for r in rows], np.int64)
+    gc = np.array([r[1] for r in rows], np.int64)
+    box = np.array([r[2]["bbox"] for r in rows], np.float64).reshape(-1, 4)
+    area = np.array([r[2]["area"] for r in rows], np.float64)
+    ign = np.array([1 if ignore(r[2]) else 0 for r in rows], np.int32)
+    num_gt = np.zeros((n_cat, 4), np.int32)
+    for a, (lo, hi) in enumerate(AREA_RNG):
+        ok = (ign == 0) & (area >= lo) & (area <= hi)
+        np.add.at(num_gt[:, a], gc[ok], 1)
+    return {"gt_pair": torch.from_numpy(_pairs(gi, gc)).to(dev), "gt_box": torch.from_numpy(box).to(dev),
+            "gt_area": torch.from_numpy(area).to(dev), "gt_ignore": torch.from_numpy(ign).to(dev),
+            "gt_id": torch.tensor([int(r[2]["id"]) for r in rows], dtype=torch.int64).to(dev),
+            "num_gt": torch.from_numpy(num_gt).to(dev), "iou_thrs": torch.from_numpy(IOU_THRS).to(dev),
+            "rec_thrs": torch.from_numpy(REC_THRS).to(dev), "area_rng": torch.tensor(AREA_RNG, dtype=torch.float64).to(dev)}
 
 
 class LvisEvaluatorFixedAP:
@@ -154,11 +161,7 @@ class LvisEvaluatorFixedAP:
         self.eval = {}
 
     def _upload(self, t):
-        """Host table -> device without a host synchronisation (pinned source, asynchronous copy)."""
-        dev = self.gt.device
-        if dev.type == "cuda":
-            t = t.pin_memory()
-        return t.to(dev, non_blocking=True)
+        return upload(t, self.gt.device)
 
     def _cut(self):
         """Keep the top ``topk`` per category (fixed AP) or 300 per image (standard) of the pool, densely."""
@@ -175,24 +178,8 @@ class LvisEvaluatorFixedAP:
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
             return
         self._cut()
-        n, p = self.n, self.pool
-        rows = torch.cat([p.score[:n].view(torch.int32)[:, None], p.box[:n].view(torch.int32), p.img[:n, None], p.cat[:n, None],
-                          p.seq[:n].view(torch.int32).view(n, 2)], 1)
-        head = torch.tensor([n, self.next_seq, int(self.bad.item())], dtype=torch.int64, device=self.gt.device)
-        parts, heads = parallel.all_gather_rows(rows, head, group)
-        total = sum(int(h[0]) for h in heads)
-        pool = ops.LvisPool(max(self.pool.cap, total), self.gt.device)
-        o = base = 0
-        for part, h in zip(parts, heads):
-            k = int(h[0])
-            pool.score[o:o + k] = part[:, 0].view(torch.float32)
-            pool.box[o:o + k] = part[:, 1:5].contiguous().view(torch.float32)
-            pool.img[o:o + k], pool.cat[o:o + k] = part[:, 5], part[:, 6]
-            pool.seq[o:o + k] = part[:, 7:9].contiguous().view(torch.int64)[:, 0] + base
-            o += k
-            base += int(h[1])
-        self.pool, self.n, self.next_seq = pool, total, base
-        self.bad.fill_(sum(int(h[2]) for h in heads))
+        self.pool, self.n, self.next_seq, (bad,) = gather_pool(self.pool, self.n, self.next_seq, [self.bad], group)
+        self.bad.fill_(bad)
         self.eval = {}
 
     # -- evaluation ---------------------------------------------------------------------------------------------------------
@@ -253,6 +240,35 @@ class LvisEvaluatorFixedAP:
         print("saving instances results to ", save_path)
         with open(save_path, "w") as f:
             json.dump(inst, f)
+
+
+def upload(t, dev):
+    """Host table -> device without a host synchronisation (pinned source, asynchronous copy)."""
+    if dev.type == "cuda":
+        t = t.pin_memory()
+    return t.to(dev, non_blocking=True)
+
+
+def gather_pool(pool, n, next_seq, counters, group=None):
+    """All ranks' pool[:n] rows, rank 0's first, with rank r's arrival numbers shifted by the arrivals of ranks 0 .. r-1, and the
+    sums of the int32 [1] ``counters`` over the ranks.  -> (pool, rows, arrivals, [counter sums])."""
+    dev = pool.score.device
+    rows = torch.cat([pool.score[:n].view(torch.int32)[:, None], pool.box[:n].view(torch.int32), pool.img[:n, None],
+                      pool.cat[:n, None], pool.seq[:n].view(torch.int32).view(n, 2)], 1)
+    head = torch.tensor([n, next_seq] + [int(c.item()) for c in counters], dtype=torch.int64, device=dev)
+    parts, heads = parallel.all_gather_rows(rows, head, group)
+    total = sum(int(h[0]) for h in heads)
+    out = ops.LvisPool(max(pool.cap, total), dev)
+    o = base = 0
+    for part, h in zip(parts, heads):
+        k = int(h[0])
+        out.score[o:o + k] = part[:, 0].view(torch.float32)
+        out.box[o:o + k] = part[:, 1:5].contiguous().view(torch.float32)
+        out.img[o:o + k], out.cat[o:o + k] = part[:, 5], part[:, 6]
+        out.seq[o:o + k] = part[:, 7:9].contiguous().view(torch.int64)[:, 0] + base
+        o += k
+        base += int(h[1])
+    return out, total, base, [sum(int(h[2 + j]) for h in heads) for j in range(len(counters))]
 
 
 def summarize(precision, recall, freq_groups, max_dets):

@@ -1507,10 +1507,10 @@ def adamw_step_(param, grad, exp_avg, exp_avg_sq, step, lr, betas=(0.9, 0.999), 
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# LVIS box AP (csrc/lvis_eval.cu)
+# Box AP, LVIS and COCO (csrc/lvis_eval.cu)
 # ----------------------------------------------------------------------------------------------------------------------
 class LvisPool:
-    """Device-resident detection pool of the LVIS evaluator: score fp32 [cap], box fp32 xywh [cap, 4], img / cat int32 [cap]
+    """Device-resident detection pool of the box AP evaluators: score fp32 [cap], box fp32 xywh [cap, 4], img / cat int32 [cap]
     (indices into the sorted GT image / category ids; cat -1 = empty slot), seq int64 [cap] (arrival number)."""
 
     def __init__(self, cap, device):
@@ -1525,56 +1525,81 @@ class LvisPool:
         return self.score, self.box, self.img, self.cat, self.seq
 
 
-def lvis_collect(pool, base, seq_base, packed, img_idx, ratios, cat_ids, *, label_map=None, need_img, bad):
+def lvis_collect(pool, base, seq_base, packed, img_idx, ratios, cat_ids, *, label_map=None, need_img, bad, need_cat=None,
+                 wh_plus_one=False, bad_img=None):
     """Append packed detector rows fp32 [G, B, M + 1, 6] to ``pool`` at slots base + (b * G + g) * M + r (rule 1 conversion with
-    ratios fp32 [B, 2]; img_idx int32 [B]; cat_ids = sorted int32 GT category ids; label_map int32 [L] label -> category id)."""
+    ratios fp32 [B, 2], widths and heights + 1 when ``wh_plus_one``; img_idx int32 [B]; cat_ids = sorted int32 GT category ids;
+    label_map int32 [L] label -> category id).  Rows never counted are marked empty: those of images outside the GT file when
+    ``need_img``, those of categories outside it when ``need_cat`` (default: not ``need_img``).  ``bad_img`` (int32 [1]) counts
+    detections on images outside the GT file."""
     global launch_count
-    _need_cuda(packed, img_idx, ratios, cat_ids, label_map, bad)
+    _need_cuda(packed, img_idx, ratios, cat_ids, label_map, bad, bad_img)
     G, B, M1, six = packed.shape
     if six != 6 or packed.dtype != torch.float32 or not packed.is_contiguous():
         raise _lib.MqdetError("lvis_collect: contiguous fp32 [G, B, max_out + 1, 6] required")
     if base + G * B * (M1 - 1) > pool.cap:
         raise _lib.MqdetError("lvis_collect: pool full")
+    need_cat = not need_img if need_cat is None else need_cat
+    drop = int(bool(need_cat)) | (int(bool(need_img)) << 1)
     check(load().mqdet_lvis_collect(_ptr(packed), G, B, M1 - 1, _ptr(img_idx), _ptr(ratios), _ptr(label_map),
-                                    0 if label_map is None else label_map.numel(), _ptr(cat_ids), cat_ids.numel(), int(bool(need_img)),
-                                    *[_ptr(t) for t in pool.fields()], int(base), int(seq_base), _ptr(bad), _stream()), "lvis_collect")
+                                    0 if label_map is None else label_map.numel(), _ptr(cat_ids), cat_ids.numel(), drop,
+                                    int(bool(wh_plus_one)), *[_ptr(t) for t in pool.fields()], int(base), int(seq_base), _ptr(bad),
+                                    _ptr(bad_img), _stream()), "lvis_collect")
     launch_count += 1
 
 
-def lvis_cut(src, n, dst, *, by_image, n_groups, k):
-    """The first k rows per category (by_image=False) or image, by score descending then arrival, from src[:n] to dst.
-    -> int32 [1] device count of rows written."""
+CUT_BY_CATEGORY, CUT_BY_IMAGE, CUT_BY_PAIR = 0, 1, 2   # the ``group`` argument of mqdet_lvis_cut
+
+
+def lvis_cut(src, n, dst, *, n_groups, k, by_image=False, group=None, n_cat=0):
+    """The first k rows per group, by score descending then arrival, from src[:n] to dst.  ``group``: CUT_BY_CATEGORY,
+    CUT_BY_IMAGE or CUT_BY_PAIR ((image, category) pairs: n_groups = images * n_cat); without it, ``by_image`` picks between
+    the first two (the LVIS protocols).  -> int32 [1] device count of rows written."""
     global launch_count
+    if group is None:
+        group = CUT_BY_IMAGE if by_image else CUT_BY_CATEGORY
+    if group not in (CUT_BY_CATEGORY, CUT_BY_IMAGE, CUT_BY_PAIR):
+        raise _lib.MqdetError(f"lvis_cut: unknown grouping {group!r}")
     count = torch.zeros((1,), dtype=torch.int32, device=src.score.device)
     ws = torch.empty((load().mqdet_lvis_cut_workspace_bytes(n, n_groups),), dtype=torch.uint8, device=src.score.device)
-    check(load().mqdet_lvis_cut(*[_ptr(t) for t in src.fields()], int(n), int(bool(by_image)), int(n_groups), int(k),
+    check(load().mqdet_lvis_cut(*[_ptr(t) for t in src.fields()], int(n), group, int(n_groups), int(n_cat), int(k),
                                 *[_ptr(t) for t in dst.fields()], _ptr(count), _ptr(ws), _stream()), "lvis_cut")
     launch_count += 1
     return count
 
 
 def lvis_evaluate(pool, n, gt, *, want_match=False):
-    """Federated filter, greedy matching and accumulation of pool[:n] against an ``LvisGroundTruth``.
-    -> dict(precision fp64 [10, 101, K, 4], recall fp64 [10, K, 4], n_paired int32 [1], order int32 [n], tp_bits / ig_bits int64 [n],
-    match_gt int32 [n, 40] when want_match)."""
+    """Pairing, greedy matching and accumulation of pool[:n] against a ground truth's device tables ``gt.dev``: the federated
+    filter when they hold ``pos_pairs``, crowd GTs when they hold ``gt_crowd``, a maxDets axis when they hold ``max_dets``; the
+    0 < area < inf filter on detections when ``gt.det_area_filter``.  -> dict(precision fp64 [10, 101, K, 4] (LVIS) or [10, 101, K, 4, M], recall fp64 [10, K, 4] or [10, K, 4, M],
+    n_paired int32 [1], order int32 [n], tp_bits / ig_bits int64 [n], match_gt int32 [n, 40] when want_match)."""
     global launch_count
     dev = pool.score.device
     K = len(gt.cat_ids)
-    out = {"precision": torch.full((10, 101, K, 4), -1.0, dtype=torch.float64, device=dev),
-           "recall": torch.full((10, K, 4), -1.0, dtype=torch.float64, device=dev),
+    t = gt.dev
+    max_dets = t.get("max_dets")
+    M = 1 if max_dets is None else max_dets.numel()
+    tail = () if max_dets is None else (M,)
+    federated = "pos_pairs" in t
+    out = {"precision": torch.full((10, 101, K, 4) + tail, -1.0, dtype=torch.float64, device=dev),
+           "recall": torch.full((10, K, 4) + tail, -1.0, dtype=torch.float64, device=dev),
            "n_paired": torch.zeros((1,), dtype=torch.int32, device=dev),
            "order": torch.empty((max(n, 1),), dtype=torch.int32, device=dev),
            "tp_bits": torch.empty((max(n, 1),), dtype=torch.int64, device=dev),
            "ig_bits": torch.empty((max(n, 1),), dtype=torch.int64, device=dev),
            "match_gt": torch.zeros((max(n, 1), 40), dtype=torch.int32, device=dev) if want_match else None}
-    t = gt.dev
+
+    def table(name):
+        x = t.get(name)
+        return (None, 0) if x is None else (_ptr(x), x.numel())
+
     ws = torch.empty((load().mqdet_lvis_evaluate_workspace_bytes(n, t["gt_pair"].numel()),), dtype=torch.uint8, device=dev)
-    check(load().mqdet_lvis_evaluate(*[_ptr(x) for x in pool.fields()], int(n), K, _ptr(t["pos_pairs"]), t["pos_pairs"].numel(),
-                                     _ptr(t["neg_pairs"]), t["neg_pairs"].numel(), _ptr(t["nel_pairs"]), t["nel_pairs"].numel(),
-                                     _ptr(t["gt_pair"]), _ptr(t["gt_box"]), _ptr(t["gt_area"]), _ptr(t["gt_ignore"]), _ptr(t["gt_id"]),
+    check(load().mqdet_lvis_evaluate(*[_ptr(x) for x in pool.fields()], int(n), K, int(federated), *table("pos_pairs"),
+                                     *table("neg_pairs"), *table("nel_pairs"), int(gt.det_area_filter), _ptr(t["gt_pair"]), _ptr(t["gt_box"]),
+                                     _ptr(t["gt_area"]), _ptr(t["gt_ignore"]), _ptr(t.get("gt_crowd")), _ptr(t["gt_id"]),
                                      t["gt_pair"].numel(), _ptr(t["num_gt"]), _ptr(t["iou_thrs"]), _ptr(t["rec_thrs"]),
-                                     _ptr(t["area_rng"]), _ptr(out["precision"]), _ptr(out["recall"]), _ptr(out["n_paired"]),
-                                     _ptr(out["order"]), _ptr(out["tp_bits"]), _ptr(out["ig_bits"]), _ptr(out["match_gt"]), _ptr(ws),
-                                     _stream()), "lvis_evaluate")
+                                     _ptr(t["area_rng"]), _ptr(max_dets), M, _ptr(out["precision"]), _ptr(out["recall"]),
+                                     _ptr(out["n_paired"]), _ptr(out["order"]), _ptr(out["tp_bits"]), _ptr(out["ig_bits"]),
+                                     _ptr(out["match_gt"]), _ptr(ws), _stream()), "lvis_evaluate")
     launch_count += 1
     return out
