@@ -117,7 +117,10 @@ int mqdet_add_layernorm(const float* a, const float* b, const float* gamma, cons
 /* Sparse GCP attention (modeling_bert_new.py:162-248 with K/V de-duplicated per unique query):
  *   q   [B*T, H*Dh] fp16 (already scaled),  kv [B, V+1, 2*H*Dh] fp16 (row V = padding slot; K | V halves)
  *   idx [B*T, S] int32 in [0, V] (V = padding);  out [B*T, H*Dh] fp16.
- * sim = q.k (+ -1e4 on padding) -> softmax over S -> zero padding probs -> sum p*v. */
+ * sim = q.k (+ -1e4 on padding) -> softmax over S -> zero padding probs -> sum p*v.
+ * S (queries per text token) may be anything in [1, 1760]: each warp keeps its token's S indices and H x S scores in
+ * dynamic shared memory, S x (H + 1) x 4 bytes, which fits a CTA for every H up to 32 at S = 1760.  A larger S is
+ * MQDET_ERR_ARG. */
 int mqdet_gcp_sparse_attn(const void* q, const void* kv, const int32_t* idx, void* out, int64_t B, int64_t T,
                           int64_t V, int64_t S, int64_t H, int64_t Dh, void* stream);
 

@@ -8,13 +8,23 @@
 // token (B*T*S rows).  K/V only depend on the unique query, so here they are projected ONCE for the
 // V+1 rows (row V = the zero padding slot pushed through norm_kv) and the attention kernel gathers the
 // projected rows: one warp per token, 8 heads x 64 dims = 16 contiguous dims per lane, 4 lanes per head,
-// warp-shuffle reductions for q.k, softmax over S in registers.
+// warp-shuffle reductions for q.k.  A token's S indices and H x S scores live in a warp-private slice of
+// dynamic shared memory, so S (NUM_QUERY_PER_CLASS, summed over the classes a token belongs to) is open-ended
+// up to GCP_MAX_S.
+#include <algorithm>
+
 #include "common.cuh"
 #include "../../include/mqdet_b200.h"
 
 namespace mqdet {
 
-constexpr int GCP_MAX_S = 16;
+// Largest S whose one-warp slice, S x (H + 1) words, fits the 227 KB of opt-in shared memory of an sm_90 CTA for every
+// supported head split (H <= 32).  Keep ops.GCP_MAX_S equal.
+constexpr int GCP_MAX_S = 1760;
+constexpr int GCP_SMEM_MAX = 227 * 1024;
+constexpr int GCP_CHUNK = 16;  // slots whose K (or V) row loads are issued together
+constexpr long gcp_slice_bytes(long S, long H) { return S * (H + 1) * 4; }
+static_assert(gcp_slice_bytes(GCP_MAX_S, 32) <= GCP_SMEM_MAX, "GCP_MAX_S slice exceeds the shared-memory limit");
 
 __device__ __forceinline__ void ld16h(const __half* p, float (&f)[16]) {
   const uint4 a = *reinterpret_cast<const uint4*>(p);
@@ -30,58 +40,69 @@ __device__ __forceinline__ void ld16h(const __half* p, float (&f)[16]) {
   }
 }
 
-// Generic in heads/dim as long as H*Dh == 32 * 16 (8x64 GCP) -- lanes_per_head = Dh/16.
+// Generic in heads/dim as long as H*Dh == 32 * 16 (8x64 GCP) -- lanes_per_head = Dh/16, H = 32 / lanes_per_head.
+// Per token: sim = q.k (+ -1e4 on padding slots), max, e = exp(sim - max) and den summed in slot order, p = e / den (0 on
+// padding slots), sum p.v in slot order.  Every lane of a head holds the same score; the slice keeps one copy per head.
 __global__ void __launch_bounds__(256) gcp_sparse_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ kv,
                                                               const int* __restrict__ idx, __half* __restrict__ out,
                                                               long BT, int T, int V, int S, int lanes_per_head) {
-  const long tok = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  extern __shared__ float gcp_smem[];
+  const int lg = __ffs(lanes_per_head) - 1;  // lanes_per_head is a power of two
+  const int H = 32 >> lg;
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int head = lane >> lg;
+  const bool head_leader = (lane & (lanes_per_head - 1)) == 0;
+  int* ids = reinterpret_cast<int*>(gcp_smem + (long)warp * S * (H + 1));  // [S]
+  float* sim = reinterpret_cast<float*>(ids + S);                           // [S][H]
+  const long tok = (long)blockIdx.x * (blockDim.x >> 5) + warp;
   if (tok >= BT) return;
   const int b = (int)(tok / T);
   const int inner = 32 * 16;  // H*Dh
   const __half* kvb = kv + (long)b * (V + 1) * (2 * inner);
   float qf[16];
   ld16h(q + tok * inner + lane * 16, qf);
-  float sim[GCP_MAX_S];
-  int id[GCP_MAX_S];
+  for (int s0 = 0; s0 < S; s0 += GCP_CHUNK) {
 #pragma unroll
-  for (int s = 0; s < GCP_MAX_S; ++s) {
-    if (s < S) {
-      id[s] = idx[tok * S + s];
-      float kf[16];
-      ld16h(kvb + (long)id[s] * (2 * inner) + lane * 16, kf);
-      float d = 0.f;
+    for (int j = 0; j < GCP_CHUNK; ++j) {
+      const int s = s0 + j;
+      if (s < S) {
+        const int id = idx[tok * S + s];
+        float kf[16];
+        ld16h(kvb + (long)id * (2 * inner) + lane * 16, kf);
+        float d = 0.f;
 #pragma unroll
-      for (int i = 0; i < 16; ++i) d = fmaf(qf[i], kf[i], d);
-      for (int o = 1; o < lanes_per_head; o <<= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-      // additive -1e4 on padding slots (":219-223", "for half")
-      sim[s] = d + (id[s] == V ? -1e4f : 0.f);
+        for (int i = 0; i < 16; ++i) d = fmaf(qf[i], kf[i], d);
+        for (int o = 1; o < lanes_per_head; o <<= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+        if (lane == 0) ids[s] = id;
+        // additive -1e4 on padding slots (":219-223", "for half")
+        if (head_leader) sim[s * H + head] = d + (id == V ? -1e4f : 0.f);
+      }
     }
   }
+  __syncwarp();
   float mx = -INFINITY;
-#pragma unroll
-  for (int s = 0; s < GCP_MAX_S; ++s)
-    if (s < S) mx = fmaxf(mx, sim[s]);
+  for (int s = 0; s < S; ++s) mx = fmaxf(mx, sim[s * H + head]);
+  // e, den and p are rounded one operation at a time: never contracted with the last multiply of expf
   float den = 0.f;
-#pragma unroll
-  for (int s = 0; s < GCP_MAX_S; ++s)
-    if (s < S) {
-      sim[s] = expf(sim[s] - mx);
-      den += sim[s];
-    }
+  for (int s = 0; s < S; ++s) den = __fadd_rn(den, expf(sim[s * H + head] - mx));
   const float inv = 1.f / den;
   float acc[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+  for (int s0 = 0; s0 < S; s0 += GCP_CHUNK) {
 #pragma unroll
-  for (int s = 0; s < GCP_MAX_S; ++s) {
-    if (s < S) {
-      // probabilities of padding slots are zeroed AFTER the softmax, without renormalisation (:227-231)
-      const float p = (id[s] == V) ? 0.f : sim[s] * inv;
-      float vf[16];
-      ld16h(kvb + (long)id[s] * (2 * inner) + inner + lane * 16, vf);
+    for (int j = 0; j < GCP_CHUNK; ++j) {
+      const int s = s0 + j;
+      if (s < S) {
+        const int id = ids[s];
+        // probabilities of padding slots are zeroed AFTER the softmax, without renormalisation (:227-231)
+        const float p = (id == V) ? 0.f : __fmul_rn(expf(sim[s * H + head] - mx), inv);
+        float vf[16];
+        ld16h(kvb + (long)id * (2 * inner) + inner + lane * 16, vf);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) acc[i] = fmaf(p, vf[i], acc[i]);
+        for (int i = 0; i < 16; ++i) acc[i] = fmaf(p, vf[i], acc[i]);
+      }
     }
   }
   __half2 h[8];
@@ -155,13 +176,19 @@ extern "C" int mqdet_gcp_sparse_attn(const void* q, const void* kv, const int32_
   MQ_REQUIRE(q && kv && idx && out, "gcp_sparse_attn: null pointer");
   MQ_REQUIRE(H * Dh == 512 && (Dh % 16) == 0 && Dh <= 512, "gcp_sparse_attn: H*Dh must be 512 (got %ld x %ld)", (long)H,
              (long)Dh);
-  MQ_REQUIRE(S >= 1 && S <= GCP_MAX_S, "gcp_sparse_attn: S=%ld out of range [1,%d]", (long)S, GCP_MAX_S);
+  MQ_REQUIRE(S >= 1 && S <= GCP_MAX_S, "gcp_sparse_attn: S=%ld queries per token out of range [1,%d]", (long)S, GCP_MAX_S);
   const int lph = (int)(Dh / 16);
   MQ_REQUIRE((lph & (lph - 1)) == 0, "gcp_sparse_attn: Dh/16 must be a power of two");
   const long BT = B * T;
-  const int wpb = 8;
-  gcp_sparse_attn_kernel<<<cdiv(BT, wpb), wpb * 32, 0, (cudaStream_t)stream>>>((const __half*)q, (const __half*)kv, idx,
-                                                                             (__half*)out, BT, (int)T, (int)V, (int)S, lph);
+  const long slice = gcp_slice_bytes(S, H);
+  const int wpb = (int)std::min<long>(8, GCP_SMEM_MAX / slice);
+  const int smem = (int)(wpb * slice);
+  if (smem > 48 * 1024) {
+    const int rc = ensure_dyn_smem((const void*)gcp_sparse_attn_kernel, smem);
+    if (rc != MQDET_OK) return rc;
+  }
+  gcp_sparse_attn_kernel<<<cdiv(BT, wpb), wpb * 32, smem, (cudaStream_t)stream>>>((const __half*)q, (const __half*)kv, idx,
+                                                                                (__half*)out, BT, (int)T, (int)V, (int)S, lph);
   return check_launch("gcp_sparse_attn_kernel");
 }
 

@@ -21,6 +21,20 @@ from ...utils.weights import f32, w16
 from .modeling_bert_new import _ln16, padded_vision, sparse_index
 
 
+# Most vision queries per text token the sparse-attention backward takes (GCPB_MAX_S in csrc/train.cu); inference takes up to
+# ops.GCP_MAX_S.  MQ-Det pre-trains with 5 queries per class and finetunes with 1 to 10.
+GCP_TRAIN_MAX_S = 16
+
+
+def _train_index(attention_mask):
+    """sparse_index(attention_mask), rejected above GCP_TRAIN_MAX_S queries per token before any training compute is launched."""
+    idx = sparse_index(attention_mask)
+    if idx.shape[2] > GCP_TRAIN_MAX_S:
+        raise MqdetError(f"GCP training: a text token has {idx.shape[2]} vision queries; the GCP backward takes at most "
+                         f"GCP_TRAIN_MAX_S = {GCP_TRAIN_MAX_S} (set VISION_QUERY.NUM_QUERY_PER_CLASS so that no token exceeds it)")
+    return idx
+
+
 def _wT16(weight):
     """[out, in] parameter -> fp16 [in, out_p]: the B operand of dX = dY W (K = out)."""
     return ops.transpose_cast(weight.detach().float().contiguous())
@@ -41,8 +55,8 @@ class GCPBlockTrain:
             raise MqdetError("GCPBlockTrain: CUDA tensors required (no CPU fallback)")
         B, T, D = x.shape
         V = vision.shape[1]
+        idx = _train_index(attention_mask)
         x32 = x.float().contiguous()
-        idx = sparse_index(attention_mask)
         vis_pad = padded_vision(vision)
         xn = _ln16(x32, a.norm)
         q = ops.gemm(xn.view(B * T, D), w16(a.to_q.weight), alpha=a.scale)
@@ -175,6 +189,7 @@ class QVBertModelTrain:
 
     @torch.no_grad()
     def forward(self, input_ids, attention_mask, vision, images, vision_attention_mask):
+        _train_index(vision_attention_mask)
         st = self.model.text_prefix(input_ids, attention_mask, output_hidden_states=False)
         vq = self.pre.forward(vision, images)
         return self.enc.forward(st["h32"], st["colmask"], vq, vision_attention_mask)

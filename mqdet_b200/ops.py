@@ -491,13 +491,21 @@ def gcp_build_index(mask, S):
     return idx, counts
 
 
+# Most vision queries one text token can attend to in gcp_sparse_attn (GCP_MAX_S in csrc/gcp.cu: the largest S whose per-warp
+# shared-memory slice of indices and per-head scores fits a CTA at 32 heads).
+GCP_MAX_S = 1760
+
+
 def gcp_sparse_attn(q, kv, idx, heads, dim_head):
-    """q [B, T, H*Dh] fp16 (scaled), kv [B, V+1, 2*H*Dh] fp16, idx [B, T, S] int32 -> [B, T, H*Dh] fp16."""
+    """q [B, T, H*Dh] fp16 (scaled), kv [B, V+1, 2*H*Dh] fp16, idx [B, T, S] int32 -> [B, T, H*Dh] fp16.
+    Any S in [1, GCP_MAX_S]."""
     global launch_count
     _need_cuda(q, kv, idx)
     B, T, inner = q.shape
     V = kv.shape[1] - 1
     S = idx.shape[2]
+    if not 1 <= S <= GCP_MAX_S:
+        raise _lib.MqdetError(f"gcp_sparse_attn: {S} vision queries per text token; the kernel takes 1 to GCP_MAX_S = {GCP_MAX_S}")
     out = torch.empty_like(q)
     check(load().mqdet_gcp_sparse_attn(_ptr(q), _ptr(kv), _ptr(idx), _ptr(out), B, T, V, S, heads, dim_head, _stream()),
           "gcp_sparse_attn")
