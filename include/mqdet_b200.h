@@ -556,6 +556,28 @@ int mqdet_nms_by_class(const float* boxes, const float* scores, const int32_t* l
                        int64_t B, int64_t cap, const int32_t* classes, int64_t C, float thresh, int vote, int64_t top_n,
                        int64_t max_out, float* out, void* workspace, void* stream);
 
+/* ---- the test transform (data/transforms: Resize -> ToTensor -> Normalize, then to_image_list) on the device (transform.cu) ----
+ *   mqdet_resize_coeffs_ksize : weights per row of the coefficient table of one (n_in, n_out) length pair: 2 * ceil(support) + 1,
+ *                               support = max(n_in / n_out, 1) (fp64); 0 for a non-positive length.
+ *   mqdet_resize_coeffs       : table i32 [n_out][2 + ksize] = (first input index, taps, weights): Pillow's bilinear resampler
+ *                               (PIL.Image.resize(..., BILINEAR)) for one length pair, computed on the device in fp64 with every
+ *                               operation rounded: scale = n_in / n_out, center = (i + 0.5) * scale, first = int(center -
+ *                               support + 0.5) >= 0, end = int(center + support + 0.5) <= n_in, weight = triangle((x + first -
+ *                               center + 0.5) * (1 / max(scale, 1))) over their sequential sum, then x 2^22 rounded half away
+ *                               from zero; zeros past the taps.
+ *   mqdet_test_transform      : B uint8 HWC RGB images -> out f32 [B][3][Hp][Wp].  src, hw (h, w per image), xtab, ytab, mean [3]
+ *                               and std [3] are HOST arrays; src / xtab / ytab hold device pointers (xtab: the (w, ow) table,
+ *                               ytab: the (h, oh) table of the image).  Per image: horizontal pass then vertical pass, each
+ *                               (1 << 21 + sum value * weight) >> 22 clipped to [0, 255] (uint8 intermediate); then per pixel
+ *                               v / 255 (ToTensor); bgr != 0: output channel c reads input channel 2 - c; times255 != 0: v * 255;
+ *                               (v - mean[c]) / std[c]; every step one rounded fp32 operation.  Pixels outside oh x ow are 0.
+ *                               resized (optional) u8 [B][oh][ow][3]: the resized image.  Hp, Wp, h, w < 65536. */
+int64_t mqdet_resize_coeffs_ksize(int64_t n_in, int64_t n_out);
+int mqdet_resize_coeffs(int64_t n_in, int64_t n_out, int32_t* table, void* stream);
+int mqdet_test_transform(const void* const* src, const int64_t* hw, const int32_t* const* xtab, const int32_t* const* ytab, int64_t B,
+                         int64_t oh, int64_t ow, int64_t Hp, int64_t Wp, int bgr, int times255, const float* mean, const float* std,
+                         float* out, uint8_t* resized, void* stream);
+
 /* ---- Box AP on the device (lvis_eval.cu): LVIS (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval, both protocols) and COCO
  *      (od_eval.py + pycocotools COCOeval, bbox).  Where the protocols differ the rule is an argument, never a protocol switch.
  *   mqdet_lvis_collect : packed f32 [G][B][M + 1][6] detector rows (row M = (count, ...)) -> pool slots base + (b * G + g) * M + r:

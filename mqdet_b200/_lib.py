@@ -178,7 +178,11 @@ SIGNATURES = {
     "mqdet_nms_by_class_workspace_bytes": (c_int64, [c_int64, c_int64, c_int64]),
     "mqdet_nms_by_class": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float,
                                    c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
-    "mqdet_lvis_collect": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
+    "mqdet_resize_coeffs_ksize": (c_int64, [c_int64, c_int64]),
+    "mqdet_resize_coeffs": (c_int, [c_int64, c_int64, c_void_p, c_void_p]),
+    "mqdet_test_transform": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_lvis_collect":(c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
                                    c_void_p]),
     "mqdet_lvis_cut_workspace_bytes": (c_int64, [c_int64, c_int64]),

@@ -42,7 +42,9 @@ def mq_glip_t_cfg(**over):
                 RANGES=((96, 10000), (96, 10000), (64, 10000), (64, 10000), (64, 10000), (0, 10000), (0, 10000), (0, 256),
                         (0, 256), (0, 192), (0, 192), (0, 96)),
                 MAX_SIZE=2500, FLIP=True, SPECIAL_NMS="none", TH=0.6, PRE_NMS_TOP_N=1000, NUM_CLASSES=81, SELECT_CLASSES=()),
-        INPUT=NS(PIXEL_MEAN=[103.530, 116.280, 123.675], PIXEL_STD=[57.375, 57.120, 58.395]),
+        # the test transform (engine/transforms.py): config/defaults.py:68-78 and the yaml's INPUT block
+        INPUT=NS(PIXEL_MEAN=[103.530, 116.280, 123.675], PIXEL_STD=[57.375, 57.120, 58.395], MIN_SIZE_TEST=800, MAX_SIZE_TEST=1333,
+                 FORMAT="", TO_BGR255=True),
         DATALOADER=NS(SIZE_DIVISIBILITY=32),
     )
     for k, v in over.items():
@@ -71,7 +73,7 @@ def mq_groundingdino_t_cfg(**over):
     """configs/pretrain/mq-groundingdino-t.yaml + the GROUNDINGDINO block of maskrcnn_benchmark/config/defaults.py:944-1001
     (Swin-T with three outputs + one extra stride-2 level, 6 encoder / 6 decoder layers, 900 queries, two-stage "standard",
     text enhancer + fusion layers + text cross-attention, box threshold 0.05)."""
-    base = {"INPUT.PIXEL_MEAN": [0.485, 0.456, 0.406], "INPUT.PIXEL_STD": [0.229, 0.224, 0.225],
+    base = {"INPUT.PIXEL_MEAN": [0.485, 0.456, 0.406], "INPUT.PIXEL_STD": [0.229, 0.224, 0.225], "INPUT.FORMAT": "rgb",
             "MODEL.ROI_BOX_HEAD.POOLER_SCALES": (0.125, 0.0625, 0.03125, 0.015625)}
     base.update(over)
     cfg = mq_glip_t_cfg(**{k: v for k, v in base.items() if not k.startswith("GROUNDINGDINO.")})

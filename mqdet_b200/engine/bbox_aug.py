@@ -16,6 +16,7 @@ from .. import ops
 from .._lib import MqdetError
 from ..structures.bounding_box import BoxList
 from ..structures.image_list import ImageList
+from .transforms import TestTransform, model_device, upload
 
 _MODES = {"none": "nms", "nms": "nms", "vote": "vote"}
 
@@ -156,3 +157,20 @@ def im_detect_bbox_aug(model, images_by_scale, orig_sizes, captions, positive_ma
     share their size in every pass (the restriction of ``forward_device``) and their original size."""
     packed, _ = im_detect_bbox_aug_device(model, images_by_scale, orig_sizes, captions, positive_map, cap)
     return unpack(packed, orig_sizes)
+
+
+def im_detect_bbox_aug_images(model, images_u8, captions, positive_map, cap=None):
+    """box_aug.py:12-62 from decoded images, as the reference runs it (im_detect_bbox_scale on the original PIL images):
+    images_u8 = uint8 HWC RGB numpy arrays or tensors of one original size -> list[BoxList] in original-image coordinates.
+    Each image crosses to the device once; every ``TEST.SCALES`` batch is made from it there by
+    ``TestTransform(cfg, scale, TEST.MAX_SIZE)`` (bit-identical to the reference's transform), then merged as
+    ``im_detect_bbox_aug``."""
+    cfg = model.cfg
+    dev = model_device(model)
+    images = upload(images_u8, dev)
+    batches, orig = [], None
+    for scale in cfg.TEST.SCALES:
+        il, orig = TestTransform(cfg, scale, cfg.TEST.MAX_SIZE)(images, dev, pad=False)
+        batches.append(il.tensors)
+    packed, _ = im_detect_bbox_aug_device(model, batches, orig, captions, positive_map, cap)
+    return unpack(packed, orig)

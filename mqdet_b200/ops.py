@@ -660,6 +660,57 @@ def nms_by_class(boxes, scores, labels, count, classes, thresh, *, mode="nms", t
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# The test transform: PIL-exact resize, ToTensor, Normalize, padding (csrc/transform.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+def resize_coeffs(n_in, n_out, device):
+    """Coefficient table of PIL's bilinear resampler for one length pair: int32 [n_out, 2 + ksize] rows of (first input
+    index, taps, 22-bit fixed-point weights), built on the device."""
+    global launch_count
+    n_in, n_out = int(n_in), int(n_out)
+    K = int(load().mqdet_resize_coeffs_ksize(n_in, n_out))
+    if K <= 0:
+        raise _lib.MqdetError(f"resize_coeffs: bad lengths {n_in} -> {n_out}")
+    table = torch.empty((n_out, 2 + K), dtype=torch.int32, device=device)
+    check(load().mqdet_resize_coeffs(n_in, n_out, _ptr(table), _stream()), "resize_coeffs")
+    launch_count += 1
+    return table
+
+
+def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False, times255=False, want_resized=False):
+    """uint8 [h_i, w_i, 3] CUDA images (RGB) -> fp32 [B, 3, Hp, Wp]: each image resized to ``out_hw`` = (oh, ow) with
+    ``xtabs[i]`` = resize_coeffs(w_i, ow) and ``ytabs[i]`` = resize_coeffs(h_i, oh), then / 255, channels reversed (``bgr``),
+    x 255 (``times255``), (x - mean) / std, zero beyond (oh, ow) up to ``pad_hw``.  With ``want_resized`` also returns the
+    resized uint8 images [B, oh, ow, 3]."""
+    global launch_count
+    B = len(images)
+    if B == 0 or len(xtabs) != B or len(ytabs) != B:
+        raise _lib.MqdetError("test_transform: one x and one y coefficient table per image required")
+    _need_cuda(*images, *xtabs, *ytabs)
+    (oh, ow), (Hp, Wp) = (int(v) for v in out_hw), (int(v) for v in pad_hw)
+    for im, xt, yt in zip(images, xtabs, ytabs):
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or not im.is_contiguous():
+            raise _lib.MqdetError(f"test_transform: contiguous uint8 [h, w, 3] images required (got {im.dtype} {tuple(im.shape)})")
+        h, w = im.shape[:2]
+        for t, n_in, n_out in ((xt, w, ow), (yt, h, oh)):
+            K = int(load().mqdet_resize_coeffs_ksize(n_in, n_out))
+            if t.dtype != torch.int32 or not t.is_contiguous() or tuple(t.shape) != (n_out, 2 + K):
+                raise _lib.MqdetError(f"test_transform: the coefficient table of {n_in} -> {n_out} must be int32 [{n_out}, {2 + K}]")
+    dev = images[0].device
+    out = torch.empty((B, 3, Hp, Wp), dtype=torch.float32, device=dev)
+    resized = torch.empty((B, oh, ow, 3), dtype=torch.uint8, device=dev) if want_resized else None
+    src = (ctypes.c_void_p * B)(*[im.data_ptr() for im in images])
+    hw = (ctypes.c_int64 * (2 * B))(*[int(v) for im in images for v in im.shape[:2]])
+    xp = (ctypes.c_void_p * B)(*[t.data_ptr() for t in xtabs])
+    yp = (ctypes.c_void_p * B)(*[t.data_ptr() for t in ytabs])
+    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s = (ctypes.c_float * 3)(*[float(v) for v in std])
+    check(load().mqdet_test_transform(src, hw, xp, yp, B, oh, ow, Hp, Wp, int(bool(bgr)), int(bool(times255)), m, s, _ptr(out),
+                                      _ptr(resized), _stream()), "test_transform")
+    launch_count += -(-B // 64)
+    return (out, resized) if want_resized else out
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # DyHead vision path
 # ----------------------------------------------------------------------------------------------------------------------
 class Levels:

@@ -1,7 +1,7 @@
 """BoxList — the output type of the drop-in boundary (maskrcnn_benchmark/structures/bounding_box.py:19-285).
 
 Only the part of the interface that crosses the hot-path boundary: construction, per-box fields, indexing, device moves,
-xyxy <-> xywh with the reference's inclusive-pixel (+1) convention, clipping, area.  The reference's class is a superset
+xyxy <-> xywh with the reference's inclusive-pixel (+1) convention, resizing, clipping, area.  The reference's class is a superset
 and can be passed wherever this one is accepted; tests/test_host_cpu.py pins the shared behaviour against it.
 """
 import torch
@@ -64,6 +64,19 @@ class BoxList(object):
             return self
         b = self.bbox
         return self[(b[:, 3] > b[:, 1]) & (b[:, 2] > b[:, 0])]
+
+    def resize(self, size):
+        """Boxes scaled from ``self.size`` to ``size`` = (width, height): one tensor-times-ratio product when both ratios are
+        equal, else per coordinate on the xyxy form; fields are carried over (those that are not tensors resized too)."""
+        rw, rh = (float(s) / float(s0) for s, s0 in zip(size, self.size))
+        fields = {k: (v if torch.is_tensor(v) else v.resize(size)) for k, v in self.extra_fields.items()}
+        if rw == rh:
+            out = BoxList(self.bbox * rw, size, self.mode)
+        else:
+            b = self.convert("xyxy").bbox
+            out = BoxList(torch.cat((b[:, 0:1] * rw, b[:, 1:2] * rh, b[:, 2:3] * rw, b[:, 3:4] * rh), dim=-1), size, "xyxy")
+        out.extra_fields.update(fields)
+        return out.convert(self.mode)
 
     def area(self):
         b = self.bbox
