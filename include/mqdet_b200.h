@@ -535,7 +535,12 @@ int mqdet_gdino_set_loss(const float* logits, const float* boxes, const int32_t*
  *                            labels i32 [B][cap] behind count[b] (device-resident, updated in place).  Per candidate, in this
  *                            order: flip != 0: x1' = pass_w - x2 - 1, x2' = pass_w - x1 - 1; has_range != 0: kept only if
  *                            lo2 < (x2 - x1 + 1)(y2 - y1 + 1) < hi2; x *= ratio_x, y *= ratio_y.  Survivors keep the candidate
- *                            order.  What does not fit in cap is counted in overflow[b], not written.  cap <= 131072.
+ *                            order.  What does not fit in cap is counted in overflow[b] (bits 0..29, saturating), not
+ *                            written.  cap <= 131072.
+ *   mqdet_bbox_aug_collect_packed : the same for one pass's packed detector rows f32 [B][M + 1][6] = (x1, y1, x2, y2, score,
+ *                            label) with row M = (count, ...), as mqdet_gdino_detections writes them; the count is read on the
+ *                            device.  Same per-row steps, order and arithmetic; rows keep their order.  A count that is not an
+ *                            integer in [0, M] reads no row of that image and sets bit 30 of overflow[b].  M <= 16777216.
  *   mqdet_nms_by_class     : merge_result_from_multi_scales for the whole batch.  classes = sorted i32 [C] (boxes of any other
  *                            label are dropped).  Per (image, class): order by score descending, equal scores by ascending
  *                            merged index; vote == 0: greedy suppression of later boxes with IoU > thresh (+1 box convention),
@@ -551,6 +556,9 @@ int mqdet_bbox_aug_collect(const float* cand_boxes, const float* cand_scores, co
                            int64_t B, int64_t S, int flip, float pass_w, int has_range, float lo2, float hi2, float ratio_x,
                            float ratio_y, float* boxes, float* scores, int32_t* labels, int64_t cap, int32_t* count,
                            int32_t* overflow, void* stream);
+int mqdet_bbox_aug_collect_packed(const float* packed, int64_t B, int64_t M, int flip, float pass_w, int has_range, float lo2,
+                                  float hi2, float ratio_x, float ratio_y, float* boxes, float* scores, int32_t* labels, int64_t cap,
+                                  int32_t* count, int32_t* overflow, void* stream);
 int64_t mqdet_nms_by_class_workspace_bytes(int64_t B, int64_t cap, int64_t C);
 int mqdet_nms_by_class(const float* boxes, const float* scores, const int32_t* labels, const int32_t* count, const int32_t* overflow,
                        int64_t B, int64_t cap, const int32_t* classes, int64_t C, float thresh, int vote, int64_t top_n,

@@ -7,6 +7,7 @@
 //   hflip_pad_kernel       : normalised image -> horizontally flipped, zero-padded batch tensor
 //   aug_collect_kernel     : one pass's candidates -> flip, keep range, resize -> appended behind the earlier passes
 //                            (one CTA per image, ballot scan: candidate order kept; running count on the device)
+//   aug_collect_packed_kernel : the same for one pass's packed detector rows (MQ-GroundingDINO), count read on the device
 //   aug_tile_sort_kernel   : 64-bit keys (class rank | ~score | merged index), bitonic sort of 2048-key tiles
 //   aug_merge_pass_kernel  : one doubling of the sorted run length (rank by binary search in the sibling run)
 //   aug_segments_kernel    : class segment table from the sorted keys
@@ -29,6 +30,9 @@ constexpr int AUG_TILE = 2048;             // keys sorted in shared memory per C
 constexpr int AUG_CH = 128;                // boxes of one class examined together
 constexpr int AUG_NMS_THREADS = 512;       // AUG_CH x 4: four kept-list slices / four 32-bit mask words per box
 constexpr int AUG_KCACHE = 2048;           // kept boxes held in shared memory; later ones are read from the global list
+// overflow[b] holds two things: bits 0..29 count the boxes that did not fit (saturating at AUG_BAD_COUNT - 1, so the count
+// never reaches bit 30), bit 30 flags a packed pass whose count row was not an integer in [0, M].  unpack reads bit 30 first.
+constexpr int AUG_BAD_COUNT = 1 << 30;
 
 __device__ __forceinline__ unsigned ordered_bits(float s) {  // ascending-sortable
   const unsigned u = __float_as_uint(s);
@@ -56,39 +60,61 @@ __global__ void __launch_bounds__(256) hflip_pad_kernel(const float* __restrict_
   out[i] = (x < w && y < h) ? in[(p * h + y) * w + (w - 1 - x)] : 0.f;
 }
 
-// One CTA per image.  Candidate order is kept: per 1024 candidates a ballot scan gives every survivor its slot.
-__global__ void __launch_bounds__(1024) aug_collect_kernel(const float* __restrict__ cboxes, const float* __restrict__ cscores,
-                                                           const float* __restrict__ clabels, const int* __restrict__ totals,
-                                                           int S, int flip, float pass_w, int has_range, float lo2, float hi2,
-                                                           float rx, float ry, float* __restrict__ boxes,
-                                                           float* __restrict__ scores, int* __restrict__ labels, int cap,
-                                                           int* __restrict__ count, int* __restrict__ overflow) {
-  const int b = blockIdx.x;
-  const int n = min(totals[b], S);
-  cboxes += (long)b * S * 4; cscores += (long)b * S; clabels += (long)b * S;
-  boxes += (long)b * cap * 4; scores += (long)b * cap; labels += (long)b * cap;
+// One pass's steps for one box, in the order of im_detect_bbox_aug: un-flip, keep range, resize.  -> whether the box stays.
+__device__ __forceinline__ int aug_pass_box(float4& bx, int flip, float pass_w, int has_range, float lo2, float hi2, float rx,
+                                            float ry) {
+  if (flip) {  // BoxList.transpose(FLIP_LEFT_RIGHT), TO_REMOVE = 1
+    const float x1 = __fsub_rn(__fsub_rn(pass_w, bx.z), 1.f), x2 = __fsub_rn(__fsub_rn(pass_w, bx.x), 1.f);
+    bx.x = x1; bx.z = x2;
+  }
+  int f = 1;
+  if (has_range) {  // remove_boxes: both bounds strict
+    const float area = __fmul_rn(__fadd_rn(__fsub_rn(bx.z, bx.x), 1.f), __fadd_rn(__fsub_rn(bx.w, bx.y), 1.f));
+    f = (area > lo2) && (area < hi2);
+  }
+  bx.x = __fmul_rn(bx.x, rx); bx.z = __fmul_rn(bx.z, rx);  // BoxList.resize to the original image
+  bx.y = __fmul_rn(bx.y, ry); bx.w = __fmul_rn(bx.w, ry);
+  return f;
+}
+
+// The two inputs of a collect, one image each: the cand_* arrays of atss_postprocess, and packed detector rows
+// (x1, y1, x2, y2, score, label) as gdino_detections writes them.
+struct AugCandRows {
+  const float4* boxes;
+  const float* scores;
+  const float* labels;
+  __device__ __forceinline__ void load(int i, float4& bx, float& s, int& lab) const {
+    bx = boxes[i]; s = scores[i]; lab = (int)labels[i];
+  }
+};
+struct AugPackedRows {
+  const float* rows;
+  __device__ __forceinline__ void load(int i, float4& bx, float& s, int& lab) const {
+    const float* r = rows + (long)i * 6;
+    bx = make_float4(r[0], r[1], r[2], r[3]); s = r[4]; lab = (int)r[5];
+  }
+};
+
+// One CTA appends the first n rows of one image's pass behind count[0] (pointers already at the image).  Row order is kept:
+// per 1024 rows a ballot scan gives every survivor its slot.
+template <class Rows>
+__device__ __forceinline__ void aug_collect_image(const Rows src, int n, int flip, float pass_w, int has_range, float lo2,
+                                                  float hi2, float rx, float ry, float* __restrict__ boxes,
+                                                  float* __restrict__ scores, int* __restrict__ labels, int cap,
+                                                  int* __restrict__ count, int* __restrict__ overflow) {
   __shared__ int warp_tot[32];
   __shared__ int running;
-  if (threadIdx.x == 0) running = count[b];
+  if (threadIdx.x == 0) running = *count;
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int base = 0; base < n; base += 1024) {
     const int i = base + threadIdx.x;
-    int f = 0;
+    int f = 0, lab = 0;
+    float sc = 0.f;
     float4 bx = make_float4(0.f, 0.f, 0.f, 0.f);
     if (i < n) {
-      bx = reinterpret_cast<const float4*>(cboxes)[i];
-      if (flip) {  // BoxList.transpose(FLIP_LEFT_RIGHT), TO_REMOVE = 1
-        const float x1 = __fsub_rn(__fsub_rn(pass_w, bx.z), 1.f), x2 = __fsub_rn(__fsub_rn(pass_w, bx.x), 1.f);
-        bx.x = x1; bx.z = x2;
-      }
-      f = 1;
-      if (has_range) {  // remove_boxes: both bounds strict
-        const float area = __fmul_rn(__fadd_rn(__fsub_rn(bx.z, bx.x), 1.f), __fadd_rn(__fsub_rn(bx.w, bx.y), 1.f));
-        f = (area > lo2) && (area < hi2);
-      }
-      bx.x = __fmul_rn(bx.x, rx); bx.z = __fmul_rn(bx.z, rx);  // BoxList.resize to the original image
-      bx.y = __fmul_rn(bx.y, ry); bx.w = __fmul_rn(bx.w, ry);
+      src.load(i, bx, sc, lab);
+      f = aug_pass_box(bx, flip, pass_w, has_range, lo2, hi2, rx, ry);
     }
     const unsigned ball = __ballot_sync(0xffffffffu, f);
     if (lane == 0) warp_tot[warp] = __popc(ball);
@@ -102,8 +128,8 @@ __global__ void __launch_bounds__(1024) aug_collect_kernel(const float* __restri
     const int pos = start + woff + __popc(ball & ((1u << lane) - 1));
     if (f && pos < cap) {
       reinterpret_cast<float4*>(boxes)[pos] = bx;
-      scores[pos] = cscores[i];
-      labels[pos] = (int)clabels[i];
+      scores[pos] = sc;
+      labels[pos] = lab;
     }
     __syncthreads();
     if (threadIdx.x == 0) running = start + tot;
@@ -111,9 +137,41 @@ __global__ void __launch_bounds__(1024) aug_collect_kernel(const float* __restri
   }
   if (threadIdx.x == 0) {
     const int r = running;
-    count[b] = min(r, cap);
-    if (r > cap) overflow[b] += r - cap;
+    *count = min(r, cap);
+    if (r > cap) {
+      const int lost = (int)min((long long)(*overflow & (AUG_BAD_COUNT - 1)) + (r - cap), (long long)AUG_BAD_COUNT - 1);
+      *overflow = (*overflow & AUG_BAD_COUNT) | lost;
+    }
   }
+}
+
+// One CTA per image.
+__global__ void __launch_bounds__(1024) aug_collect_kernel(const float* __restrict__ cboxes, const float* __restrict__ cscores,
+                                                           const float* __restrict__ clabels, const int* __restrict__ totals,
+                                                           int S, int flip, float pass_w, int has_range, float lo2, float hi2,
+                                                           float rx, float ry, float* __restrict__ boxes,
+                                                           float* __restrict__ scores, int* __restrict__ labels, int cap,
+                                                           int* __restrict__ count, int* __restrict__ overflow) {
+  const int b = blockIdx.x;
+  const AugCandRows src{reinterpret_cast<const float4*>(cboxes) + (long)b * S, cscores + (long)b * S, clabels + (long)b * S};
+  aug_collect_image(src, min(totals[b], S), flip, pass_w, has_range, lo2, hi2, rx, ry, boxes + (long)b * cap * 4,
+                    scores + (long)b * cap, labels + (long)b * cap, cap, count + b, overflow + b);
+}
+
+// One CTA per image; packed [B][M + 1][6], row M = (count, ...).  A count that is not an integer in [0, M] reads no row and
+// sets AUG_BAD_COUNT in overflow[b], which unpack reports.
+__global__ void __launch_bounds__(1024) aug_collect_packed_kernel(const float* __restrict__ packed, int M, int flip, float pass_w,
+                                                                  int has_range, float lo2, float hi2, float rx, float ry,
+                                                                  float* __restrict__ boxes, float* __restrict__ scores,
+                                                                  int* __restrict__ labels, int cap, int* __restrict__ count,
+                                                                  int* __restrict__ overflow) {
+  const int b = blockIdx.x;
+  const float* rows = packed + (long)b * (M + 1) * 6;
+  const float cnt = rows[(long)M * 6];
+  const bool ok = cnt >= 0.f && cnt <= (float)M && cnt == floorf(cnt);
+  aug_collect_image(AugPackedRows{rows}, ok ? (int)cnt : 0, flip, pass_w, has_range, lo2, hi2, rx, ry, boxes + (long)b * cap * 4,
+                    scores + (long)b * cap, labels + (long)b * cap, cap, count + b, overflow + b);
+  if (!ok && threadIdx.x == 0) overflow[b] |= AUG_BAD_COUNT;
 }
 
 // ---- sort ----------------------------------------------------------------------------------------------------------
@@ -493,6 +551,18 @@ extern "C" int mqdet_bbox_aug_collect(const float* cand_boxes, const float* cand
                                                                      pass_w, has_range, lo2, hi2, ratio_x, ratio_y, boxes, scores,
                                                                      labels, (int)cap, count, overflow);
   return check_launch("aug_collect_kernel");
+}
+
+extern "C" int mqdet_bbox_aug_collect_packed(const float* packed, int64_t B, int64_t M, int flip, float pass_w, int has_range,
+                                             float lo2, float hi2, float ratio_x, float ratio_y, float* boxes, float* scores,
+                                             int32_t* labels, int64_t cap, int32_t* count, int32_t* overflow, void* stream) {
+  MQ_REQUIRE(packed && boxes && scores && labels && count && overflow, "bbox_aug_collect_packed: null pointer");
+  MQ_REQUIRE(B > 0 && M > 0 && M <= (1 << 24) && cap > 0 && cap <= AUG_MAX_CAP,
+             "bbox_aug_collect_packed: bad sizes B=%ld M=%ld cap=%ld (M <= %d, cap <= %d)", (long)B, (long)M, (long)cap, 1 << 24,
+             AUG_MAX_CAP);
+  aug_collect_packed_kernel<<<(unsigned)B, 1024, 0, (cudaStream_t)stream>>>(packed, (int)M, flip, pass_w, has_range, lo2, hi2, ratio_x,
+                                                                            ratio_y, boxes, scores, labels, (int)cap, count, overflow);
+  return check_launch("aug_collect_packed_kernel");
 }
 
 extern "C" int64_t mqdet_nms_by_class_workspace_bytes(int64_t B, int64_t cap, int64_t C) {

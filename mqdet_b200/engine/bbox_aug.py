@@ -1,4 +1,4 @@
-"""Multi-scale + horizontal-flip test-time augmentation for MQ-GLIP, drop-in for
+"""Multi-scale + horizontal-flip test-time augmentation for MQ-GLIP and MQ-GroundingDINO, drop-in for
 maskrcnn_benchmark/data/datasets/evaluation/box_aug.py (``TEST.USE_MULTISCALE``).
 
 The detector runs on every image at each of ``TEST.SCALES`` and again on the flipped image when ``TEST.FLIP``; boxes outside
@@ -9,6 +9,13 @@ The reference merges on the host (a Python loop over the classes of every image,
 per image, numpy ``np.delete`` per voting cluster).  Here the candidates of a pass never leave the device: each pass appends
 to a per-image device buffer (``ops.bbox_aug_collect``), one ``ops.nms_by_class`` merges the whole batch, and the packed result
 is the one device->host copy.  Nothing synchronises with the host between the first forward and that copy.
+
+What a pass hands to the merge is what the reference's box_aug.py receives from the model: for MQ-GLIP the pre-NMS candidates
+of ATSSPostProcessor (``cand_*``, bbox_aug_enabled), for MQ-GroundingDINO its final output (convert_groundingdino_to_glip_output:
+every query above box_threshold, in query order, clipped, no NMS), i.e. the packed rows of ``gdino_detections``
+(``ops.bbox_aug_collect_packed``).  A GroundingDINO pass runs through ``forward_chunked_device`` with the prompt as its only
+chunk: that path takes the fusion layers' stable-softmax maximum per image, so every image of the batch gets what the
+reference's one-image forward gives it (``forward_device`` takes one maximum over the whole batch).
 """
 import torch
 
@@ -35,7 +42,7 @@ def _classes(test_cfg, device):
     if sel != sorted(set(sel)):   # the result lists the classes in table order; the reference walks SELECT_CLASSES as given
         raise ValueError(f"TEST.SELECT_CLASSES must be ascending without repeats (got {tuple(sel)})")
     cls = sel if len(sel) else list(range(1, int(test_cfg.NUM_CLASSES)))
-    return torch.tensor(cls, dtype=torch.int32, device=device)
+    return ops.upload_async(torch.tensor(cls, dtype=torch.int32), device)
 
 
 def result_rows(test_cfg, cap):
@@ -53,6 +60,8 @@ def unpack(packed, sizes):
     res = []
     for b, size in enumerate(sizes):
         n, lost = int(round(float(pk[b, rows, 0]))), int(round(float(pk[b, rows, 1])))
+        if lost >= ops.BBOX_AUG_BAD_COUNT:
+            raise MqdetError(f"image {b}: a detector pass gave a count row that is not an integer in [0, rows]")
         if lost:
             raise MqdetError(f"image {b}: {lost} candidates did not fit in the merged buffer; raise `cap`")
         if n > rows:
@@ -110,7 +119,10 @@ def merge_result_from_multi_scales(boxlists, cfg, cap=None):
 def im_detect_bbox_aug_device(model, images_by_scale, orig_sizes, captions, positive_map, cap=None):
     """Device-resident form of ``im_detect_bbox_aug``: returns (packed fp32 [B, rows + 1, 6], merged ``ops.MergedBoxes``);
     packed rows are (x1, y1, x2, y2, score, label) in original-image coordinates, row ``rows`` = (count, candidates lost to a
-    full merged buffer, 0...).  ``cap``: merged candidates kept per image (default: every candidate of every pass)."""
+    full merged buffer, 0...).  ``cap``: merged candidates kept per image (default: every candidate of every pass, for
+    MQ-GroundingDINO passes x num_queries)."""
+    from ..modeling.groundingdino.groundingdino import GroundingDINO
+    gdino = isinstance(model, GroundingDINO)
     cfg = model.cfg
     t = cfg.TEST
     mode = _mode(t)
@@ -121,6 +133,7 @@ def im_detect_bbox_aug_device(model, images_by_scale, orig_sizes, captions, posi
     B = images_by_scale[0].shape[0]
     if any(tuple(s) != tuple(orig_sizes[0]) for s in orig_sizes):
         raise NotImplementedError("im_detect_bbox_aug batches images of one original size; call it per size group")
+    classes = _classes(t, images_by_scale[0].device)
     div = int(cfg.DATALOADER.SIZE_DIVISIBILITY)
     merged = None
     for x, rng in zip(images_by_scale, ranges):
@@ -135,16 +148,23 @@ def im_detect_bbox_aug_device(model, images_by_scale, orig_sizes, captions, posi
             else:
                 batch = x.new_zeros((B, x.shape[1], H, W))
                 batch[..., :h, :w] = x
-            out = model.forward_device(ImageList(batch, [(h, w)] * B), captions, positive_map)
-            if merged is None:
+            images = ImageList(batch, [(h, w)] * B)
+            if gdino:
+                out = model.forward_chunked_device(images, [captions], [positive_map], chunks_per_pass=1)
+                S = out["det_packed"].shape[2] - 1
+            else:
+                out = model.forward_device(images, captions, positive_map)
                 S = out["cand_scores"].shape[1]
+            if merged is None:
                 passes = len(scales) * (2 if t.FLIP else 1)
                 merged = ops.MergedBoxes(B, min(S * passes, ops.BBOX_AUG_MAX_CAP) if cap is None else cap, x.device)
-            ops.bbox_aug_collect(merged, out["cand_boxes"], out["cand_scores"], out["cand_labels"], out["cand_totals"], (w, h),
-                                 orig_sizes[0], flip=flip, keep_range=rng)
-    packed = ops.nms_by_class(merged.boxes, merged.scores, merged.labels, merged.count, _classes(t, merged.boxes.device),
-                              float(t.TH), mode=mode, top_n=int(t.PRE_NMS_TOP_N), max_out=result_rows(t, merged.cap),
-                              overflow=merged.overflow)
+            if gdino:
+                ops.bbox_aug_collect_packed(merged, out["det_packed"][0], (w, h), orig_sizes[0], flip=flip, keep_range=rng)
+            else:
+                ops.bbox_aug_collect(merged, out["cand_boxes"], out["cand_scores"], out["cand_labels"], out["cand_totals"], (w, h),
+                                     orig_sizes[0], flip=flip, keep_range=rng)
+    packed = ops.nms_by_class(merged.boxes, merged.scores, merged.labels, merged.count, classes, float(t.TH), mode=mode,
+                              top_n=int(t.PRE_NMS_TOP_N), max_out=result_rows(t, merged.cap), overflow=merged.overflow)
     return packed, merged
 
 
@@ -154,7 +174,8 @@ def im_detect_bbox_aug(model, images_by_scale, orig_sizes, captions, positive_ma
     images_by_scale: one fp32 CUDA batch [B, 3, h_i, w_i] per entry of ``TEST.SCALES``, already resized
     (``T.Resize(scale, TEST.MAX_SIZE)``) and normalised, not padded — resizing is work of the data pipeline, as in the
     reference; the flipped passes are made here on the device.  orig_sizes: (width, height) per image.  The images of a batch
-    share their size in every pass (the restriction of ``forward_device``) and their original size."""
+    share their size in every pass (the restriction of ``forward_device``) and their original size.  ``model``: MQ-GLIP
+    (``GeneralizedVLRCNN_New``) or MQ-GroundingDINO (``GroundingDINO``; each image's result is the one it gets alone)."""
     packed, _ = im_detect_bbox_aug_device(model, images_by_scale, orig_sizes, captions, positive_map, cap)
     return unpack(packed, orig_sizes)
 

@@ -362,37 +362,56 @@ class GroundingDINO(nn.Module):
     @torch.no_grad()
     def _chunk_pass_state(self, image_sizes, padded_hw, level_hw, B, dev, sts):
         """Everything one pass of ``forward_chunked_device`` needs besides the image features, for elements e = chunk * B + image:
-        the image half of the geometry (computed once per image geometry, repeated per chunk), the text half and the BERT inputs
-        of the chunks, the vision queries zero-padded to the pass's largest count (the pad_sequence padding of
-        QuerySelector.forward, query_selector.py:112-116), and the per-element class tables.  Cached per (image geometry, chunk
-        group); the cache holds the passes of the current image geometry only."""
+        the image half of the geometry (computed once per image geometry, repeated per chunk) and the text half of
+        ``_chunk_text_state``.  Cached per (image geometry, chunk group); the cache holds the passes of the current image geometry
+        only.  Building it uploads nothing that waits for the stream, so a new geometry (the next scale of test-time
+        augmentation) does not stall the host."""
         ikey = self._image_key(image_sizes, padded_hw, level_hw)
         cache = self.__dict__.get("_chunk_pass_cache")
         if cache is None or cache["ikey"] != ikey:
             masks, poss = self._level_masks(image_sizes, padded_hw, level_hw, B, dev)
             img_geo = self.transformer.prepare_image(masks, poss)
             img_geo["levels"] = ops.get_levels(list(level_hw), dev)
-            img_geo["img_wh"] = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32, device=dev)
+            wh = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32)
+            img_geo["img_wh"] = ops.upload_async(wh, dev)
             cache = self._chunk_pass_cache = dict(ikey=ikey, img_geo=img_geo, passes={})
         gkey = tuple(st["key"] for st in sts)
         ps = cache["passes"].get(gkey)
         if ps is not None:
             return ps
         G = len(sts)
-
-        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...], element e = chunk * B + image
-            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
-
         img_geo = cache["img_geo"]
         ps = Transformer.repeat_image_geometry(img_geo, G)
         ps["levels"] = img_geo["levels"]
         ps["img_wh"] = img_geo["img_wh"].repeat(G, 1).contiguous()
+        ps.update(self._chunk_text_state(sts, B, dev))
+        if len(cache["passes"]) >= self.CHUNK_GROUP_CAPACITY:
+            cache["passes"].clear()
+        cache["passes"][gkey] = ps
+        return ps
+
+    @torch.no_grad()
+    def _chunk_text_state(self, sts, B, dev):
+        """The text half of a pass, a function of the chunk group and the batch size only: the text half of the geometry and the
+        BERT inputs of the chunks, the vision queries zero-padded to the group's largest count (the pad_sequence padding of
+        QuerySelector.forward, query_selector.py:112-116), and the per-element class tables.  Cached apart from the image
+        geometry, so every geometry's pass shares these tensors (the GCP index table is built once per vision mask tensor)."""
+        key = (tuple(st["key"] for st in sts), B)
+        cache = self.__dict__.setdefault("_chunk_text_cache", {})
+        ts = cache.get(key)
+        if ts is not None:
+            return ts
+        G = len(sts)
+
+        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...], element e = chunk * B + image
+            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
+
         token_mask = per_element([st["token_mask"] for st in sts])
         self_mask, position_ids = per_element([st["self_mask"] for st in sts]), per_element([st["position_ids"] for st in sts])
-        ps.update(self.transformer.prepare_text(token_mask, position_ids, self_mask))
-        ps["per_element_max"] = True   # each chunk's fusion scores are shifted by their own maximum (one chunk per reference forward)
-        ps["ids"], ps["bert_mask"], ps["position_ids"] = per_element([st["ids"] for st in sts]), self_mask.float().contiguous(), position_ids
-        ps["vision"] = ps["vmask"] = None
+        ts = dict(self.transformer.prepare_text(token_mask, position_ids, self_mask))
+        ts["per_element_max"] = True   # each chunk's fusion scores are shifted by their own maximum (one chunk per reference forward)
+        ts["ids"], ts["bert_mask"], ts["position_ids"] = per_element([st["ids"] for st in sts]), self_mask.float().contiguous(), position_ids
+        ts["vision"] = ts["vmask"] = None
         if sts[0]["vision"] is not None:
             Vmax = max(st["vision"].shape[0] for st in sts)
             vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
@@ -400,8 +419,8 @@ class GroundingDINO(nn.Module):
             for g, st in enumerate(sts):
                 vision[g, :st["vision"].shape[0]] = st["vision"]
                 vmask[g, :st["vmask"].shape[0]] = st["vmask"]
-            ps["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
-            ps["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
+            ts["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
+            ts["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
         Cmax = max(max(len(st["cols"]) for st in sts), 1)
         mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
         tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
@@ -410,12 +429,12 @@ class GroundingDINO(nn.Module):
             for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
                 tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
                 lab_h[g, j] = c
-        ps["tokmap"] = tok_h.to(dev).repeat_interleave(B, dim=0).contiguous()
-        ps["class_labels"] = lab_h.to(dev).repeat_interleave(B, dim=0).contiguous()
-        if len(cache["passes"]) >= self.CHUNK_GROUP_CAPACITY:
-            cache["passes"].clear()
-        cache["passes"][gkey] = ps
-        return ps
+        ts["tokmap"] = ops.upload_async(tok_h, dev).repeat_interleave(B, dim=0).contiguous()
+        ts["class_labels"] = ops.upload_async(lab_h, dev).repeat_interleave(B, dim=0).contiguous()
+        if len(cache) >= self.CHUNK_GROUP_CAPACITY:
+            cache.clear()
+        cache[key] = ts
+        return ts
 
     @torch.no_grad()
     def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):

@@ -568,10 +568,19 @@ def ml_nms(boxes, scores, labels, thresh):
     return keep[: int(num.item())]
 
 
+def upload_async(t, device):
+    """Small host tensor -> ``device`` without waiting for the stream: staged in pinned memory and copied asynchronously (a
+    copy from pageable memory synchronises the stream first).  Other devices get a plain copy."""
+    if torch.device(device).type != "cuda":
+        return t.to(device)
+    return t.pin_memory().to(device, non_blocking=True)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # Multi-scale / flip test-time augmentation: the cross-pass merge (csrc/bbox_aug.cu)
 # ----------------------------------------------------------------------------------------------------------------------
 BBOX_AUG_MAX_CAP = 1 << 17
+BBOX_AUG_BAD_COUNT = 1 << 30   # set in MergedBoxes.overflow by a packed pass whose count row is not an integer in [0, rows]
 
 
 def hflip_pad(images, out_hw):
@@ -612,7 +621,6 @@ def bbox_aug_collect(merged, cand_boxes, cand_scores, cand_labels, cand_totals, 
     (BoxList.transpose), drop boxes whose area is outside ``keep_range`` = (lo, hi), both bounds strict (remove_boxes), scale
     from ``pass_size`` to ``orig_size`` (both (width, height); BoxList.resize), in that order.  Candidate order is kept and
     the running count stays on the device."""
-    import numpy as np
     global launch_count
     _need_cuda(cand_boxes, cand_scores, cand_labels, cand_totals)
     B, S = cand_scores.shape
@@ -621,15 +629,41 @@ def bbox_aug_collect(merged, cand_boxes, cand_scores, cand_labels, cand_totals, 
             raise _lib.MqdetError("bbox_aug_collect: contiguous fp32 boxes / scores / labels and int32 totals required")
     if B != merged.B or tuple(cand_boxes.shape) != (B, S, 4):
         raise _lib.MqdetError(f"bbox_aug_collect: candidates {tuple(cand_boxes.shape)} do not match a merged buffer of {merged.B} images")
+    check(load().mqdet_bbox_aug_collect(_ptr(cand_boxes), _ptr(cand_scores), _ptr(cand_labels), _ptr(cand_totals), B, S,
+                                        *_aug_pass_args(pass_size, orig_size, flip, keep_range), _ptr(merged.boxes),
+                                        _ptr(merged.scores), _ptr(merged.labels), merged.cap, _ptr(merged.count),
+                                        _ptr(merged.overflow), _stream()), "bbox_aug_collect")
+    launch_count += 1
+    return merged
+
+
+def _aug_pass_args(pass_size, orig_size, flip, keep_range):
+    """(flip, pass_w, has_range, lo2, hi2, ratio_x, ratio_y) of a collect, rounded to fp32 as the reference's tensors are."""
+    import numpy as np
     rx, ry = float(orig_size[0]) / float(pass_size[0]), float(orig_size[1]) / float(pass_size[1])
     rx32, ry32 = float(np.float32(rx)), float(np.float32(ry))      # tensor * python_float multiplies by the fp32 ratio
     lo2 = hi2 = 0.0
     if keep_range is not None:
         lo2, hi2 = float(np.float32(keep_range[0] * keep_range[0])), float(np.float32(keep_range[1] * keep_range[1]))
-    check(load().mqdet_bbox_aug_collect(_ptr(cand_boxes), _ptr(cand_scores), _ptr(cand_labels), _ptr(cand_totals), B, S, int(bool(flip)),
-                                        float(pass_size[0]), int(keep_range is not None), lo2, hi2, rx32, ry32, _ptr(merged.boxes),
-                                        _ptr(merged.scores), _ptr(merged.labels), merged.cap, _ptr(merged.count),
-                                        _ptr(merged.overflow), _stream()), "bbox_aug_collect")
+    return int(bool(flip)), float(pass_size[0]), int(keep_range is not None), lo2, hi2, rx32, ry32
+
+
+def bbox_aug_collect_packed(merged, packed, pass_size, orig_size, *, flip=False, keep_range=None):
+    """``bbox_aug_collect`` for one pass's packed detector rows fp32 [B, M + 1, 6] (x1, y1, x2, y2, score, label; row M =
+    (count, ...)), the output of ``gdino_detections``: the same steps in the same order, rows kept in order.  The count is read on
+    the device; one that is not an integer in [0, M] reads no row and flags the image in ``merged.overflow``
+    (``BBOX_AUG_BAD_COUNT``)."""
+    global launch_count
+    _need_cuda(packed)
+    if packed.dtype != torch.float32 or not packed.is_contiguous() or packed.dim() != 3 or packed.shape[2] != 6 or packed.shape[1] < 2:
+        raise _lib.MqdetError(f"bbox_aug_collect_packed: contiguous fp32 [B, M + 1, 6] rows required (got {packed.dtype} "
+                              f"{tuple(packed.shape)})")
+    B, M = packed.shape[0], packed.shape[1] - 1
+    if B != merged.B:
+        raise _lib.MqdetError(f"bbox_aug_collect_packed: {B} images do not match a merged buffer of {merged.B} images")
+    check(load().mqdet_bbox_aug_collect_packed(_ptr(packed), B, M, *_aug_pass_args(pass_size, orig_size, flip, keep_range),
+                                               _ptr(merged.boxes), _ptr(merged.scores), _ptr(merged.labels), merged.cap,
+                                               _ptr(merged.count), _ptr(merged.overflow), _stream()), "bbox_aug_collect_packed")
     launch_count += 1
     return merged
 
