@@ -586,6 +586,13 @@ int mqdet_test_transform(const void* const* src, const int64_t* hw, const int32_
                          int64_t oh, int64_t ow, int64_t Hp, int64_t Wp, int bgr, int times255, const float* mean, const float* std,
                          float* out, uint8_t* resized, void* stream);
 
+/* ---- vision-only evaluation (VISION_QUERY.MASK_DURING_INFERENCE; generalized_vl_rcnn_new.py:397-407) (prompt_mask.cu) ----
+ *   mqdet_mask_prompt_tokens : token ids i64 [E][T] -> out i64 [E][T]: out[e][t] = mask_id when c = tok_cat[e][t] (i32, -1 = the
+ *                              token belongs to no category) lies in [0, C) and flags[e][c] (u8 [E][C]) is non-zero, else ids[e][t].
+ *                              out must not alias ids.  Nothing is read on the host; flags may be null when C == 0. */
+int mqdet_mask_prompt_tokens(const int64_t* ids, const int32_t* tok_cat, const uint8_t* flags, int64_t E, int64_t T, int64_t C,
+                             int64_t mask_id, int64_t* out, void* stream);
+
 /* ---- Box AP on the device (lvis_eval.cu): LVIS (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval, both protocols) and COCO
  *      (od_eval.py + pycocotools COCOeval, bbox).  Where the protocols differ the rule is an argument, never a protocol switch.
  *   mqdet_lvis_collect : packed f32 [G][B][M + 1][6] detector rows (row M = (count, ...)) -> pool slots base + (b * G + g) * M + r:

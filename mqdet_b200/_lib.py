@@ -184,6 +184,7 @@ SIGNATURES = {
     "mqdet_resize_coeffs": (c_int, [c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_test_transform": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_mask_prompt_tokens": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_lvis_collect":(c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
                                    c_void_p]),

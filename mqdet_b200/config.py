@@ -35,7 +35,8 @@ def mq_glip_t_cfg(**over):
                         AUGMENT_IMAGE_WITH_QUERY=False, TEXT_DROPOUT=0.4, NEW_MASK_TOKEN=False, QUERY_FUSION=False,
                         SHARE_KV=False, NUM_QUERY_PER_CLASS=5, SELECT_FPN_LEVEL=True, QUERY_BANK_PATH="",
                         LEARNABLE_BANK=False, ADD_VISION_LAYER=False, PURE_TEXT_RATE=0.0, RANDOM_KSHOT=False,
-                        EXPAND_RATIO=1.5, MAX_QUERY_NUMBER=5000, SIMILARITY_THRESHOLD=0.85),
+                        EXPAND_RATIO=1.5, MAX_QUERY_NUMBER=5000, SIMILARITY_THRESHOLD=0.85,
+                        MASK_DURING_INFERENCE=False),
         # multi-scale / flip test-time augmentation (engine/bbox_aug.py), the values of config/defaults.py:856-867
         TEST=NS(MDETR_STYLE_AGGREGATE_CLASS_NUM=-1, USE_MULTISCALE=False,
                 SCALES=(400, 500, 600, 640, 700, 900, 1000, 1100, 1200, 1300, 1400, 1800),

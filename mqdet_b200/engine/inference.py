@@ -34,6 +34,11 @@ class InferenceEngine:
         """model: GeneralizedVLRCNN_New (eval, on its CUDA device); captions / positive_map: the prompt of the run;
         batch_shape: (B, 3, H, W) of the padded batch tensor; image_sizes: [(h, w)] * B un-padded sizes;
         gather_every: steps whose packed results are exchanged by one all-gather (N > 1)."""
+        # vision-only evaluation: at TEXT_DROPOUT >= 1 the masked ids are part of the captured prompt state
+        self.mask_rate = model.text_mask_rate()
+        if 0 < self.mask_rate < 1:
+            raise NotImplementedError("VISION_QUERY.TEXT_DROPOUT < 1 with VISION_QUERY.MASK_DURING_INFERENCE: every forward draws new "
+                                      "token masks, which a replayed graph cannot do; use forward_device")
         self.model = model
         self.captions, self.positive_map = captions, positive_map
         self.dev = next(model.parameters()).device
@@ -142,6 +147,8 @@ class InferenceEngine:
         main.wait_event(self.res_done[k])   # the previous result of this slot has been gathered / copied out
         if self.use_graph:
             self.graphs[k].replay()
+            if self.mask_rate > 0:   # the draws of the eager forward, so that Python's random advances as in the reference
+                self.model.draw_text_masks(self.model._prompt["has"], self.mask_rate)
         else:
             self.outs[k] = self._forward(k)
         self._collect(k, to_host)

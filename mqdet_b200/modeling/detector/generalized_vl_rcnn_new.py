@@ -12,6 +12,7 @@ Parameter names follow the reference (``backbone.body.*``, ``backbone.fpn.*``, `
     offline; with an HF tokenizer attached (``self.tokenizer``) plain strings work as in the reference;
   * the eval-time ``assert B == 1`` (:354) is lifted: a batch shares one prompt (the training-branch tensor layout).
 """
+import random
 from collections import OrderedDict
 
 import torch
@@ -26,6 +27,8 @@ from ..language_backbone.bert_model_new import BertEncoder
 from ..poolers import Pooler
 from ..query_selector.query_selector import QuerySelector
 from ..rpn.vldyhead import VLDyHeadModule
+
+MASK_TOKEN_ID = 103   # [MASK] of the bert-base-uncased vocabulary (tokenizer.mask_token_id)
 
 
 def build_backbone(cfg):
@@ -160,6 +163,51 @@ class GeneralizedVLRCNN_New(nn.Module):
         pk = tuple((int(k), tuple(int(t) for t in (v if not isinstance(v, int) else [v]))) for k, v in sorted(positive_map.items()))
         return (ck, pk, int(B), int(bank_version))
 
+    def text_mask_rate(self):
+        """Vision-only evaluation (generalized_vl_rcnn_new.py:397-407): VISION_QUERY.TEXT_DROPOUT when MASK_DURING_INFERENCE
+        masks prompt tokens at inference, else 0.  Each forward draws one ``random.random()`` per category per image; the
+        tokens of a category whose draw is below the rate and that has vision queries become [MASK]."""
+        vq = self.cfg.VISION_QUERY
+        if not (vq.ENABLED and getattr(vq, "MASK_DURING_INFERENCE", False) and vq.TEXT_DROPOUT > 0):
+            return 0.0
+        if vq.PURE_TEXT_RATE != 0:
+            raise NotImplementedError("VISION_QUERY.MASK_DURING_INFERENCE needs VISION_QUERY.PURE_TEXT_RATE == 0 (the reference "
+                                      f"asserts it), got {vq.PURE_TEXT_RATE}")
+        if vq.NEW_MASK_TOKEN:
+            raise NotImplementedError("VISION_QUERY.NEW_MASK_TOKEN=True with VISION_QUERY.MASK_DURING_INFERENCE: the reference's "
+                                      "learned mask token branch is disabled; use the [MASK] token (NEW_MASK_TOKEN=False)")
+        if self.query_selector.query_bank is None:
+            raise MqdetError("VISION_QUERY.MASK_DURING_INFERENCE: vision-only evaluation needs a query bank")
+        return float(vq.TEXT_DROPOUT)
+
+    def _mask_tables(self, ids, all_map, has, rate):
+        """Per-prompt tables of the token masking: ``tok_cat`` int32 [E, T] (row of ``all_map`` each token belongs to, -1 for
+        none) and the per-image has-query lists; at rate >= 1 every draw is below the rate, so the masked ids are cached too."""
+        E, T = ids.shape
+        pos = all_map != 0
+        if pos.shape[1] != T:
+            raise MqdetError(f"MASK_DURING_INFERENCE: {T} token ids per prompt but MAX_QUERY_LEN = {pos.shape[1]}")
+        if (pos.sum(0) > 1).any():
+            raise MqdetError("MASK_DURING_INFERENCE: a token belongs to two categories of the positive map")
+        cat = torch.full((T,), -1, dtype=torch.int32)
+        rows, toks = pos.nonzero(as_tuple=True)
+        cat[toks] = rows.to(torch.int32)
+        tok_cat = ops.upload_async(cat[None].expand(E, -1).contiguous(), ids.device)
+        tab = dict(tok_cat=tok_cat, has=has, mask_rate=rate)
+        if rate >= 1.0:
+            tab["ids_masked"] = ops.mask_prompt_tokens(ids, tok_cat, ops.upload_async(torch.tensor(has, dtype=torch.uint8), ids.device),
+                                                       self.mask_token_id())
+        return tab
+
+    def mask_token_id(self):
+        return getattr(self.tokenizer, "mask_token_id", None) or MASK_TOKEN_ID
+
+    @staticmethod
+    def draw_text_masks(has, rate):
+        """:402-406 for the images of ``has`` (one has-query list per image) in order: one ``random.random()`` per category,
+        drawn for every category -> [len(has)][C] flags, 1 = mask the category's tokens."""
+        return [[int(random.random() < rate and h == 1) for h in row] for row in has]
+
     def max_out(self):
         """Rows of the fixed-shape per-image result: DETECTIONS_PER_IMG plus head-room for the reference's `>= kth score`
         ties (rpn/inference.py:757-767), rounded up to a multiple of 32 (100 -> 128, LVIS 300 -> 352)."""
@@ -197,7 +245,8 @@ class GeneralizedVLRCNN_New(nn.Module):
         st = self._prompt
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
         same_objects = st is not None and st["captions"] is captions and st["positive_map"] is positive_map
-        key = self._prompt_key(captions, positive_map, B, bank_version)
+        rate = self.text_mask_rate()
+        key = self._prompt_key(captions, positive_map, B, bank_version) + (rate,)
         if st is not None and st["key"] == key:
             if not same_objects:
                 st["captions"], st["positive_map"] = captions, positive_map
@@ -207,13 +256,29 @@ class GeneralizedVLRCNN_New(nn.Module):
         if ids.shape[0] == 1 and B > 1:
             ids, am = ids.expand(B, -1).contiguous(), am.expand(B, -1).contiguous()
         vision = vmask = None
+        self._prompt = dict(key=key, captions=captions, positive_map=positive_map, B=B, ids=ids, am=am, mask_rate=0.0)
         if self.query_selector is not None and self.query_selector.query_bank is not None:
             labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
-            vision, vmask, _ = self.query_selector([labels] * B, [all_map] * B, None)
+            vision, vmask, has = self.query_selector([labels] * B, [all_map] * B, None)
             vision, vmask = vision.float().contiguous(), vmask.float().contiguous()
-        self._prompt = dict(key=key, captions=captions, positive_map=positive_map, B=B, ids=ids, am=am, vision=vision,
-                            vmask=vmask)
+            if rate > 0:
+                self._prompt.update(self._mask_tables(ids, all_map, has, rate))
+        self._prompt.update(vision=vision, vmask=vmask)
         return self._prompt
+
+    def _prompt_ids(self, st):
+        """The token ids of one forward: the prompt's own, or those of vision-only evaluation.  At rate >= 1 the cached masked
+        ids; below, this forward's draws are uploaded (pinned, asynchronous) and masked on the device.  The draws advance
+        Python's ``random`` exactly as the reference's per-image forwards do, in both cases."""
+        rate = st["mask_rate"]
+        if rate == 0:
+            return st["ids"]
+        flags = self.draw_text_masks(st["has"], rate)
+        if rate >= 1.0:
+            return st["ids_masked"]
+        dev = st["ids"].device
+        flags = ops.upload_async(torch.tensor(flags, dtype=torch.uint8), dev)
+        return ops.mask_prompt_tokens(st["ids"], st["tok_cat"], flags, self.mask_token_id())
 
     @torch.no_grad()
     def forward_device(self, images, captions, positive_map, max_out=None):
@@ -228,6 +293,7 @@ class GeneralizedVLRCNN_New(nn.Module):
             raise MqdetError("GeneralizedVLRCNN_New: CUDA images required (no CPU fallback)")
         B = x.shape[0]
         st = self._prompt_state(captions, positive_map, B, x.device)
+        ids = self._prompt_ids(st)
         # The embeddings and the BERT layers before the first GCP block depend on the prompt only: they run on a second
         # stream next to the visual backbone (fork / join by events; capturable as a second graph branch).
         prefix = None
@@ -238,14 +304,14 @@ class GeneralizedVLRCNN_New(nn.Module):
             fork.record(main)
             with torch.cuda.stream(side):
                 side.wait_event(fork)
-                prefix = self.language_backbone.body.model.text_prefix(st["ids"], st["am"])
+                prefix = self.language_backbone.body.model.text_prefix(ids, st["am"])
                 join.record(side)
         feats = self.backbone.body.forward_flat(x)
         pyr16, levels = self.backbone.fpn.forward_flat([feats[i] for i in (1, 2, 3)])
         if prefix is not None:
             main.wait_event(join)
         pooled = ops.avgpool2_levels(pyr16, levels) if st["vision"] is not None else None  # flatten_fpn_features (:291-293)
-        lang = self.language_backbone.body({"input_ids": st["ids"], "attention_mask": st["am"], "text_prefix": prefix,
+        lang = self.language_backbone.body({"input_ids": ids, "attention_mask": st["am"], "text_prefix": prefix,
                                             "vision_inputs": {"vision": st["vision"], "images": pooled,
                                                               "vision_attention_mask": st["vmask"],
                                                               "batched_pos_category_map": None}})
@@ -258,25 +324,30 @@ class GeneralizedVLRCNN_New(nn.Module):
     # ---- many-category prompts: chunked evaluation (LVIS) --------------------------------------------------------------
     @torch.no_grad()
     def _chunk_state(self, captions, positive_map, dev):
-        """Per-chunk prompt state (token ids, selected vision queries + token mask, class columns in ascending label order),
-        cached by content like ``_prompt_state``."""
+        """Per-chunk prompt state (token ids, selected vision queries + token mask, class columns in ascending label order,
+        the token masking tables of vision-only evaluation), cached by content like ``_prompt_state``."""
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
-        key = self._prompt_key(captions, positive_map, 1, bank_version)
+        rate = self.text_mask_rate()
+        key = self._prompt_key(captions, positive_map, 1, bank_version) + (rate,)
         cache = self.__dict__.setdefault("_chunk_cache", {})
         st = cache.get(key)
         if st is not None:
             return st
         ids, am = self._tokenize(captions, dev)
+        ids, am = ids[:1], am[:1]
         vision = vmask = None
+        tab = dict(mask_rate=0.0)
         if self.query_selector is not None and self.query_selector.query_bank is not None:
             labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
-            vision, vmask, _ = self.query_selector([labels], [all_map], None)
+            vision, vmask, has = self.query_selector([labels], [all_map], None)
             vision, vmask = vision[0].float().contiguous(), vmask[0].float().contiguous()
+            if rate > 0:
+                tab = self._mask_tables(ids.contiguous(), all_map, has, rate)
         cols = sorted(int(k) for k in positive_map)
         toks = [([positive_map[c]] if isinstance(positive_map[c], int) else list(positive_map[c])) for c in cols]
         if len(cache) > 4096:
             cache.clear()
-        st = cache[key] = dict(ids=ids[:1], am=am[:1], vision=vision, vmask=vmask, cols=cols, toks=toks)
+        st = cache[key] = dict(ids=ids, am=am, vision=vision, vmask=vmask, cols=cols, toks=toks, **tab)
         return st
 
     @torch.no_grad()
@@ -304,11 +375,20 @@ class GeneralizedVLRCNN_New(nn.Module):
         max_out = self.max_out()
         packed = torch.empty((len(chunk_ids), B, max_out + 1, 6), dtype=torch.float32, device=dev)
         pooled = None
+        states = [self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in chunk_ids]
+        rate = states[0]["mask_rate"] if states else 0.0
+        if rate > 0:   # vision-only evaluation: the draws of the reference's forwards, images outer, chunks inner (inference.py:600-625)
+            flags = [[self.draw_text_masks(st["has"], rate)[0] for st in states] for _ in range(B)]
         for p0 in range(0, len(chunk_ids), chunks_per_pass):
-            group = chunk_ids[p0:p0 + chunks_per_pass]
-            G = len(group)
-            sts = [self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in group]
-            ids = torch.cat([st["ids"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
+            sts = states[p0:p0 + chunks_per_pass]
+            G = len(sts)
+            ids = torch.cat([st["ids_masked" if rate >= 1.0 else "ids"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
+            if 0 < rate < 1.0:
+                Cmax = max(len(st["has"][0]) for st in sts)
+                fl = torch.tensor([flags[b][p0 + g] + [0] * (Cmax - len(flags[b][p0 + g])) for g in range(G) for b in range(B)],
+                                  dtype=torch.uint8)
+                tok_cat = torch.cat([st["tok_cat"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
+                ids = ops.mask_prompt_tokens(ids, tok_cat, ops.upload_async(fl, dev), self.mask_token_id())
             am = torch.cat([st["am"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
             vision = vmask = None
             if sts[0]["vision"] is not None:

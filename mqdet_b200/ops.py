@@ -745,6 +745,31 @@ def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# Vision-only evaluation: [MASK] over the tokens of the categories drawn for masking (csrc/prompt_mask.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+def mask_prompt_tokens(ids, tok_cat, flags, mask_id, out=None):
+    """int64 token ids [E, T] -> a new int64 [E, T] (or ``out``): ``mask_id`` where the token's category ``tok_cat[e, t]``
+    (int32 [E, T], -1 = none) has ``flags[e, category]`` set (uint8 [E, C]), the id otherwise.  One launch, no host read."""
+    global launch_count
+    _need_cuda(ids, tok_cat, flags)
+    if ids.dtype != torch.int64 or ids.dim() != 2 or not ids.is_contiguous():
+        raise _lib.MqdetError("mask_prompt_tokens: contiguous int64 [E, T] token ids required")
+    E, T = ids.shape
+    if tok_cat.dtype != torch.int32 or tuple(tok_cat.shape) != (E, T) or not tok_cat.is_contiguous():
+        raise _lib.MqdetError(f"mask_prompt_tokens: contiguous int32 [{E}, {T}] category table required")
+    if flags.dtype != torch.uint8 or flags.dim() != 2 or flags.shape[0] != E or not flags.is_contiguous():
+        raise _lib.MqdetError(f"mask_prompt_tokens: contiguous uint8 [{E}, C] flags required")
+    if out is None:
+        out = torch.empty_like(ids)
+    elif out.dtype != torch.int64 or out.shape != ids.shape or not out.is_contiguous():
+        raise _lib.MqdetError(f"mask_prompt_tokens: out must be contiguous int64 [{E}, {T}]")
+    check(load().mqdet_mask_prompt_tokens(_ptr(ids), _ptr(tok_cat), _ptr(flags) if flags.numel() else None, E, T, flags.shape[1],
+                                          int(mask_id), _ptr(out), _stream()), "mask_prompt_tokens")
+    launch_count += 1
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # DyHead vision path
 # ----------------------------------------------------------------------------------------------------------------------
 class Levels:
