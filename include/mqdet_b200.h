@@ -339,10 +339,15 @@ int mqdet_avgpool2_levels(const void* x, const int32_t* level_hw, int64_t nlev, 
  * (torchvision roi_align, aligned = True, sampling_ratio 0 = adaptive) over the fp16 pyramid x [B][N][C] (levels concatenated).
  * rois [R][5] = (image index, x1, y1, x2, y2) fp32 in image pixels; scales HOST float [nlev] (POOLER_SCALES).
  * mean_only != 0: out [R][C] = mean over the pooled x pooled bins (query_feats.mean(dim=[-2,-1]), :263);
- * otherwise out [R][C][pooled][pooled] fp32.  level_out int32 [R] optional. */
+ * otherwise out [R][C][pooled][pooled] fp32.  level_out int32 [R] optional.  With R == 0 nothing is read or written. */
 int mqdet_roi_align_levels(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B, int64_t C,
                            const float* rois, int64_t R, int64_t pooled, int64_t sampling_ratio, int mean_only, float* out,
                            int32_t* level_out, void* stream);
+/* mqdet_roi_align_levels_counted: the same over rois [cap][5] of which the first *count (int32, device) are in use; the rows
+ * past the count are neither read nor written, so the count never crosses to the host. */
+int mqdet_roi_align_levels_counted(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B, int64_t C,
+                                   const float* rois, const int32_t* count, int64_t cap, int64_t pooled, int64_t sampling_ratio,
+                                   int mean_only, float* out, int32_t* level_out, void* stream);
 
 /* ---- GroundingDINO: multi-scale deformable attention forward (groundingdino_new/models/GroundingDINO/ms_deform_attn.py:93-133,
  * 285-331; supersedes groundingdino_new._C.ms_deform_attn_forward, csrc_groundingdino/vision.cpp:53-56) ---------------------------
@@ -592,6 +597,29 @@ int mqdet_test_transform(const void* const* src, const int64_t* hw, const int32_
  *                              out must not alias ids.  Nothing is read on the host; flags may be null when C == 0. */
 int mqdet_mask_prompt_tokens(const int64_t* ids, const int32_t* tok_cat, const uint8_t* flags, int64_t E, int64_t T, int64_t C,
                              int64_t mask_id, int64_t* out, void* stream);
+
+/* ---- test-time vision-query update (VISION_QUERY.NUM_TURNS; engine/inference.py:383-497) (query_bank.cu) -------------------
+ *   mqdet_query_candidates  : packed detector rows f32 [B][M + 1][6] = (x1, y1, x2, y2, score, label), row M = (count, ...), of
+ *                             images img_w x img_h -> rois f32 [cap][5] = (image index, x1, y1, x2, y2), labels i32 [cap] and
+ *                             *count (device): every row with score > score_thr, grown about its centre (dw = (w * expand_ratio -
+ *                             w) / 2, x1 - dw, x2 + dw; likewise in y), clamped to [0, img_w - 1] x [0, img_h - 1], kept when
+ *                             x2 > x1 and y2 > y1; image-then-row order; every step one rounded fp32 operation.  A count row that
+ *                             is not an integer in [0, M] reads no row of that image and adds 1 to *bad (i32, device; it
+ *                             accumulates over calls).  cap >= B * M.  One CTA.
+ *   mqdet_query_bank_norms  : row_norm f32 [L][cap] = ||bank[l][j]||_2 for j < bank_count[l] (a bank uploaded from the host).
+ *   mqdet_query_bank_update : bank f32 [L][cap][C] with bank_count i32 [L] rows in use and their row_norm; for the first *count
+ *                             features f32 [.][C] with labels i32 (device) in order, per label l in [0, L): skip the feature when
+ *                             bank_count[l] >= max_query, or when some row j of the bank has (row / max(||row||, 1e-12)) .
+ *                             (x / max(||x||, 1e-12)) > sim_thr (rows appended earlier by this call included); else append it.
+ *                             Labels outside [0, L) are ignored.  One CTA per label; the sums run in a fixed order, so a rerun is
+ *                             bit-identical.  max_query <= cap. */
+int mqdet_query_candidates(const float* packed, int64_t B, int64_t M, float score_thr, float expand_ratio, int64_t img_w, int64_t img_h,
+                           float* rois, int32_t* labels, int64_t cap, int32_t* count, int32_t* bad, void* stream);
+int mqdet_query_bank_norms(const float* bank, const int32_t* bank_count, int64_t L, int64_t cap, int64_t C, float* row_norm,
+                           void* stream);
+int mqdet_query_bank_update(const float* feats, const int32_t* labels, const int32_t* count, int64_t C, float* bank,
+                            int32_t* bank_count, float* row_norm, int64_t L, int64_t cap, int64_t max_query, float sim_thr,
+                            void* stream);
 
 /* ---- Box AP on the device (lvis_eval.cu): LVIS (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval, both protocols) and COCO
  *      (od_eval.py + pycocotools COCOeval, bbox).  Where the protocols differ the rule is an argument, never a protocol switch.

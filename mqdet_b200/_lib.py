@@ -107,6 +107,8 @@ SIGNATURES = {
                                         c_int64, c_void_p, c_void_p]),
     "mqdet_roi_align_levels": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64,
                                        c_int, c_void_p, c_void_p, c_void_p]),
+    "mqdet_roi_align_levels_counted": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_int64,
+                                               c_int64, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
     "mqdet_ms_deform_attn": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64,
                                      c_int64, c_int64, c_int64, c_void_p, c_int, c_void_p]),
     "mqdet_dense_cross_attn": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int64,
@@ -185,6 +187,11 @@ SIGNATURES = {
     "mqdet_test_transform": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mqdet_mask_prompt_tokens": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    "mqdet_query_candidates": (c_int, [c_void_p, c_int64, c_int64, c_float, c_float, c_int64, c_int64, c_void_p, c_void_p, c_int64,
+                                       c_void_p, c_void_p, c_void_p]),
+    "mqdet_query_bank_norms": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    "mqdet_query_bank_update": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
+                                        c_float, c_void_p]),
     "mqdet_lvis_collect":(c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
                                    c_void_p]),

@@ -36,7 +36,9 @@ def mq_glip_t_cfg(**over):
                         SHARE_KV=False, NUM_QUERY_PER_CLASS=5, SELECT_FPN_LEVEL=True, QUERY_BANK_PATH="",
                         LEARNABLE_BANK=False, ADD_VISION_LAYER=False, PURE_TEXT_RATE=0.0, RANDOM_KSHOT=False,
                         EXPAND_RATIO=1.5, MAX_QUERY_NUMBER=5000, SIMILARITY_THRESHOLD=0.85,
-                        MASK_DURING_INFERENCE=False),
+                        MASK_DURING_INFERENCE=False,
+                        # the test-time query update (engine/online_update.py), the values of config/defaults.py
+                        SCORE_THRESHOLD=0.6, MAX_TEST_QUERY_NUMBER=100, NUM_TURNS=1, OFFLINE_WITH_ONLINE=False),
         # multi-scale / flip test-time augmentation (engine/bbox_aug.py), the values of config/defaults.py:856-867
         TEST=NS(MDETR_STYLE_AGGREGATE_CLASS_NUM=-1, USE_MULTISCALE=False,
                 SCALES=(400, 500, 600, 640, 700, 900, 1000, 1100, 1200, 1300, 1400, 1800),

@@ -48,9 +48,9 @@ __device__ __forceinline__ float bilinear_nhwc(const __half* __restrict__ f, int
 // else out [R][C][P][P] (the Pooler.forward layout).  level_out (optional) receives the mapped level of every box.
 __global__ void roi_align_levels_kernel(const __half* __restrict__ x, RoiLevels lv, int N, int C, const float* __restrict__ rois,
                                         int R, int P, int sampling_ratio, int mean_only, float* __restrict__ out,
-                                        int* __restrict__ level_out) {
+                                        int* __restrict__ level_out, const int* __restrict__ n_dev) {
   const int r = blockIdx.x;
-  if (r >= R) return;
+  if (r >= R || (n_dev && r >= *n_dev)) return;
   const float* roi = rois + (long)r * 5;
   const int b = (int)roi[0];
   const float x1 = roi[1], y1 = roi[2], x2 = roi[3], y2 = roi[4];
@@ -93,10 +93,10 @@ __global__ void roi_align_levels_kernel(const __half* __restrict__ x, RoiLevels 
 
 using namespace mqdet;
 
-extern "C" int mqdet_roi_align_levels(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B,
-                                      int64_t C, const float* rois, int64_t R, int64_t pooled, int64_t sampling_ratio,
-                                      int mean_only, float* out, int32_t* level_out, void* stream) {
-  MQ_REQUIRE(x && level_hw && scales && out && (rois || R == 0), "roi_align_levels: null pointer");
+static int roi_align_launch(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B, int64_t C,
+                            const float* rois, int64_t R, const int32_t* n_dev, int64_t pooled, int64_t sampling_ratio, int mean_only,
+                            float* out, int32_t* level_out, void* stream) {
+  MQ_REQUIRE(x && level_hw && scales && ((rois && out) || R == 0), "roi_align_levels: null pointer");
   MQ_REQUIRE(nlev >= 1 && nlev <= MQDET_MAX_LEVELS && B >= 1 && C >= 1 && pooled >= 1 && pooled <= 32 && sampling_ratio >= 0,
              "roi_align_levels: bad arguments");
   if (R == 0) return MQDET_OK;
@@ -115,6 +115,20 @@ extern "C" int mqdet_roi_align_levels(const void* x, const int32_t* level_hw, in
   lv.k_min = -log2f(scales[0]);
   lv.k_max = -log2f(scales[nlev - 1]);
   roi_align_levels_kernel<<<(unsigned)R, 256, 0, (cudaStream_t)stream>>>((const __half*)x, lv, off, (int)C, rois, (int)R, (int)pooled,
-                                                                      (int)sampling_ratio, mean_only, out, level_out);
+                                                                      (int)sampling_ratio, mean_only, out, level_out, n_dev);
   return check_launch("roi_align_levels_kernel");
+}
+
+extern "C" int mqdet_roi_align_levels(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B,
+                                      int64_t C, const float* rois, int64_t R, int64_t pooled, int64_t sampling_ratio,
+                                      int mean_only, float* out, int32_t* level_out, void* stream) {
+  return roi_align_launch(x, level_hw, nlev, scales, B, C, rois, R, nullptr, pooled, sampling_ratio, mean_only, out, level_out, stream);
+}
+
+// The same over the first *count (device) of cap rows: blocks past the count return at once, so no host read is needed.
+extern "C" int mqdet_roi_align_levels_counted(const void* x, const int32_t* level_hw, int64_t nlev, const float* scales, int64_t B,
+                                              int64_t C, const float* rois, const int32_t* count, int64_t cap, int64_t pooled,
+                                              int64_t sampling_ratio, int mean_only, float* out, int32_t* level_out, void* stream) {
+  MQ_REQUIRE(count, "roi_align_levels_counted: null count");
+  return roi_align_launch(x, level_hw, nlev, scales, B, C, rois, cap, count, pooled, sampling_ratio, mean_only, out, level_out, stream);
 }

@@ -94,6 +94,11 @@ class GeneralizedVLRCNN_New(nn.Module):
         self.query_selector.load_query_bank(path)
         self.invalidate_prompt_cache()
 
+    def set_query_bank(self, bank):
+        """In-memory bank {label: tensor[n, scales, C]} (device tensors are used in place): ``load_query_bank`` without the file."""
+        self.query_selector.set_query_bank(bank)
+        self.invalidate_prompt_cache()
+
     def save_query_bank(self, query_images, path):
         """The on-disk bank format of tools/extract_vision_query.py: torch.save of {label: FloatTensor[n, n_scales, C]}."""
         torch.save({int(k): v.detach().cpu() for k, v in query_images.items()}, path)
@@ -316,7 +321,7 @@ class GeneralizedVLRCNN_New(nn.Module):
                                                               "vision_attention_mask": st["vmask"],
                                                               "batched_pos_category_map": None}})
         out = self.rpn.forward_flat(pyr16, levels, images.image_sizes, lang["hidden"], lang["masks"], positive_map, max_out)
-        out["image_sizes"] = images.image_sizes
+        out["image_sizes"], out["levels"] = images.image_sizes, levels
         out["pyramid16"], out["lang_hidden"] = pyr16, lang["hidden"]  # inputs of the fusion tower (parity tests read them)
         out["vision_query_gates"] = lang["vision_query_gates"]
         return out

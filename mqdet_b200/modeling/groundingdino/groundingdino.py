@@ -180,6 +180,11 @@ class GroundingDINO(nn.Module):
         self.query_selector.load_query_bank(query_path)
         self._prompt = None
 
+    def set_query_bank(self, bank):
+        """In-memory bank {label: tensor[n, scales, C]} (device tensors are used in place): ``load_query_bank`` without the file."""
+        self.query_selector.set_query_bank(bank)
+        self._prompt = None
+
     @torch.no_grad()
     def get_labels_and_maps_from_positive_map(self, positive_map, dtype=torch.float):
         """groundingdino.py:436-445."""
@@ -482,7 +487,8 @@ class GroundingDINO(nn.Module):
             logits, boxes = self._last_layer_heads(tr, ps["valid_ratios"], ps["text_token_mask"])
             det = ops.gdino_detections(logits, boxes, ps["tokmap"], ps["img_wh"], self.box_threshold, class_labels=ps["class_labels"])
             packed[p0:p0 + G] = det.view(G, B, nq + 1, 6)
-        return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "srcs": src32}
+        return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "srcs": src32, "pyramid16": src16,
+                "levels": ops.get_levels(sizes, dev)}
 
     def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
         """-> list[BoxList] (mode xyxy, fields labels / scores): per image, the per-chunk detections concatenated in chunk order

@@ -6,6 +6,7 @@ row to each query, pads over the batch and binarises the mask.
 """
 import os
 import random
+from collections import defaultdict
 
 import numpy as np
 import torch
@@ -35,8 +36,12 @@ class QuerySelector(nn.Module):
         self.bank_version += 1
 
     def set_query_bank(self, bank):
-        """In-memory bank {label: tensor[n, scales, C]} (tests / synthetic benchmarks; no file on disk)."""
-        self.query_bank = {k: v.to(self.device) for k, v in bank.items()}
+        """In-memory bank {label: tensor[n, scales, C]} (no file on disk).  A ``defaultdict(list)`` stays one, as ``torch.load`` of
+        the reference's saved banks keeps it: a label without exemplars reads as ``[]``."""
+        q = defaultdict(list) if isinstance(bank, defaultdict) else {}
+        for k, v in bank.items():
+            q[k] = v.to(self.device) if torch.is_tensor(v) else v
+        self.query_bank = q
         self.bank_version += 1
 
     def _pick(self, label):

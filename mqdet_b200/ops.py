@@ -770,6 +770,119 @@ def mask_prompt_tokens(ids, tok_cat, flags, mask_id, out=None):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# The test-time vision-query update: candidates, the counted pooling, the bank update (csrc/query_bank.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+class QueryBank:
+    """Device-resident vision-query bank with one pooled scale per query: rows fp32 [L, cap, C] (row j of label l), count int32
+    [L] (rows in use), norm fp32 [L, cap] (the L2 norm of every row in use).  Labels index the first axis directly."""
+
+    def __init__(self, L, cap, C, device):
+        if L < 1 or cap < 1 or C < 1:
+            raise _lib.MqdetError(f"QueryBank: bad sizes L={L} cap={cap} C={C}")
+        self.L, self.cap, self.C = int(L), int(cap), int(C)
+        self.rows = torch.zeros((L, cap, C), dtype=torch.float32, device=device)
+        self.count = torch.zeros((L,), dtype=torch.int32, device=device)
+        self.norm = torch.zeros((L, cap), dtype=torch.float32, device=device)
+
+    @classmethod
+    def from_dict(cls, bank, L, min_cap, C, device):
+        """{label: tensor [n, 1, C]} (the reference's format; missing labels and ``[]`` entries are empty) -> a bank whose capacity
+        per label is max(min_cap, the most rows any label brings).  Uploaded without waiting for the stream."""
+        global launch_count
+        items = {int(k): v for k, v in (bank or {}).items() if torch.is_tensor(v) and v.shape[0] > 0}
+        for k, v in items.items():
+            if v.dim() != 3 or v.shape[1] != 1 or v.shape[2] != C:
+                raise _lib.MqdetError(f"QueryBank: label {k} has rows {tuple(v.shape)}; [n, 1, {C}] required (one pooled scale)")
+            if not 0 <= k < L:
+                raise _lib.MqdetError(f"QueryBank: label {k} outside [0, {L})")
+        cap = max([int(min_cap)] + [v.shape[0] for v in items.values()])
+        qb = cls(L, cap, C, device)
+        if items:
+            rows = torch.zeros((L, cap, C), dtype=torch.float32)
+            cnt = torch.zeros((L,), dtype=torch.int32)
+            for k, v in items.items():
+                rows[k, :v.shape[0]] = v[:, 0].detach().to("cpu", torch.float32)
+                cnt[k] = v.shape[0]
+            qb.rows.copy_(upload_async(rows, device))
+            qb.count.copy_(upload_async(cnt, device))
+            check(load().mqdet_query_bank_norms(_ptr(qb.rows), _ptr(qb.count), L, cap, C, _ptr(qb.norm), _stream()), "query_bank_norms")
+            launch_count += 1
+        return qb
+
+    def as_dict(self, count_host):
+        """The reference's format {label: [n, 1, C]} as views of the device rows (rows below a label's count never change), given
+        the counts read on the host: a ``defaultdict(list)``, so that a label without rows reads as ``[]``."""
+        from collections import defaultdict
+        out = defaultdict(list)
+        for k, n in enumerate(count_host.tolist()):
+            if n > 0:
+                out[k] = self.rows[k, :n, None, :]
+        return out
+
+
+def query_candidates(packed, img_wh, score_thr, expand_ratio, bad):
+    """Packed detector rows fp32 [B, M + 1, 6] of images of one size ``img_wh`` = (w, h) -> (rois fp32 [B * M, 5], labels int32
+    [B * M], count int32 [1]): the rows with score > ``score_thr``, grown by ``expand_ratio`` about their centre, clipped to the image,
+    the empty ones removed, in image-then-row order; only the first ``count`` rows are written.  A count row that is not an integer in
+    [0, M] adds 1 to ``bad`` (int32 [1], device).  Nothing is read on the host."""
+    global launch_count
+    _need_cuda(packed, bad)
+    if packed.dtype != torch.float32 or not packed.is_contiguous() or packed.dim() != 3 or packed.shape[2] != 6 or packed.shape[1] < 2:
+        raise _lib.MqdetError(f"query_candidates: contiguous fp32 [B, M + 1, 6] rows required (got {packed.dtype} {tuple(packed.shape)})")
+    if bad.dtype != torch.int32 or bad.numel() != 1:
+        raise _lib.MqdetError("query_candidates: bad must be an int32 counter [1]")
+    B, M = packed.shape[0], packed.shape[1] - 1
+    dev = packed.device
+    rois = torch.empty((B * M, 5), dtype=torch.float32, device=dev)
+    labels = torch.empty((B * M,), dtype=torch.int32, device=dev)
+    count = torch.empty((1,), dtype=torch.int32, device=dev)
+    check(load().mqdet_query_candidates(_ptr(packed), B, M, float(score_thr), float(expand_ratio), int(img_wh[0]), int(img_wh[1]),
+                                        _ptr(rois), _ptr(labels), B * M, _ptr(count), _ptr(bad), _stream()), "query_candidates")
+    launch_count += 1
+    return rois, labels, count
+
+
+def roi_align_levels_counted(pyr16, levels, scales, rois, count, pooled=7, sampling_ratio=0):
+    """``roi_align_levels(mean_only=True)`` over the first ``count`` (int32 [1], device) of the rows of ``rois`` [cap, 5] -> fp32
+    [cap, C]; the rows past the count are left unwritten."""
+    import numpy as np
+    global launch_count
+    _need_cuda(pyr16, rois, count)
+    if rois.dtype != torch.float32 or not rois.is_contiguous() or rois.dim() != 2 or rois.shape[1] != 5:
+        raise _lib.MqdetError("roi_align_levels_counted: contiguous fp32 rois [cap, 5] required")
+    if pyr16.dtype != torch.float16 or not pyr16.is_contiguous() or count.dtype != torch.int32:
+        raise _lib.MqdetError("roi_align_levels_counted: contiguous fp16 pyramid and int32 count required")
+    B, N, C = pyr16.shape
+    cap = rois.shape[0]
+    out = torch.empty((cap, C), dtype=torch.float32, device=pyr16.device)
+    sc = np.asarray(scales, dtype=np.float32)
+    check(load().mqdet_roi_align_levels_counted(_ptr(pyr16), levels.hw_ptr, levels.n, sc.ctypes.data_as(ctypes.c_void_p), B, C,
+                                                _ptr(rois), _ptr(count), cap, int(pooled), int(sampling_ratio), 1, _ptr(out), None,
+                                                _stream()), "roi_align_levels_counted")
+    launch_count += 1
+    return out
+
+
+def query_bank_update(bank, feats, labels, count, max_query, sim_thr):
+    """Append the first ``count`` (int32 [1], device) pooled features fp32 [cap, C] with labels int32 [cap] to ``bank`` (a
+    ``QueryBank``) in order, as extract_query(exclude_similar=True) does: a feature is skipped when its label has ``max_query``
+    rows, or when its normalised dot product with some row of that label exceeds ``sim_thr``.  One launch, no host read."""
+    global launch_count
+    _need_cuda(feats, labels, count)
+    if feats.dtype != torch.float32 or not feats.is_contiguous() or feats.dim() != 2 or feats.shape[1] != bank.C:
+        raise _lib.MqdetError(f"query_bank_update: contiguous fp32 features [cap, {bank.C}] required")
+    if labels.dtype != torch.int32 or labels.numel() != feats.shape[0] or count.dtype != torch.int32:
+        raise _lib.MqdetError("query_bank_update: int32 labels (one per feature) and int32 count required")
+    if not 0 <= int(max_query) <= bank.cap:
+        raise _lib.MqdetError(f"query_bank_update: max_query {max_query} outside [0, {bank.cap}]")
+    check(load().mqdet_query_bank_update(_ptr(feats), _ptr(labels), _ptr(count), bank.C, _ptr(bank.rows), _ptr(bank.count),
+                                         _ptr(bank.norm), bank.L, bank.cap, int(max_query), float(sim_thr), _stream()),
+          "query_bank_update")
+    launch_count += 1
+    return bank
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # DyHead vision path
 # ----------------------------------------------------------------------------------------------------------------------
 class Levels:
