@@ -283,13 +283,15 @@ int mqdet_dyrelu_apply(const void* mid, const float* coef, const int32_t* level_
  * (ties by ascending (location, class)) -> BoxCoder.decode against the generated anchor -> clip -> sqrt(rank).
  * Outputs (row stride out_stride >= nlev*topk per image): per-level blocks out_* at [l*topk, ...), level_counts
  * [B][nlev]; dense concatenation cat_* (level 0 first) with totals[B].  out_key (optional) = level<<40|loc<<12|cls.
- * cand_ws: mqdet_atss_workspace_bytes(...) bytes. */
+ * img_wh f32 [n_sizes][2] (HOST): (w, h) of the images; element e clips its boxes to [0, w - 1] x [0, h - 1] of size e % n_sizes
+ * (n_sizes = 1: one size; = B: one per element; = images of a chunked pass, e = chunk * images + image).  B % n_sizes == 0,
+ * n_sizes <= 256.  cand_ws: mqdet_atss_workspace_bytes(...) bytes. */
 int64_t mqdet_atss_workspace_bytes(const int32_t* level_hw, int64_t nlev, int64_t C, int64_t B);
 int mqdet_atss_candidates(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
                           int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride, int64_t C,
                           int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev, const float* strides,
                           const float* base_anchors, const float* reg_scales, int64_t B, float pre_nms_thresh, int64_t topk,
-                          int64_t out_stride, float img_w, float img_h, void* cand_ws, int32_t* level_counts,
+                          int64_t out_stride, const float* img_wh, int64_t n_sizes, void* cand_ws, int32_t* level_counts,
                           float* out_boxes, float* out_scores, float* out_labels, int64_t* out_key, float* cat_boxes,
                           float* cat_scores, float* cat_labels, int32_t* totals, void* stream);
 
@@ -584,12 +586,19 @@ int mqdet_nms_by_class(const float* boxes, const float* scores, const int32_t* l
  *                               (1 << 21 + sum value * weight) >> 22 clipped to [0, 255] (uint8 intermediate); then per pixel
  *                               v / 255 (ToTensor); bgr != 0: output channel c reads input channel 2 - c; times255 != 0: v * 255;
  *                               (v - mean[c]) / std[c]; every step one rounded fp32 operation.  Pixels outside oh x ow are 0.
- *                               resized (optional) u8 [B][oh][ow][3]: the resized image.  Hp, Wp, h, w < 65536. */
+ *                               resized (optional) u8 [B][oh][ow][3]: the resized image.  Hp, Wp, h, w < 65536.
+ *   mqdet_test_transform_sizes: the same with a size per image: out_hw (HOST, i64 [B][2]) = (oh_i, ow_i) <= (Hp, Wp), the xtab / ytab
+ *                               of image i built for (w_i, ow_i) / (h_i, oh_i); image i is zero beyond its (oh_i, ow_i).  resized
+ *                               (optional) holds the resized images back to back, image i as u8 [oh_i][ow_i][3].  mqdet_test_transform
+ *                               is this call with one (oh, ow) for every image. */
 int64_t mqdet_resize_coeffs_ksize(int64_t n_in, int64_t n_out);
 int mqdet_resize_coeffs(int64_t n_in, int64_t n_out, int32_t* table, void* stream);
 int mqdet_test_transform(const void* const* src, const int64_t* hw, const int32_t* const* xtab, const int32_t* const* ytab, int64_t B,
                          int64_t oh, int64_t ow, int64_t Hp, int64_t Wp, int bgr, int times255, const float* mean, const float* std,
                          float* out, uint8_t* resized, void* stream);
+int mqdet_test_transform_sizes(const void* const* src, const int64_t* hw, const int64_t* out_hw, const int32_t* const* xtab,
+                               const int32_t* const* ytab, int64_t B, int64_t Hp, int64_t Wp, int bgr, int times255, const float* mean,
+                               const float* std, float* out, uint8_t* resized, void* stream);
 
 /* ---- vision-only evaluation (VISION_QUERY.MASK_DURING_INFERENCE; generalized_vl_rcnn_new.py:397-407) (prompt_mask.cu) ----
  *   mqdet_mask_prompt_tokens : token ids i64 [E][T] -> out i64 [E][T]: out[e][t] = mask_id when c = tok_cat[e][t] (i32, -1 = the
@@ -600,7 +609,8 @@ int mqdet_mask_prompt_tokens(const int64_t* ids, const int32_t* tok_cat, const u
 
 /* ---- test-time vision-query update (VISION_QUERY.NUM_TURNS; engine/inference.py:383-497) (query_bank.cu) -------------------
  *   mqdet_query_candidates  : packed detector rows f32 [B][M + 1][6] = (x1, y1, x2, y2, score, label), row M = (count, ...), of
- *                             images img_w x img_h -> rois f32 [cap][5] = (image index, x1, y1, x2, y2), labels i32 [cap] and
+ *                             images of img_wh (HOST, i64 [n_sizes][2] = (img_w, img_h); n_sizes = 1: one size for all, = B <= 256:
+ *                             one per image) -> rois f32 [cap][5] = (image index, x1, y1, x2, y2), labels i32 [cap] and
  *                             *count (device): every row with score > score_thr, grown about its centre (dw = (w * expand_ratio -
  *                             w) / 2, x1 - dw, x2 + dw; likewise in y), clamped to [0, img_w - 1] x [0, img_h - 1], kept when
  *                             x2 > x1 and y2 > y1; image-then-row order; every step one rounded fp32 operation.  A count row that
@@ -613,8 +623,8 @@ int mqdet_mask_prompt_tokens(const int64_t* ids, const int32_t* tok_cat, const u
  *                             (x / max(||x||, 1e-12)) > sim_thr (rows appended earlier by this call included); else append it.
  *                             Labels outside [0, L) are ignored.  One CTA per label; the sums run in a fixed order, so a rerun is
  *                             bit-identical.  max_query <= cap. */
-int mqdet_query_candidates(const float* packed, int64_t B, int64_t M, float score_thr, float expand_ratio, int64_t img_w, int64_t img_h,
-                           float* rois, int32_t* labels, int64_t cap, int32_t* count, int32_t* bad, void* stream);
+int mqdet_query_candidates(const float* packed, int64_t B, int64_t M, float score_thr, float expand_ratio, const int64_t* img_wh,
+                           int64_t n_sizes, float* rois, int32_t* labels, int64_t cap, int32_t* count, int32_t* bad, void* stream);
 int mqdet_query_bank_norms(const float* bank, const int32_t* bank_count, int64_t L, int64_t cap, int64_t C, float* row_norm,
                            void* stream);
 int mqdet_query_bank_update(const float* feats, const int32_t* labels, const int32_t* count, int64_t C, float* bank,

@@ -97,7 +97,7 @@ SIGNATURES = {
     "mqdet_atss_workspace_bytes": (c_int64, [c_void_p, c_int64, c_int64, c_int64]),
     "mqdet_atss_candidates": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                       c_void_p, c_int64,
-                                      c_void_p, c_void_p, c_void_p, c_int64, c_float, c_int64, c_int64, c_float, c_float,
+                                      c_void_p, c_void_p, c_void_p, c_int64, c_float, c_int64, c_int64, c_void_p, c_int64,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p]),
     "mqdet_ml_nms_batched_workspace_bytes": (c_int64, [c_int64, c_int64]),
@@ -186,8 +186,10 @@ SIGNATURES = {
     "mqdet_resize_coeffs": (c_int, [c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_test_transform": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mqdet_test_transform_sizes": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_int,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mqdet_mask_prompt_tokens": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
-    "mqdet_query_candidates": (c_int, [c_void_p, c_int64, c_int64, c_float, c_float, c_int64, c_int64, c_void_p, c_void_p, c_int64,
+    "mqdet_query_candidates": (c_int, [c_void_p, c_int64, c_int64, c_float, c_float, c_void_p, c_int64, c_void_p, c_void_p, c_int64,
                                        c_void_p, c_void_p, c_void_p]),
     "mqdet_query_bank_norms": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "mqdet_query_bank_update": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,

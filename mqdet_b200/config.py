@@ -44,11 +44,14 @@ def mq_glip_t_cfg(**over):
                 SCALES=(400, 500, 600, 640, 700, 900, 1000, 1100, 1200, 1300, 1400, 1800),
                 RANGES=((96, 10000), (96, 10000), (64, 10000), (64, 10000), (64, 10000), (0, 10000), (0, 10000), (0, 256),
                         (0, 256), (0, 192), (0, 192), (0, 96)),
-                MAX_SIZE=2500, FLIP=True, SPECIAL_NMS="none", TH=0.6, PRE_NMS_TOP_N=1000, NUM_CLASSES=81, SELECT_CLASSES=()),
+                MAX_SIZE=2500, FLIP=True, SPECIAL_NMS="none", TH=0.6, PRE_NMS_TOP_N=1000, NUM_CLASSES=81, SELECT_CLASSES=(),
+                # images per test batch (the yaml's TEST block); read only by engine.batches.reference_test_batches
+                IMS_PER_BATCH=8),
         # the test transform (engine/transforms.py): config/defaults.py:68-78 and the yaml's INPUT block
         INPUT=NS(PIXEL_MEAN=[103.530, 116.280, 123.675], PIXEL_STD=[57.375, 57.120, 58.395], MIN_SIZE_TEST=800, MAX_SIZE_TEST=1333,
                  FORMAT="", TO_BGR255=True),
-        DATALOADER=NS(SIZE_DIVISIBILITY=32),
+        # ASPECT_RATIO_GROUPING: config/defaults.py:214; read only by engine.batches.reference_test_batches
+        DATALOADER=NS(SIZE_DIVISIBILITY=32, ASPECT_RATIO_GROUPING=True),
     )
     for k, v in over.items():
         node = cfg

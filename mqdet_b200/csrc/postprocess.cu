@@ -19,6 +19,15 @@ namespace mqdet {
 constexpr int PP_MAX_T = 256;
 constexpr int PP_TOPK_MAX = 1024;
 
+constexpr int PP_MAX_SIZES = 256;   // clip sizes per launch: one per image of a padded batch (kernel-parameter table)
+
+// Clip bound of every batch element: element e clips to [0, wh[e % n][0] - 1] x [0, wh[e % n][1] - 1].  n = 1: one size for all;
+// n = B images: the elements of a chunked pass (e = chunk * B + image) repeat the image sizes chunk by chunk.
+struct PPSizes {
+  int n;
+  float wh[PP_MAX_SIZES][2];
+};
+
 struct PPLevels {
   int n;
   int H[MQDET_MAX_LEVELS], W[MQDET_MAX_LEVELS], off[MQDET_MAX_LEVELS];
@@ -92,7 +101,7 @@ __global__ void __launch_bounds__(1024) atss_select_decode_kernel(const unsigned
                                                                   const int* counts,
                                                                   const float* __restrict__ reg_ctr, PPLevels lv, int C,
                                                                   const int* __restrict__ class_labels, long labels_img_stride,
-                                                                  int topk, float img_w, float img_h, long cand_per_img,
+                                                                  int topk, const __grid_constant__ PPSizes sz, long cand_per_img,
                                                                   int out_per_img, float* __restrict__ out_boxes,
                                                                   float* __restrict__ out_scores,
                                                                   float* __restrict__ out_labels,
@@ -183,7 +192,8 @@ __global__ void __launch_bounds__(1024) atss_select_decode_kernel(const unsigned
     const float ax1 = sx + lv.base[l][0], ay1 = sy + lv.base[l][1], ax2 = sx + lv.base[l][2], ay2 = sy + lv.base[l][3];
     const DecodedBox d = box_decode(r[0] * sc, r[1] * sc, r[2] * sc, r[3] * sc, ax1, ay1, ax2, ay2);
     float x1 = d.x1, y1 = d.y1, x2 = d.x2, y2 = d.y2;
-    // clip_to_image(remove_empty=False), TO_REMOVE = 1
+    // clip_to_image(remove_empty=False), TO_REMOVE = 1, to this element's own image size
+    const float img_w = sz.wh[b % sz.n][0], img_h = sz.wh[b % sz.n][1];
     x1 = fminf(fmaxf(x1, 0.f), img_w - 1.f);
     y1 = fminf(fmaxf(y1, 0.f), img_h - 1.f);
     x2 = fminf(fmaxf(x2, 0.f), img_w - 1.f);
@@ -300,7 +310,7 @@ extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const
                                      int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride,
                                      int64_t C, int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev,
                                      const float* strides, const float* base_anchors, const float* reg_scales, int64_t B,
-                                     float pre_nms_thresh, int64_t topk, int64_t out_stride, float img_w, float img_h,
+                                     float pre_nms_thresh, int64_t topk, int64_t out_stride, const float* img_wh, int64_t n_sizes,
                                      void* cand_ws,
                                      int32_t* level_counts, float* out_boxes, float* out_scores, float* out_labels,
                                      int64_t* out_key, float* cat_boxes, float* cat_scores, float* cat_labels,
@@ -310,6 +320,15 @@ extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const
              "atss_candidates: null pointer");
   MQ_REQUIRE(T > 0 && T <= PP_MAX_T, "atss_candidates: T=%ld exceeds %d", (long)T, PP_MAX_T);
   MQ_REQUIRE(topk > 0 && topk <= PP_TOPK_MAX, "atss_candidates: topk=%ld exceeds %d", (long)topk, PP_TOPK_MAX);
+  MQ_REQUIRE(img_wh && n_sizes >= 1 && n_sizes <= PP_MAX_SIZES && B % n_sizes == 0,
+             "atss_candidates: %ld image sizes for %ld batch elements (one, or one per image of the pass, at most %d)",
+             (long)n_sizes, (long)B, PP_MAX_SIZES);
+  PPSizes sz{};
+  sz.n = (int)n_sizes;
+  for (int64_t i = 0; i < n_sizes; ++i) {
+    sz.wh[i][0] = img_wh[2 * i];
+    sz.wh[i][1] = img_wh[2 * i + 1];
+  }
   PPLevels lv;
   const int N = fill_pp_levels(&lv, level_hw, nlev, strides, base_anchors, reg_scales, C);
   MQ_REQUIRE(N > 0, "atss_candidates: bad level table");
@@ -333,7 +352,7 @@ extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const
   // level_counts is rewritten in place with min(count, topk) by the select kernel (it reads the raw count first)
   atss_select_decode_kernel<<<(unsigned)(B * nlev), 1024, 0, st>>>((const unsigned long long*)cand_ws, level_counts, reg_ctr,
                                                                   lv, (int)C, class_labels, (long)labels_img_stride, (int)topk,
-                                                                  img_w, img_h, cand_per_img,
+                                                                  sz, cand_per_img,
                                                                   out_per_img, out_boxes, out_scores, out_labels,
                                                                   (long long*)out_key, level_counts);
   rc = check_launch("atss_select_decode_kernel");

@@ -1,8 +1,8 @@
 // mqdet_b200 — the test-time vision-query update (VISION_QUERY.NUM_TURNS; maskrcnn_benchmark/engine/inference.py:383-497).
 //
 //   query_candidates_kernel : packed detector rows [B][M + 1][6] -> the boxes extract_query pools: score > SCORE_THRESHOLD, grown
-//                             by EXPAND_RATIO about their centre (expand_bbox, generalized_vl_rcnn_new.py:32-49), clipped to the
-//                             image and the empty ones removed (BoxList.clip_to_image(remove_empty=True)); image-then-row order
+//                             by EXPAND_RATIO about their centre (expand_bbox, generalized_vl_rcnn_new.py:32-49), clipped to its
+//                             own image's size and the empty ones removed (BoxList.clip_to_image(remove_empty=True)); image-then-row order
 //   query_bank_update_kernel: one CTA per label walks the pooled features of its label in arrival order and applies the bank
 //                             bookkeeping of extract_query (:268-288, exclude_similar=True): the per-label cap, the cosine test
 //                             against every row already in the bank (rows appended earlier in the same call included), the append
@@ -13,9 +13,18 @@
 
 namespace mqdet {
 
+constexpr int QC_MAX_IMAGES = 256;   // clip sizes per launch (kernel-parameter table)
+
+// Clip bound of image b: [0, hi[n == 1 ? 0 : b][0]] x [0, hi[..][1]] = (w - 1, h - 1) of one size for all, or of each image.
+struct QCSizes {
+  int n;
+  float hi[QC_MAX_IMAGES][2];
+};
+
 // One CTA; images in order, per 1024 rows a ballot scan gives every kept box its slot (row order kept).
 __global__ void __launch_bounds__(1024) query_candidates_kernel(const float* __restrict__ packed, int B, int M, float score_thr,
-                                                                float ratio, float hi_x, float hi_y, float* __restrict__ rois,
+                                                                float ratio, const __grid_constant__ QCSizes sz,
+                                                                float* __restrict__ rois,
                                                                 int* __restrict__ labels, int* __restrict__ count,
                                                                 int* __restrict__ bad) {
   __shared__ int warp_tot[32];
@@ -25,6 +34,7 @@ __global__ void __launch_bounds__(1024) query_candidates_kernel(const float* __r
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int b = 0; b < B; ++b) {
     const float* rows = packed + (long)b * (M + 1) * 6;
+    const float hi_x = sz.hi[sz.n == 1 ? 0 : b][0], hi_y = sz.hi[sz.n == 1 ? 0 : b][1];
     const float cnt = rows[(long)M * 6];
     const bool ok = cnt >= 0.f && cnt <= (float)M && cnt == floorf(cnt);
     const int n = ok ? (int)cnt : 0;
@@ -148,15 +158,25 @@ __global__ void __launch_bounds__(QB_THREADS) query_bank_norms_kernel(const floa
 
 using namespace mqdet;
 
-extern "C" int mqdet_query_candidates(const float* packed, int64_t B, int64_t M, float score_thr, float expand_ratio, int64_t img_w,
-                                      int64_t img_h, float* rois, int32_t* labels, int64_t cap, int32_t* count, int32_t* bad,
-                                      void* stream) {
-  MQ_REQUIRE(packed && rois && labels && count && bad, "query_candidates: null pointer");
-  MQ_REQUIRE(B > 0 && M > 0 && M <= (1 << 24) && img_w > 0 && img_h > 0 && img_w < (1 << 24) && img_h < (1 << 24),
-             "query_candidates: bad sizes B=%ld M=%ld image %ldx%ld", (long)B, (long)M, (long)img_w, (long)img_h);
+extern "C" int mqdet_query_candidates(const float* packed, int64_t B, int64_t M, float score_thr, float expand_ratio,
+                                      const int64_t* img_wh, int64_t n_sizes, float* rois, int32_t* labels, int64_t cap, int32_t* count,
+                                      int32_t* bad, void* stream) {
+  MQ_REQUIRE(packed && img_wh && rois && labels && count && bad, "query_candidates: null pointer");
+  MQ_REQUIRE(B > 0 && M > 0 && M <= (1 << 24) && (n_sizes == 1 || n_sizes == B) && n_sizes <= QC_MAX_IMAGES,
+             "query_candidates: bad sizes B=%ld M=%ld with %ld image sizes (one, or one per image, at most %d)", (long)B, (long)M,
+             (long)n_sizes, QC_MAX_IMAGES);
+  QCSizes sz{};
+  sz.n = (int)n_sizes;
+  for (int64_t i = 0; i < n_sizes; ++i) {
+    const int64_t w = img_wh[2 * i], h = img_wh[2 * i + 1];
+    MQ_REQUIRE(w > 0 && h > 0 && w < (1 << 24) && h < (1 << 24), "query_candidates: bad sizes B=%ld M=%ld image %ld %ldx%ld", (long)B,
+               (long)M, (long)i, (long)w, (long)h);
+    sz.hi[i][0] = (float)(w - 1);
+    sz.hi[i][1] = (float)(h - 1);
+  }
   MQ_REQUIRE(cap >= B * M && B * M < (1L << 30), "query_candidates: capacity %ld below B * M = %ld", (long)cap, (long)(B * M));
-  query_candidates_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(packed, (int)B, (int)M, score_thr, expand_ratio, (float)(img_w - 1),
-                                                                (float)(img_h - 1), rois, labels, count, bad);
+  query_candidates_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(packed, (int)B, (int)M, score_thr, expand_ratio, sz, rois, labels,
+                                                                count, bad);
   return check_launch("query_candidates_kernel");
 }
 

@@ -6,15 +6,19 @@
 //
 //   resize_coeffs_kernel  : one (in, out) length pair -> per output index: first input index, tap count and the 22-bit
 //                           fixed-point weights of Pillow's bilinear resampler (fp64, every operation rounded)
-//   test_transform_kernel : B uint8 HWC RGB images (any source sizes) -> one fp32 [B, 3, Hp, Wp] batch of a common (oh, ow).
+//   test_transform_kernel : B uint8 HWC RGB images (any source sizes) -> one fp32 [B, 3, Hp, Wp] batch, image i resized to its
+//                           own (oh_i, ow_i) and zero beyond it (to_image_list of a batch of differently sized images).
 //                           One CTA per (128 output columns, 16 output rows, image): it walks the intermediate rows its 16
 //                           output rows read, computes each one's horizontal pass for its columns (uint8, clipped, held in
 //                           registers only) and adds it into the vertical accumulators of the rows whose window holds it.
+//                           A CTA whose tile lies wholly outside its image's (oh_i, ow_i) only writes zeros.
 //
 // Pillow's resampler is integer arithmetic behind fp64 coefficients, so it is reproduced bit for bit: the coefficient kernel
 // uses __d*_rn intrinsics (no contraction; Pillow's x86-64 build has no FMA), the passes are the same int32 sums.  A pass whose
 // length does not change is the identity through its coefficients (weights {2^22, 0}), so it is not special-cased.
 // ToTensor / Normalize are fp32 operations one at a time (__f*_rn), as torch computes them on the CPU.
+#include <vector>
+
 #include "common.cuh"
 #include "../../include/mqdet_b200.h"
 
@@ -29,7 +33,9 @@ struct TTImage {
   const uint8_t* src;                     // [h][w][3]
   const int32_t* xtab;                    // [ow][2 + kx]: first column, taps, weights
   const int32_t* ytab;                    // [oh][2 + ky]
+  uint8_t* resized;                       // [oh][ow][3] or null
   int h, w, kx, ky;
+  int oh, ow;                             // the resized size; the rest of the padded [Hp, Wp] plane is zero
 };
 
 struct TTBatch {
@@ -82,16 +88,21 @@ __device__ __forceinline__ int tt_clip8(int acc) {
   return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
-__global__ void __launch_bounds__(TT_TX) test_transform_kernel(const __grid_constant__ TTBatch batch, int oh, int ow, int Hp, int Wp,
-                                                               int bgr, int times255, float m0, float m1, float m2, float s0,
-                                                               float s1, float s2, float* __restrict__ out,
-                                                               uint8_t* __restrict__ resized) {
+__global__ void __launch_bounds__(TT_TX, 4) test_transform_kernel(const __grid_constant__ TTBatch batch, int Hp, int Wp, int bgr,
+                                                               int times255, float m0, float m1, float m2, float s0, float s1,
+                                                               float s2, float* __restrict__ out) {
   const TTImage& im = batch.im[blockIdx.z];
+  const int oh = im.oh, ow = im.ow;
   const int x = blockIdx.x * TT_TX + threadIdx.x;
   const int y0 = blockIdx.y * TT_TY;
   const long plane = (long)Hp * Wp;
   float* o = out + (long)blockIdx.z * 3 * plane;
   if (x >= Wp) return;
+  if (blockIdx.x * TT_TX >= ow || y0 >= oh) {   // the tile is padding only
+    for (int r = 0; r < TT_TY && y0 + r < Hp; ++r)
+      for (int c = 0; c < 3; ++c) o[c * plane + (long)(y0 + r) * Wp + x] = 0.f;
+    return;
+  }
 
   int acc[TT_TY][3];
   int ylo[TT_TY], yn[TT_TY];
@@ -148,8 +159,8 @@ __global__ void __launch_bounds__(TT_TX) test_transform_kernel(const __grid_cons
     int u[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) u[c] = tt_clip8(acc[r][c]);
-    if (in && resized) {
-      uint8_t* d = resized + (((long)blockIdx.z * oh + y) * ow + x) * 3;
+    if (in && im.resized) {
+      uint8_t* d = im.resized + ((long)y * ow + x) * 3;
       d[0] = (uint8_t)u[0];
       d[1] = (uint8_t)u[1];
       d[2] = (uint8_t)u[2];
@@ -184,6 +195,41 @@ extern "C" int mqdet_resize_coeffs(int64_t n_in, int64_t n_out, int32_t* table, 
   return check_launch("resize_coeffs_kernel");
 }
 
+extern "C" int mqdet_test_transform_sizes(const void* const* src, const int64_t* hw, const int64_t* out_hw, const int32_t* const* xtab,
+                                          const int32_t* const* ytab, int64_t B, int64_t Hp, int64_t Wp, int bgr, int times255,
+                                          const float* mean, const float* stdv, float* out, uint8_t* resized, void* stream) {
+  MQ_REQUIRE(src && hw && out_hw && xtab && ytab && mean && stdv && out, "test_transform: null pointer");
+  MQ_REQUIRE(B > 0 && Hp > 0 && Wp > 0 && Hp < (1 << 16) && Wp < (1 << 16), "test_transform: bad sizes B=%ld padded to %ldx%ld",
+             (long)B, (long)Hp, (long)Wp);
+  for (int64_t b = 0; b < B; ++b) {
+    MQ_REQUIRE(src[b] && xtab[b] && ytab[b], "test_transform: null pointer for image %ld", (long)b);
+    MQ_REQUIRE(hw[2 * b] > 0 && hw[2 * b + 1] > 0 && hw[2 * b] < (1 << 16) && hw[2 * b + 1] < (1 << 16),
+               "test_transform: image %ld has bad size %ldx%ld", (long)b, (long)hw[2 * b], (long)hw[2 * b + 1]);
+    MQ_REQUIRE(out_hw[2 * b] > 0 && out_hw[2 * b + 1] > 0 && out_hw[2 * b] <= Hp && out_hw[2 * b + 1] <= Wp,
+               "test_transform: image %ld has bad size %ldx%ld padded to %ldx%ld", (long)b, (long)out_hw[2 * b], (long)out_hw[2 * b + 1],
+               (long)Hp, (long)Wp);
+  }
+  for (int c = 0; c < 3; ++c) MQ_REQUIRE(stdv[c] != 0.f, "test_transform: std[%d] is zero", c);
+  long roff = 0;   // resized images back to back
+  for (int64_t b0 = 0; b0 < B; b0 += TT_MAX_B) {
+    const int nb = (int)(B - b0 < TT_MAX_B ? B - b0 : TT_MAX_B);
+    TTBatch batch;
+    memset(&batch, 0, sizeof(batch));
+    for (int i = 0; i < nb; ++i) {
+      const int64_t b = b0 + i, oh = out_hw[2 * b], ow = out_hw[2 * b + 1];
+      batch.im[i] = TTImage{(const uint8_t*)src[b], xtab[b], ytab[b], resized ? resized + roff : nullptr, (int)hw[2 * b],
+                            (int)hw[2 * b + 1], tt_ksize(hw[2 * b + 1], ow), tt_ksize(hw[2 * b], oh), (int)oh, (int)ow};
+      roff += oh * ow * 3;
+    }
+    const dim3 grid(cdiv(Wp, TT_TX), cdiv(Hp, TT_TY), nb);
+    test_transform_kernel<<<grid, TT_TX, 0, (cudaStream_t)stream>>>(batch, (int)Hp, (int)Wp, bgr, times255, mean[0], mean[1], mean[2],
+                                                                    stdv[0], stdv[1], stdv[2], out + b0 * 3 * Hp * Wp);
+    const int rc = check_launch("test_transform_kernel");
+    if (rc != MQDET_OK) return rc;
+  }
+  return MQDET_OK;
+}
+
 extern "C" int mqdet_test_transform(const void* const* src, const int64_t* hw, const int32_t* const* xtab,
                                     const int32_t* const* ytab, int64_t B, int64_t oh, int64_t ow, int64_t Hp, int64_t Wp, int bgr,
                                     int times255, const float* mean, const float* stdv, float* out, uint8_t* resized,
@@ -191,27 +237,10 @@ extern "C" int mqdet_test_transform(const void* const* src, const int64_t* hw, c
   MQ_REQUIRE(src && hw && xtab && ytab && mean && stdv && out, "test_transform: null pointer");
   MQ_REQUIRE(B > 0 && oh > 0 && ow > 0 && Hp >= oh && Wp >= ow && Hp < (1 << 16) && Wp < (1 << 16),
              "test_transform: bad sizes B=%ld %ldx%ld padded to %ldx%ld", (long)B, (long)oh, (long)ow, (long)Hp, (long)Wp);
+  std::vector<int64_t> out_hw(2 * B);
   for (int64_t b = 0; b < B; ++b) {
-    MQ_REQUIRE(src[b] && xtab[b] && ytab[b], "test_transform: null pointer for image %ld", (long)b);
-    MQ_REQUIRE(hw[2 * b] > 0 && hw[2 * b + 1] > 0 && hw[2 * b] < (1 << 16) && hw[2 * b + 1] < (1 << 16),
-               "test_transform: image %ld has bad size %ldx%ld", (long)b, (long)hw[2 * b], (long)hw[2 * b + 1]);
+    out_hw[2 * b] = oh;
+    out_hw[2 * b + 1] = ow;
   }
-  for (int c = 0; c < 3; ++c) MQ_REQUIRE(stdv[c] != 0.f, "test_transform: std[%d] is zero", c);
-  for (int64_t b0 = 0; b0 < B; b0 += TT_MAX_B) {
-    const int nb = (int)(B - b0 < TT_MAX_B ? B - b0 : TT_MAX_B);
-    TTBatch batch;
-    memset(&batch, 0, sizeof(batch));
-    for (int i = 0; i < nb; ++i) {
-      const int64_t b = b0 + i;
-      batch.im[i] = TTImage{(const uint8_t*)src[b], xtab[b], ytab[b], (int)hw[2 * b], (int)hw[2 * b + 1],
-                            tt_ksize(hw[2 * b + 1], ow), tt_ksize(hw[2 * b], oh)};
-    }
-    const dim3 grid(cdiv(Wp, TT_TX), cdiv(Hp, TT_TY), nb);
-    test_transform_kernel<<<grid, TT_TX, 0, (cudaStream_t)stream>>>(
-        batch, (int)oh, (int)ow, (int)Hp, (int)Wp, bgr, times255, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2],
-        out + b0 * 3 * Hp * Wp, resized ? resized + b0 * oh * ow * 3 : nullptr);
-    const int rc = check_launch("test_transform_kernel");
-    if (rc != MQDET_OK) return rc;
-  }
-  return MQDET_OK;
+  return mqdet_test_transform_sizes(src, hw, out_hw.data(), xtab, ytab, B, Hp, Wp, bgr, times255, mean, stdv, out, resized, stream);
 }

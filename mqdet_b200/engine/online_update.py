@@ -13,6 +13,9 @@ copy (the row counts) ends it.  The exception is the detector's prompt state (se
 the bank: the first batch after a bank is installed rebuilds it on the host, and so does a batch whose size differs from the one
 before (the prompt state and the GCP index table are cached for one batch size).  The bank only depends on the order of the images, so batches of consecutive images of one size give
 what the reference's one-image loop gives.
+Batches may also be padded batches of differently sized images, as the reference's test loader forms them (``make_batches(...,
+orig_hw=...)``): each image's boxes are clipped to its own size, and the bank is the one the reference's loop builds over the same
+batches (its batched forward sees the zero padding too).
 
 Quirk kept from the reference: ``online_update`` installs the bank of turn t - 1 at the start of turn t and the evaluation that follows
 does not reload it, so the evaluation uses the bank as it was after turn NUM_TURNS - 1 (with one turn, the bank the model had before).
@@ -45,11 +48,22 @@ def check_config(cfg):
                                   "reads no detections (IndexError)")
 
 
-def make_batches(images, max_batch, size_divisible=32):
+def make_batches(images, max_batch, size_divisible=32, orig_hw=None, aspect_grouping=True):
     """Consecutive images (fp32 [3, h, w] device tensors, normalised) -> ImageLists of at most ``max_batch`` images of one size, in
-    order; a new batch starts when the size changes."""
+    order; a new batch starts when the size changes.
+
+    With ``orig_hw`` (the images' original (height, width), in dataset order) the batches are instead those of the reference's test
+    loader, ``engine.batches.reference_test_batches(orig_hw, max_batch, aspect_grouping)``: each is padded to its largest image,
+    rounded up to ``size_divisible``, as the reference's ``BatchCollator`` pads it."""
     if max_batch < 1:
         raise ValueError(f"max_batch must be >= 1, got {max_batch}")
+    if orig_hw is not None:
+        from .batches import reference_test_batches
+        images = list(images)
+        if len(orig_hw) != len(images):
+            raise ValueError(f"orig_hw has {len(orig_hw)} sizes for {len(images)} images")
+        return [to_image_list([images[i] for i in idx], size_divisible)
+                for idx in reference_test_batches(orig_hw, max_batch, aspect_grouping)]
     out, cur = [], []
     for im in images:
         if cur and (len(cur) == max_batch or tuple(cur[0].shape[-2:]) != tuple(im.shape[-2:])):
@@ -67,8 +81,9 @@ def _is_gdino(model):
 
 
 def _detect(model, images, captions, positive_map):
-    """One forward -> (packed rows [B, M + 1, 6], fp16 pyramid [B, N, C], levels, (w, h)).  MQ-GroundingDINO runs the chunked path
-    with the prompt as its only chunk: it takes the fusion softmax maximum per image, as the reference's one-image forward does."""
+    """One forward -> (packed rows [B, M + 1, 6], fp16 pyramid [B, N, C], levels, (w, h) of the batch, or [(w_b, h_b)] per image for a
+    padded batch of differently sized images).  MQ-GroundingDINO runs the chunked path with the prompt as its only chunk: it takes the
+    fusion softmax maximum per image, as the reference's one-image forward does."""
     if _is_gdino(model):
         out = model.forward_chunked_device(images, [captions], [positive_map])
         packed = out["det_packed"][0]
@@ -78,7 +93,7 @@ def _detect(model, images, captions, positive_map):
     sizes = out["image_sizes"]
     h, w = sizes[0]
     if any(tuple(s) != (h, w) for s in sizes):
-        raise MqdetError("online_update: every batch holds images of one size (see make_batches)")
+        return packed, out["pyramid16"], out["levels"], [(int(w), int(h)) for h, w in sizes]
     return packed, out["pyramid16"], out["levels"], (int(w), int(h))
 
 
@@ -99,8 +114,8 @@ def update_turn(model, batches, captions, positive_map, bank, cfg, bad):
 
 @torch.no_grad()
 def online_update(model, batches, captions, positive_map, cfg, bank=None):
-    """Run ``VISION_QUERY.NUM_TURNS`` turns of the test-time update over ``batches`` (ImageLists of consecutive images of one size, in
-    dataset order; see ``make_batches``) with one prompt (``captions``, ``positive_map``: the detection prompt of the dataset).
+    """Run ``VISION_QUERY.NUM_TURNS`` turns of the test-time update over ``batches`` (ImageLists in dataset order: of consecutive
+    images of one size, or padded batches of differently sized images as the reference's test loader forms them; see ``make_batches``) with one prompt (``captions``, ``positive_map``: the detection prompt of the dataset).
 
     ``bank``: the starting bank {label: [n, 1, C]}; by default ``torch.load(VISION_QUERY.QUERY_BANK_PATH)`` when that file exists,
     else empty.  Returns {"banks": the bank after every turn, "eval_bank": the bank the evaluation that follows uses (the model's

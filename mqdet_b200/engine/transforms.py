@@ -109,20 +109,28 @@ class TestTransform:
     def target_size(self, h, w):
         return get_size((w, h), self.size, self.max_size)
 
-    def __call__(self, images, device, pad=True, want_resized=False):
-        """images: uint8 HWC RGB numpy arrays or tensors (host or ``device``) -> (ImageList, orig_sizes [(w, h)]).  All images
-        must resize to one size (the batches of ``forward_device`` share one).  ``pad=False`` leaves the batch at the resized
-        size; ``want_resized`` adds the resized uint8 images [B, oh, ow, 3] as a third result."""
+    def __call__(self, images, device, pad=True, want_resized=False, mixed_sizes=False):
+        """images: uint8 HWC RGB numpy arrays or tensors (host or ``device``) -> (ImageList, orig_sizes [(w, h)]).  By default all
+        images must resize to one size, so that a batch holds no padding beyond SIZE_DIVISIBILITY and ``want_resized`` has one
+        shape.  ``pad=False`` leaves the batch at the resized size; ``want_resized`` adds the resized uint8 images [B, oh, ow, 3]
+        as a third result.
+
+        ``mixed_sizes=True`` takes images that resize to different sizes, as the reference's test loader batches them: each is
+        resized to its own target size and the batch is zero-padded to the largest, rounded up to SIZE_DIVISIBILITY (its
+        ``to_image_list``); ``image_sizes`` holds every image's own target size.  ``want_resized`` is then refused."""
         if len(images) == 0:
             raise MqdetError("TestTransform: no images")
         device = _cuda_device(device)
         dev_images = upload(images, device)
         sizes = [tuple(im.shape[:2]) for im in dev_images]
-        targets = {self.target_size(h, w) for h, w in sizes}
-        if len(targets) != 1:
+        per_image = [self.target_size(h, w) for h, w in sizes]
+        targets = set(per_image)
+        if len(targets) != 1 and not mixed_sizes:
             raise MqdetError(f"TestTransform: the images resize to different sizes {sorted(targets)}; batch images of one target "
-                             "size together")
-        oh, ow = targets.pop()
+                             "size together, or pass mixed_sizes=True for one padded batch")
+        if mixed_sizes and want_resized:
+            raise MqdetError("TestTransform: want_resized needs one target size; it is not available with mixed_sizes=True")
+        oh, ow = max(h for h, _ in per_image), max(w for _, w in per_image)
         div = self.div if pad else 0
         Hp, Wp = (-(-oh // div) * div, -(-ow // div) * div) if div > 0 else (oh, ow)
         tables = {}
@@ -132,10 +140,15 @@ class TestTransform:
                 tables[(n_in, n_out)] = ops.resize_coeffs(n_in, n_out, device)
             return tables[(n_in, n_out)]
 
-        res = ops.test_transform(dev_images, [table(w, ow) for _, w in sizes], [table(h, oh) for h, _ in sizes], (oh, ow), (Hp, Wp),
-                                 self.mean, self.std, bgr=self.bgr, times255=self.times255, want_resized=want_resized)
+        if mixed_sizes:
+            res = ops.test_transform(dev_images, [table(w, t[1]) for (_, w), t in zip(sizes, per_image)],
+                                     [table(h, t[0]) for (h, _), t in zip(sizes, per_image)], per_image, (Hp, Wp), self.mean, self.std,
+                                     bgr=self.bgr, times255=self.times255)
+        else:
+            res = ops.test_transform(dev_images, [table(w, ow) for _, w in sizes], [table(h, oh) for h, _ in sizes], (oh, ow),
+                                     (Hp, Wp), self.mean, self.std, bgr=self.bgr, times255=self.times255, want_resized=want_resized)
         batch, resized = res if want_resized else (res, None)
-        il = ImageList(batch, [(oh, ow)] * len(sizes))
+        il = ImageList(batch, list(per_image))
         orig = [(w, h) for h, w in sizes]
         return (il, orig, resized) if want_resized else (il, orig)
 
@@ -145,10 +158,11 @@ def model_device(model):
 
 
 @torch.no_grad()
-def predict(model, images_u8, captions, positive_map):
+def predict(model, images_u8, captions, positive_map, mixed_sizes=False):
     """Decoded uint8 RGB images -> list[BoxList] in original-image coordinates, for MQ-GLIP and MQ-GroundingDINO: the test
     transform on the device, the detector's forward, and BoxList.resize back to each image's size (as the reference's
-    evaluators map the results)."""
-    il, orig = TestTransform(model.cfg)(images_u8, model_device(model))
+    evaluators map the results).  ``mixed_sizes=True``: images of different target sizes form one padded batch (see
+    ``TestTransform``)."""
+    il, orig = TestTransform(model.cfg)(images_u8, model_device(model), mixed_sizes=mixed_sizes)
     res = model(il, captions=captions, positive_map=positive_map)
     return [bl.resize(size) for bl, size in zip(res, orig)]

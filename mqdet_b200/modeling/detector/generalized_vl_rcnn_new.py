@@ -422,7 +422,7 @@ class GeneralizedVLRCNN_New(nn.Module):
                                                                   "images": pooled.repeat(G, 1, 1) if vision is not None else None,
                                                                   "vision_attention_mask": vmask,
                                                                   "batched_pos_category_map": None}})
-            out = self.rpn.forward_flat(pyr16.repeat(G, 1, 1), levels, list(images.image_sizes) * G, lang["hidden"], lang["masks"],
+            out = self.rpn.forward_flat(pyr16.repeat(G, 1, 1), levels, images.image_sizes, lang["hidden"], lang["masks"],
                                         None, max_out, tokmap=tokmap, class_labels=labels)
             packed[p0:p0 + G] = out["det_packed"].view(G, B, max_out + 1, 6)
         return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "pyramid16": pyr16}

@@ -377,6 +377,8 @@ class VLDyHeadModule(nn.Module):
     def forward_flat(self, pyr16, levels, image_sizes, lang_hidden, lang_masks, positive_map, max_out=None, tokmap=None,
                      class_labels=None):
         """pyr16 [B,N,256] fp16 -> device-resident detections: dict(det [B,max_out,6], num [B], ...).
+        ``image_sizes``: the (h, w) of every element, or of the B images when the elements are chunks of them (e = chunk * B + image);
+        each element's boxes are clipped to its own image, as the reference's post-processor clips each BoxList.
         ``tokmap`` int32 [B,C,max_tok] (+ ``class_labels`` int32 [B,C]): explicit per-element positive maps (batched prompt
         chunks) instead of the one ``positive_map`` dict shared by the batch."""
         cfg = self.cfg
@@ -389,10 +391,10 @@ class VLDyHeadModule(nn.Module):
                 self._tokmap = (pkey, ops.make_tokmap(positive_map, cfg.MODEL.DYHEAD.NUM_CLASSES - 1, pyr16.device))
             tokmap = self._tokmap[1]
         ih, iw = image_sizes[0]
-        if any(tuple(s) != (ih, iw) for s in image_sizes):
-            raise NotImplementedError("forward_flat batches images of one size; use forward() per size group")
+        if any(tuple(s) != (ih, iw) for s in image_sizes):   # a padded batch: each element clips to its own image size
+            ih, iw = [float(h) for h, _ in image_sizes], [float(w) for _, w in image_sizes]
         out = ops.atss_postprocess(r["dot_product_logits"], r["reg_ctr"], tokmap, levels, cfg.MODEL.RPN.ANCHOR_STRIDE,
-                                   cfg.MODEL.RPN.ANCHOR_SIZES, self._reg_scales()[:levels.n], float(iw), float(ih),
+                                   cfg.MODEL.RPN.ANCHOR_SIZES, self._reg_scales()[:levels.n], iw, ih,
                                    pre_nms_thresh=cfg.MODEL.ATSS.INFERENCE_TH, pre_nms_top_n=cfg.MODEL.ATSS.PRE_NMS_TOP_N,
                                    nms_thresh=cfg.MODEL.ATSS.NMS_TH, max_det=cfg.MODEL.ATSS.DETECTIONS_PER_IMG,
                                    max_out=max_out, class_labels=class_labels)

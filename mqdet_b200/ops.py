@@ -714,14 +714,19 @@ def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False
     """uint8 [h_i, w_i, 3] CUDA images (RGB) -> fp32 [B, 3, Hp, Wp]: each image resized to ``out_hw`` = (oh, ow) with
     ``xtabs[i]`` = resize_coeffs(w_i, ow) and ``ytabs[i]`` = resize_coeffs(h_i, oh), then / 255, channels reversed (``bgr``),
     x 255 (``times255``), (x - mean) / std, zero beyond (oh, ow) up to ``pad_hw``.  With ``want_resized`` also returns the
-    resized uint8 images [B, oh, ow, 3]."""
+    resized uint8 images [B, oh, ow, 3].  ``out_hw`` may also be B per-image sizes [(oh_i, ow_i)] (a padded batch of differently
+    sized images, the tables built for each image's own size); ``want_resized`` then needs them all equal."""
     global launch_count
     B = len(images)
     if B == 0 or len(xtabs) != B or len(ytabs) != B:
         raise _lib.MqdetError("test_transform: one x and one y coefficient table per image required")
     _need_cuda(*images, *xtabs, *ytabs)
-    (oh, ow), (Hp, Wp) = (int(v) for v in out_hw), (int(v) for v in pad_hw)
-    for im, xt, yt in zip(images, xtabs, ytabs):
+    per_image = isinstance(out_hw[0], (tuple, list))
+    sizes = [(int(h), int(w)) for h, w in out_hw] if per_image else [(int(out_hw[0]), int(out_hw[1]))] * B
+    if len(sizes) != B:
+        raise _lib.MqdetError(f"test_transform: {len(sizes)} output sizes for {B} images")
+    Hp, Wp = (int(v) for v in pad_hw)
+    for im, xt, yt, (oh, ow) in zip(images, xtabs, ytabs, sizes):
         if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or not im.is_contiguous():
             raise _lib.MqdetError(f"test_transform: contiguous uint8 [h, w, 3] images required (got {im.dtype} {tuple(im.shape)})")
         h, w = im.shape[:2]
@@ -729,8 +734,11 @@ def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False
             K = int(load().mqdet_resize_coeffs_ksize(n_in, n_out))
             if t.dtype != torch.int32 or not t.is_contiguous() or tuple(t.shape) != (n_out, 2 + K):
                 raise _lib.MqdetError(f"test_transform: the coefficient table of {n_in} -> {n_out} must be int32 [{n_out}, {2 + K}]")
+    if want_resized and len(set(sizes)) != 1:
+        raise _lib.MqdetError("test_transform: want_resized needs one output size for every image")
     dev = images[0].device
     out = torch.empty((B, 3, Hp, Wp), dtype=torch.float32, device=dev)
+    oh, ow = sizes[0]
     resized = torch.empty((B, oh, ow, 3), dtype=torch.uint8, device=dev) if want_resized else None
     src = (ctypes.c_void_p * B)(*[im.data_ptr() for im in images])
     hw = (ctypes.c_int64 * (2 * B))(*[int(v) for im in images for v in im.shape[:2]])
@@ -738,8 +746,13 @@ def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False
     yp = (ctypes.c_void_p * B)(*[t.data_ptr() for t in ytabs])
     m = (ctypes.c_float * 3)(*[float(v) for v in mean])
     s = (ctypes.c_float * 3)(*[float(v) for v in std])
-    check(load().mqdet_test_transform(src, hw, xp, yp, B, oh, ow, Hp, Wp, int(bool(bgr)), int(bool(times255)), m, s, _ptr(out),
-                                      _ptr(resized), _stream()), "test_transform")
+    if per_image:
+        ohw = (ctypes.c_int64 * (2 * B))(*[v for p in sizes for v in p])
+        check(load().mqdet_test_transform_sizes(src, hw, ohw, xp, yp, B, Hp, Wp, int(bool(bgr)), int(bool(times255)), m, s, _ptr(out),
+                                                _ptr(resized), _stream()), "test_transform")
+    else:
+        check(load().mqdet_test_transform(src, hw, xp, yp, B, oh, ow, Hp, Wp, int(bool(bgr)), int(bool(times255)), m, s, _ptr(out),
+                                          _ptr(resized), _stream()), "test_transform")
     launch_count += -(-B // 64)
     return (out, resized) if want_resized else out
 
@@ -821,7 +834,8 @@ class QueryBank:
 
 
 def query_candidates(packed, img_wh, score_thr, expand_ratio, bad):
-    """Packed detector rows fp32 [B, M + 1, 6] of images of one size ``img_wh`` = (w, h) -> (rois fp32 [B * M, 5], labels int32
+    """Packed detector rows fp32 [B, M + 1, 6] of images of one size ``img_wh`` = (w, h), or of B sizes ``img_wh`` = [(w_b, h_b)]
+    (a padded batch of differently sized images; each image's boxes are clipped to its own size) -> (rois fp32 [B * M, 5], labels int32
     [B * M], count int32 [1]): the rows with score > ``score_thr``, grown by ``expand_ratio`` about their centre, clipped to the image,
     the empty ones removed, in image-then-row order; only the first ``count`` rows are written.  A count row that is not an integer in
     [0, M] adds 1 to ``bad`` (int32 [1], device).  Nothing is read on the host."""
@@ -836,7 +850,9 @@ def query_candidates(packed, img_wh, score_thr, expand_ratio, bad):
     rois = torch.empty((B * M, 5), dtype=torch.float32, device=dev)
     labels = torch.empty((B * M,), dtype=torch.int32, device=dev)
     count = torch.empty((1,), dtype=torch.int32, device=dev)
-    check(load().mqdet_query_candidates(_ptr(packed), B, M, float(score_thr), float(expand_ratio), int(img_wh[0]), int(img_wh[1]),
+    wh = [(int(w), int(h)) for w, h in img_wh] if isinstance(img_wh[0], (tuple, list)) else [(int(img_wh[0]), int(img_wh[1]))]
+    wh_h = (ctypes.c_int64 * (2 * len(wh)))(*[v for p in wh for v in p])
+    check(load().mqdet_query_candidates(_ptr(packed), B, M, float(score_thr), float(expand_ratio), wh_h, len(wh),
                                         _ptr(rois), _ptr(labels), B * M, _ptr(count), _ptr(bad), _stream()), "query_candidates")
     launch_count += 1
     return rois, labels, count
@@ -1072,7 +1088,9 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
                      pre_nms_top_n=1000, nms_thresh=0.6, max_det=100, max_out=128, want_keys=False, class_labels=None):
     """logits [B,N,T], reg_ctr [B,N,5] -> dict(det [B,max_out,6], num [B], + the pre-NMS candidates). All on device.
     tokmap int32 [C, max_tok] (shared) or [B, C, max_tok] (one positive map per image: batched prompt chunks);
-    class_labels int32 [C] / [B, C] or None (label of score column c = c + 1)."""
+    class_labels int32 [C] / [B, C] or None (label of score column c = c + 1).
+    ``img_w`` / ``img_h``: the clip size of every element, or sequences of n per-image sizes (a padded batch of differently sized
+    images); element e clips to size e % n, so a chunked pass (e = chunk * B + image) passes its B image sizes."""
     import numpy as np
     global launch_count
     _need_cuda(logits, reg_ctr, tokmap)
@@ -1091,6 +1109,8 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
     stride_h = np.asarray(strides, dtype=np.float32)
     base_h = np.asarray([base_anchor(s, a) for s, a in zip(strides, anchor_sizes)], dtype=np.float32)
     scale_h = np.asarray(reg_scales, dtype=np.float32)
+    wh_h = np.ascontiguousarray(np.stack(np.broadcast_arrays(np.asarray(img_w, dtype=np.float32).reshape(-1),
+                                                             np.asarray(img_h, dtype=np.float32).reshape(-1)), 1))
     S = (L * pre_nms_top_n + 255) // 256 * 256
     ws = torch.empty((int(load().mqdet_atss_workspace_bytes(levels.hw_ptr, L, C, B)),), dtype=torch.uint8, device=dev)
     lvl_counts = torch.empty((B, L), dtype=torch.int32, device=dev)
@@ -1104,7 +1124,7 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
                                        lab_stride, C, max_tok, T, levels.hw_ptr, L,
                                        stride_h.ctypes.data_as(ctypes.c_void_p), base_h.ctypes.data_as(ctypes.c_void_p),
                                        scale_h.ctypes.data_as(ctypes.c_void_p), B, float(pre_nms_thresh), int(pre_nms_top_n),
-                                       S, float(img_w), float(img_h), _ptr(ws), _ptr(lvl_counts), _ptr(ob), _ptr(osc),
+                                       S, wh_h.ctypes.data_as(ctypes.c_void_p), wh_h.shape[0], _ptr(ws), _ptr(lvl_counts), _ptr(ob), _ptr(osc),
                                        _ptr(ol), _ptr(okey), _ptr(cb), _ptr(csc), _ptr(cl), _ptr(totals), _stream()),
           "atss_candidates")
     nws = torch.empty((int(load().mqdet_ml_nms_batched_workspace_bytes(B, S)),), dtype=torch.uint8, device=dev)
