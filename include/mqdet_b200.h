@@ -294,6 +294,15 @@ int mqdet_atss_candidates(const void* logits, int logits_dtype, const float* reg
                           int64_t out_stride, const float* img_wh, int64_t n_sizes, void* cand_ws, int32_t* level_counts,
                           float* out_boxes, float* out_scores, float* out_labels, int64_t* out_key, float* cat_boxes,
                           float* cat_scores, float* cat_labels, int32_t* totals, void* stream);
+/* mqdet_atss_candidates with the (w, h) table img_wh_dev f32 [n_sizes][2] in DEVICE memory, read by the kernel (same n_sizes
+ * rules): a CUDA graph captured over it clips each replay to the sizes the table holds then. */
+int mqdet_atss_candidates_sizes_dev(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
+                                    int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride, int64_t C,
+                                    int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev, const float* strides,
+                                    const float* base_anchors, const float* reg_scales, int64_t B, float pre_nms_thresh,
+                                    int64_t topk, int64_t out_stride, const float* img_wh_dev, int64_t n_sizes, void* cand_ws,
+                                    int32_t* level_counts, float* out_boxes, float* out_scores, float* out_labels, int64_t* out_key,
+                                    float* cat_boxes, float* cat_scores, float* cat_labels, int32_t* totals, void* stream);
 
 /* Batched multi-label NMS: rows of n_max (multiple of 256) candidates per image, counts on the device. */
 int64_t mqdet_ml_nms_batched_workspace_bytes(int64_t B, int64_t n_max);

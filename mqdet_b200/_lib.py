@@ -100,6 +100,11 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p, c_int64, c_float, c_int64, c_int64, c_void_p, c_int64,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p]),
+    "mqdet_atss_candidates_sizes_dev": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64,
+                                                c_int64, c_void_p, c_int64,
+                                                c_void_p, c_void_p, c_void_p, c_int64, c_float, c_int64, c_int64, c_void_p, c_int64,
+                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p]),
     "mqdet_ml_nms_batched_workspace_bytes": (c_int64, [c_int64, c_int64]),
     "mqdet_ml_nms_batched": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_int64, c_void_p,
                                      c_void_p, c_void_p, c_void_p]),

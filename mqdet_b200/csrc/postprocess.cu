@@ -22,9 +22,11 @@ constexpr int PP_TOPK_MAX = 1024;
 constexpr int PP_MAX_SIZES = 256;   // clip sizes per launch: one per image of a padded batch (kernel-parameter table)
 
 // Clip bound of every batch element: element e clips to [0, wh[e % n][0] - 1] x [0, wh[e % n][1] - 1].  n = 1: one size for all;
-// n = B images: the elements of a chunked pass (e = chunk * B + image) repeat the image sizes chunk by chunk.
+// n = B images: the elements of a chunked pass (e = chunk * B + image) repeat the image sizes chunk by chunk.  The table travels
+// by value in ``wh``, or lives in device memory at ``dev`` (non-null), so that a captured graph reads the sizes of each replay.
 struct PPSizes {
   int n;
+  const float* dev;
   float wh[PP_MAX_SIZES][2];
 };
 
@@ -193,7 +195,8 @@ __global__ void __launch_bounds__(1024) atss_select_decode_kernel(const unsigned
     const DecodedBox d = box_decode(r[0] * sc, r[1] * sc, r[2] * sc, r[3] * sc, ax1, ay1, ax2, ay2);
     float x1 = d.x1, y1 = d.y1, x2 = d.x2, y2 = d.y2;
     // clip_to_image(remove_empty=False), TO_REMOVE = 1, to this element's own image size
-    const float img_w = sz.wh[b % sz.n][0], img_h = sz.wh[b % sz.n][1];
+    const float* wh = sz.dev ? sz.dev + 2 * (b % sz.n) : sz.wh[b % sz.n];
+    const float img_w = wh[0], img_h = wh[1];
     x1 = fminf(fmaxf(x1, 0.f), img_w - 1.f);
     y1 = fminf(fmaxf(y1, 0.f), img_h - 1.f);
     x2 = fminf(fmaxf(x2, 0.f), img_w - 1.f);
@@ -306,26 +309,27 @@ static int fill_pp_levels(PPLevels* lv, const int32_t* level_hw, int64_t nlev, c
   return off;
 }
 
-extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
-                                     int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride,
-                                     int64_t C, int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev,
-                                     const float* strides, const float* base_anchors, const float* reg_scales, int64_t B,
-                                     float pre_nms_thresh, int64_t topk, int64_t out_stride, const float* img_wh, int64_t n_sizes,
-                                     void* cand_ws,
-                                     int32_t* level_counts, float* out_boxes, float* out_scores, float* out_labels,
-                                     int64_t* out_key, float* cat_boxes, float* cat_scores, float* cat_labels,
-                                     int32_t* totals, void* stream) {
+// The two entries share everything but where the clip table comes from: a host table copied into the kernel parameters, or a
+// device table the select kernel reads.
+static int atss_candidates_impl(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
+                                int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride, int64_t C,
+                                int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev, const float* strides,
+                                const float* base_anchors, const float* reg_scales, int64_t B, float pre_nms_thresh, int64_t topk,
+                                int64_t out_stride, const float* img_wh, const float* img_wh_dev, int64_t n_sizes, void* cand_ws,
+                                int32_t* level_counts, float* out_boxes, float* out_scores, float* out_labels, int64_t* out_key,
+                                float* cat_boxes, float* cat_scores, float* cat_labels, int32_t* totals, void* stream) {
   MQ_REQUIRE(logits && reg_ctr && tokmap_dev && level_hw && strides && base_anchors && cand_ws && level_counts && out_boxes &&
                  out_scores && out_labels && cat_boxes && cat_scores && cat_labels && totals,
              "atss_candidates: null pointer");
   MQ_REQUIRE(T > 0 && T <= PP_MAX_T, "atss_candidates: T=%ld exceeds %d", (long)T, PP_MAX_T);
   MQ_REQUIRE(topk > 0 && topk <= PP_TOPK_MAX, "atss_candidates: topk=%ld exceeds %d", (long)topk, PP_TOPK_MAX);
-  MQ_REQUIRE(img_wh && n_sizes >= 1 && n_sizes <= PP_MAX_SIZES && B % n_sizes == 0,
+  MQ_REQUIRE((img_wh || img_wh_dev) && n_sizes >= 1 && n_sizes <= PP_MAX_SIZES && B % n_sizes == 0,
              "atss_candidates: %ld image sizes for %ld batch elements (one, or one per image of the pass, at most %d)",
              (long)n_sizes, (long)B, PP_MAX_SIZES);
   PPSizes sz{};
   sz.n = (int)n_sizes;
-  for (int64_t i = 0; i < n_sizes; ++i) {
+  sz.dev = img_wh_dev;
+  for (int64_t i = 0; img_wh && i < n_sizes; ++i) {
     sz.wh[i][0] = img_wh[2 * i];
     sz.wh[i][1] = img_wh[2 * i + 1];
   }
@@ -360,6 +364,37 @@ extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const
   atss_concat_kernel<<<(unsigned)B, 256, 0, st>>>(out_boxes, out_scores, out_labels, level_counts, (int)nlev, (int)topk,
                                                   out_per_img, cat_boxes, cat_scores, cat_labels, totals);
   return check_launch("atss_concat_kernel");
+}
+
+extern "C" int mqdet_atss_candidates(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
+                                     int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride,
+                                     int64_t C, int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev,
+                                     const float* strides, const float* base_anchors, const float* reg_scales, int64_t B,
+                                     float pre_nms_thresh, int64_t topk, int64_t out_stride, const float* img_wh, int64_t n_sizes,
+                                     void* cand_ws,
+                                     int32_t* level_counts, float* out_boxes, float* out_scores, float* out_labels,
+                                     int64_t* out_key, float* cat_boxes, float* cat_scores, float* cat_labels,
+                                     int32_t* totals, void* stream) {
+  MQ_REQUIRE(img_wh, "atss_candidates: null image size table");
+  return atss_candidates_impl(logits, logits_dtype, reg_ctr, tokmap_dev, tokmap_img_stride, class_labels, labels_img_stride, C,
+                              max_tok, T, level_hw, nlev, strides, base_anchors, reg_scales, B, pre_nms_thresh, topk, out_stride,
+                              img_wh, nullptr, n_sizes, cand_ws, level_counts, out_boxes, out_scores, out_labels, out_key, cat_boxes,
+                              cat_scores, cat_labels, totals, stream);
+}
+
+extern "C" int mqdet_atss_candidates_sizes_dev(const void* logits, int logits_dtype, const float* reg_ctr, const int32_t* tokmap_dev,
+                                               int64_t tokmap_img_stride, const int32_t* class_labels, int64_t labels_img_stride,
+                                               int64_t C, int64_t max_tok, int64_t T, const int32_t* level_hw, int64_t nlev,
+                                               const float* strides, const float* base_anchors, const float* reg_scales, int64_t B,
+                                               float pre_nms_thresh, int64_t topk, int64_t out_stride, const float* img_wh_dev,
+                                               int64_t n_sizes, void* cand_ws, int32_t* level_counts, float* out_boxes,
+                                               float* out_scores, float* out_labels, int64_t* out_key, float* cat_boxes,
+                                               float* cat_scores, float* cat_labels, int32_t* totals, void* stream) {
+  MQ_REQUIRE(img_wh_dev, "atss_candidates_sizes_dev: null image size table");
+  return atss_candidates_impl(logits, logits_dtype, reg_ctr, tokmap_dev, tokmap_img_stride, class_labels, labels_img_stride, C,
+                              max_tok, T, level_hw, nlev, strides, base_anchors, reg_scales, B, pre_nms_thresh, topk, out_stride,
+                              nullptr, img_wh_dev, n_sizes, cand_ws, level_counts, out_boxes, out_scores, out_labels, out_key,
+                              cat_boxes, cat_scores, cat_labels, totals, stream);
 }
 
 extern "C" int64_t mqdet_atss_workspace_bytes(const int32_t* level_hw, int64_t nlev, int64_t C, int64_t B) {

@@ -19,7 +19,16 @@ images + one prompt), same outputs (``list[BoxList]`` per batch), but
     away from the persistent one-CTA-per-SM kernels of the next forward, so the collective is kept rare, not per step.
 
 Nothing here computes: it is stream / graph / buffer plumbing around ``GeneralizedVLRCNN_New.forward_device``.
+
+``run_batches`` / ``run_images`` of both engines take the reference's test-loader batches instead: padded batches of differently
+sized images, whose batch size and padded shape change from batch to batch (``engine/batches.py::reference_test_batches``).  They
+keep one CUDA graph per padded batch shape (B, Hp, Wp) in ``ShapeGraphs``; the image sizes are not part of a graph, they travel in a
+device table the forward reads.
 """
+import random
+import time
+from collections import OrderedDict
+
 import torch
 import torch.distributed as dist
 
@@ -29,11 +38,13 @@ from ..structures.image_list import ImageList
 
 
 class InferenceEngine:
-    def __init__(self, model, captions, positive_map, batch_shape, image_sizes, *, use_graph=True, gather=True, warmup=2,
-                 gather_every=8):
+    def __init__(self, model, captions, positive_map, batch_shape=None, image_sizes=None, *, use_graph=True, gather=True, warmup=2,
+                 gather_every=8, max_graphs=None):
         """model: GeneralizedVLRCNN_New (eval, on its CUDA device); captions / positive_map: the prompt of the run;
         batch_shape: (B, 3, H, W) of the padded batch tensor; image_sizes: [(h, w)] * B un-padded sizes;
-        gather_every: steps whose packed results are exchanged by one all-gather (N > 1)."""
+        gather_every: steps whose packed results are exchanged by one all-gather (N > 1).
+        Without ``batch_shape`` / ``image_sizes`` nothing is captured up front and only ``run_batches`` / ``run_images`` serve;
+        ``max_graphs`` bounds their live graphs (default ``ShapeGraphs.MAX_GRAPHS``)."""
         # vision-only evaluation: at TEXT_DROPOUT >= 1 the masked ids are part of the captured prompt state
         self.mask_rate = model.text_mask_rate()
         if 0 < self.mask_rate < 1:
@@ -44,6 +55,15 @@ class InferenceEngine:
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise MqdetError("InferenceEngine: the model must live on a CUDA device (no CPU fallback)")
+        self.warmup, self.max_graphs = max(1, warmup), max_graphs
+        self.batches = None                     # ShapeGraphs of run_batches / run_images, built on first use
+        self.graphs, self.outs = [None, None], [None, None]
+        self.use_graph = bool(use_graph)
+        self.max_out = model.max_out()
+        if batch_shape is None or image_sizes is None:
+            if batch_shape is not None or image_sizes is not None:
+                raise ValueError("InferenceEngine: batch_shape and image_sizes go together")
+            return
         self.image_sizes = [tuple(s) for s in image_sizes]
         self.B = int(batch_shape[0])
         self.world = dist.get_world_size() if (gather and dist.is_available() and dist.is_initialized()) else 1
@@ -51,9 +71,6 @@ class InferenceEngine:
         self.copy_stream = torch.cuda.Stream(device=self.dev)
         self.up_done = [torch.cuda.Event(), torch.cuda.Event()]   # upload into stage[k] finished
         self.fw_done = [torch.cuda.Event(), torch.cuda.Event()]   # the forward that read stage[k] finished
-        self.graphs = [None, None]
-        self.outs = [None, None]
-        self.max_out = model.max_out()
         # local packed result of a step -> pinned host (the BoxLists of `run`)
         self.host = [torch.empty((self.B, self.max_out + 1, 6), dtype=torch.float32).pin_memory() for _ in range(2)]
         self.d2h_done = [torch.cuda.Event(), torch.cuda.Event()]
@@ -82,7 +99,6 @@ class InferenceEngine:
                 self._collect(k, to_host=False)
         self.flush()
         torch.cuda.synchronize(self.dev)
-        self.use_graph = bool(use_graph)
         if self.use_graph:
             pool = None
             for k in range(2):  # one graph per staging buffer (the input address is baked into the graph); the two graphs
@@ -181,23 +197,45 @@ class InferenceEngine:
         self.graphs = [None, None]
         self.outs = [None, None]
         self.use_graph = False
+        if self.batches is not None:
+            self.batches.close()
+            self.batches = None
         torch.cuda.synchronize(self.dev)
 
     def to_boxlists(self, k=0):
         """BoxLists of the LOCAL images from pinned host buffer k (waits for that step's device->host copy only)."""
-        from ..structures.bounding_box import BoxList
         self.d2h_done[k].synchronize()
-        mine = self.host[k]
-        res = []
-        for b, (h, w) in enumerate(self.image_sizes):
-            n = int(round(float(mine[b, self.max_out, 0])))
-            if n > self.max_out:
-                raise MqdetError(f"image {b}: {n} detections exceed the {self.max_out}-row result buffer")
-            bl = BoxList(mine[b, :n, :4].clone(), (w, h), mode="xyxy")
-            bl.add_field("labels", mine[b, :n, 5].long())
-            bl.add_field("scores", mine[b, :n, 4].clone())
-            res.append(bl)
-        return res
+        return packed_to_boxlists(self.host[k], self.image_sizes, self.max_out)
+
+    def _shape_graphs(self):
+        if self.batches is None:
+            model, caps, pmap = self.model, self.captions, self.positive_map
+            mask_rate = self.mask_rate
+
+            def after_replay(state):   # the draws of the eager forward, so that Python's random advances as in the reference
+                if mask_rate > 0:
+                    model.draw_text_masks(state[0]["has"], mask_rate)
+
+            self.batches = ShapeGraphs(model, lambda il, wh: model.forward_device(il, caps, pmap, img_wh=wh)["det_packed"],
+                                       self.max_out + 1, lambda packed, sizes: packed_to_boxlists(packed, sizes, self.max_out),
+                                       use_graph=self.use_graph, warmup=self.warmup, max_graphs=self.max_graphs,
+                                       after_replay=after_replay)
+        return self.batches
+
+    def run_batches(self, batches):
+        """batches: iterable of ``ImageList`` (a pinned-host or device fp32 tensor [B, 3, Hp, Wp] + ``image_sizes``), e.g. the
+        reference's test-loader batches -> yields list[BoxList] per batch, each at its image's own size, equal bit for bit to
+        ``model(il, ...)``.  One graph per (B, Hp, Wp), captured the first time that shape comes (see ``ShapeGraphs``); the
+        upload of batch s+1 overlaps the forward of batch s."""
+        _refuse_multi_gpu("run_batches")
+        return self._shape_graphs().run_batches(batches)
+
+    def run_images(self, images_u8, index_batches):
+        """Decoded uint8 HWC RGB images + the index lists of ``reference_test_batches`` -> yields list[BoxList] per index list in
+        original-image coordinates, equal to ``predict(model, [images_u8[i] for i in idx], ..., mixed_sizes=True)``.  The upload and
+        the test transform run on the copy stream, straight into the staging buffer the next forward reads."""
+        _refuse_multi_gpu("run_images")
+        return self._shape_graphs().run_images(images_u8, index_batches)
 
     def run(self, batches):
         """batches: iterable of pinned (or pageable) HOST tensors [B, 3, H, W] -> yields list[BoxList] per batch, in order.
@@ -237,11 +275,21 @@ class GroundingDINOEngine:
         for boxlists in eng.run(host_batches): ...
     """
 
-    def __init__(self, model, captions, positive_map, batch_shape, image_sizes, *, use_graph=True, gather=True, warmup=2):
+    def __init__(self, model, captions, positive_map, batch_shape=None, image_sizes=None, *, use_graph=True, gather=True, warmup=2,
+                 max_graphs=None):
+        """Without ``batch_shape`` / ``image_sizes`` nothing is captured up front and only ``run_batches`` / ``run_images`` serve
+        (one graph per padded shape, at most ``max_graphs`` live, default ``ShapeGraphs.MAX_GRAPHS``)."""
         self.model, self.captions, self.positive_map = model, captions, positive_map
         self.dev = next(model.parameters()).device
         if self.dev.type != "cuda":
             raise MqdetError("GroundingDINOEngine: the model must live on a CUDA device (no CPU fallback)")
+        self.use_graph, self.warmup, self.max_graphs = bool(use_graph), max(1, warmup), max_graphs
+        self.batches = None                     # ShapeGraphs of run_batches / run_images, built on first use
+        self.graph, self.static_out, self.note = None, None, "eager launches"
+        if batch_shape is None or image_sizes is None:
+            if batch_shape is not None or image_sizes is not None:
+                raise ValueError("GroundingDINOEngine: batch_shape and image_sizes go together")
+            return
         self.image_sizes = [tuple(s) for s in image_sizes]
         self.B, self.nq = int(batch_shape[0]), int(model.num_queries)
         self.world = dist.get_world_size() if (gather and dist.is_available() and dist.is_initialized()) else 1
@@ -289,3 +337,272 @@ class GroundingDINOEngine:
             self.host.copy_(local, non_blocking=True)
             torch.cuda.current_stream(self.dev).synchronize()
             yield GroundingDINO.to_boxlists(self.host, self.image_sizes)
+
+    def _shape_graphs(self):
+        if self.batches is None:
+            from ..modeling.groundingdino.groundingdino import GroundingDINO
+            model, caps, pmap = self.model, self.captions, self.positive_map
+            self.batches = ShapeGraphs(model, lambda il, wh: model.forward_device(il, caps, pmap, img_wh=wh)["det_packed"],
+                                       int(model.num_queries) + 1, GroundingDINO.to_boxlists, use_graph=self.use_graph,
+                                       warmup=self.warmup, max_graphs=self.max_graphs)
+        return self.batches
+
+    def run_batches(self, batches):
+        """``InferenceEngine.run_batches`` for MQ-GroundingDINO: ImageLists in, list[BoxList] per batch out, each equal bit for bit
+        to ``model(il, ...)``; one graph per padded shape, so a dataset of differently sized images (the reference's one image per
+        test batch) replays a graph per shape instead of launching every kernel from the host."""
+        _refuse_multi_gpu("run_batches")
+        return self._shape_graphs().run_batches(batches)
+
+    def run_images(self, images_u8, index_batches):
+        """``InferenceEngine.run_images`` for MQ-GroundingDINO."""
+        _refuse_multi_gpu("run_images")
+        return self._shape_graphs().run_images(images_u8, index_batches)
+
+    def close(self):
+        """Drop the graphs of ``run_batches`` / ``run_images``."""
+        if self.batches is not None:
+            self.batches.close()
+            self.batches = None
+
+
+def packed_to_boxlists(packed, image_sizes, max_out):
+    """Pinned-host packed rows [B, max_out + 1, 6] (row max_out = (count, ...)) -> BoxList (mode xyxy, fields labels / scores)
+    per image at its (h, w) of ``image_sizes``."""
+    from ..structures.bounding_box import BoxList
+    res = []
+    for b, (h, w) in enumerate(image_sizes):
+        n = int(round(float(packed[b, max_out, 0])))
+        if n > max_out:
+            raise MqdetError(f"image {b}: {n} detections exceed the {max_out}-row result buffer")
+        bl = BoxList(packed[b, :n, :4].clone(), (w, h), mode="xyxy")
+        bl.add_field("labels", packed[b, :n, 5].long())
+        bl.add_field("scores", packed[b, :n, 4].clone())
+        res.append(bl)
+    return res
+
+
+def _refuse_multi_gpu(what):
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise NotImplementedError(f"{what} runs on one GPU: under GroupedBatchSampler the ranks' batch counts and tail sizes differ, "
+                                  "so the ranks would not reach the same steps; run it per rank without a process group, or "
+                                  "use run() with one batch shape")
+
+
+class _Graph:
+    __slots__ = ("graph", "state")
+
+    def __init__(self, graph, state):
+        self.graph, self.state = graph, state
+
+
+class ShapeGraphs:
+    """CUDA graphs of one detector forward keyed by the padded batch shape (B, Hp, Wp), for padded batches of differently sized
+    images.
+
+    Buffers, all allocated outside the graphs' memory pool, each sized for the largest batch the config allows (TEST.IMS_PER_BATCH
+    images of MAX_SIZE_TEST rounded up to SIZE_DIVISIBILITY on both sides; a larger batch is refused):
+      * two staging slots, each an input buffer, a device (w, h) size table and a pinned host result buffer.  The copy stream
+        writes a batch's images and sizes into slot s % 2 while the forward of the batch before runs;
+      * the graphs' own input, size table and result buffer.  Before a replay the main stream copies the slot into them (a
+        device-to-device copy of the batch, well under 1% of a forward); every graph reads the input and the table at the
+        addresses it was captured with and ends by copying its packed result into the result buffer.  So one graph serves both
+        slots, and a shape is captured once.
+    Because every graph's result leaves the pool before the graph ends, the pool holds only scratch that a replay writes before
+    it reads it: all graphs share it, and they may replay in the order of the data rather than the order of capture.
+
+    A new shape gets ``warmup`` eager forwards (they fill the per-prompt / per-batch-size caches and the lazy kernel set-up), then
+    a capture.  The single-entry caches of the model (prompt state, token map, GCP tables) are replaced when another batch size
+    comes; each graph keeps the entries it captured (``model.graph_state()``) for as long as it lives, so a replay never reads a
+    freed block.  Keeping them with the graph rather than keying the caches ties their lifetime to the one thing that reads them,
+    with no second bound or eviction policy to keep in step.  At most ``max_graphs`` graphs live; the least recently used one
+    is dropped first.  A short tail batch is its own shape: padding it with dummy images would change its results in the last
+    bits, since batch elements agree only to rounding."""
+
+    # Live graphs by default.  Measured per captured graph (tools/prof_mixed_batches.py, H100 80GB HBM3, 700 W; DESIGN.md section
+    # 5): MQ-GLIP-T 16 MB allocated / 183 MB reserved, MQ-GroundingDINO-T 43 / 113 MB.  32 graphs hold at most ~6 GB, and cover
+    # the padded shapes of a COCO-sized set at 800 / 1333 (one side at 800, the other in 32-pixel steps, per orientation).
+    MAX_GRAPHS = 32
+
+    def __init__(self, model, forward, rows, to_boxlists, *, use_graph=True, warmup=1, max_graphs=None, after_replay=None):
+        """forward(ImageList, img_wh fp32 [B, 2] device) -> packed fp32 [B, rows, 6] device result; to_boxlists(pinned packed
+        [B, rows, 6], image_sizes) -> list[BoxList]; after_replay(graph state): host work an eager forward would also do."""
+        cfg = model.cfg
+        self.model, self.forward, self.rows, self.to_boxlists = model, forward, int(rows), to_boxlists
+        self.after_replay = after_replay
+        self.use_graph, self.warmup = bool(use_graph), max(1, int(warmup))
+        self.max_graphs = self.MAX_GRAPHS if max_graphs is None else int(max_graphs)
+        if self.max_graphs < 1:
+            raise ValueError(f"max_graphs must be >= 1, got {max_graphs}")
+        self.dev = next(model.parameters()).device
+        div = int(cfg.DATALOADER.SIZE_DIVISIBILITY)
+        side = int(cfg.INPUT.MAX_SIZE_TEST)
+        side = -(-side // div) * div if div > 0 else side
+        self.max_B, self.max_hw = int(cfg.TEST.IMS_PER_BATCH), (side, side)
+        n = self.max_B * 3 * side * side
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        self.slot_in = [torch.empty((n,), **f32) for _ in range(2)]
+        self.slot_wh = [torch.empty((self.max_B, 2), **f32) for _ in range(2)]
+        self.host = [torch.empty((self.max_B, self.rows, 6), dtype=torch.float32).pin_memory() for _ in range(2)]
+        self.g_in, self.g_wh = torch.empty((n,), **f32), torch.zeros((self.max_B, 2), **f32)
+        self.g_res = torch.empty((self.max_B, self.rows, 6), **f32)
+        self.buffer_bytes = 4 * (3 * n + 3 * 2 * self.max_B + self.max_B * self.rows * 6)
+        self.copy_stream = torch.cuda.Stream(device=self.dev)
+        self.up_done = [torch.cuda.Event() for _ in range(2)]     # images + sizes of slot k uploaded
+        self.fw_done = [torch.cuda.Event() for _ in range(2)]     # slot k copied into the graph input: it may be overwritten
+        self.d2h_done = [torch.cuda.Event() for _ in range(2)]    # packed result of slot k in its pinned host buffer
+        main = torch.cuda.current_stream(self.dev)
+        for ev in self.fw_done + self.d2h_done:
+            ev.record(main)
+        self.pool = torch.cuda.graph_pool_handle()
+        self.graphs = OrderedDict()
+        self.captures, self.evictions, self.capture_s = 0, 0, 0.0
+        self.keys = set()
+
+    def close(self):
+        torch.cuda.synchronize(self.dev)
+        for e in self.graphs.values():
+            e.graph.reset()
+        self.graphs.clear()
+
+    def stats(self):
+        """Captures, seconds spent in warm-ups and captures, distinct shapes seen, evictions, graphs live."""
+        return {"captures": self.captures, "capture_s": self.capture_s, "keys": len(self.keys), "evictions": self.evictions,
+                "live": len(self.graphs)}
+
+    # -- staging (copy stream) -------------------------------------------------------------------------------------------
+    def _check_shape(self, B, Hp, Wp):
+        if not (1 <= B <= self.max_B and Hp <= self.max_hw[0] and Wp <= self.max_hw[1]):
+            raise MqdetError(f"batch [{B}, 3, {Hp}, {Wp}] exceeds the staging buffers [{self.max_B}, 3, {self.max_hw[0]}, "
+                             f"{self.max_hw[1]}] (TEST.IMS_PER_BATCH images of INPUT.MAX_SIZE_TEST rounded up to SIZE_DIVISIBILITY)")
+
+    def _stage_sizes(self, k, image_sizes):
+        """(copy stream) the (w, h) table of the batch -> slot k."""
+        wh = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32).pin_memory()
+        self.slot_wh[k][:len(image_sizes)].copy_(wh, non_blocking=True)
+
+    def _stage_batch(self, k, il):
+        x = il.tensors
+        if x.dim() != 4 or x.shape[1] != 3 or x.dtype != torch.float32:
+            raise MqdetError(f"run_batches: fp32 [B, 3, Hp, Wp] images required (got {x.dtype} {tuple(x.shape)})")
+        B, _, Hp, Wp = x.shape
+        if len(il.image_sizes) != B:
+            raise MqdetError(f"run_batches: {len(il.image_sizes)} image sizes for {B} images")
+        self._check_shape(B, Hp, Wp)
+        cs = self.copy_stream
+        produced = torch.cuda.Event()
+        produced.record(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(cs):
+            cs.wait_event(self.fw_done[k])                       # the forward before has taken slot k's contents
+            if x.is_cuda:
+                cs.wait_event(produced)
+                x.record_stream(cs)
+            self.slot_in[k][:x.numel()].view(B, 3, Hp, Wp).copy_(x, non_blocking=True)
+            self._stage_sizes(k, il.image_sizes)
+            self.up_done[k].record(cs)
+        return (B, Hp, Wp), [tuple(s) for s in il.image_sizes], None
+
+    def _stage_images(self, k, tf, images_u8, idx):
+        cs = self.copy_stream
+        produced = torch.cuda.Event()                            # device images may come from work on the main stream
+        produced.record(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(cs):
+            cs.wait_event(self.fw_done[k])
+            cs.wait_event(produced)
+            il, orig = tf([images_u8[i] for i in idx], self.dev, mixed_sizes=True, out=self.slot_in[k])
+            B, _, Hp, Wp = il.tensors.shape
+            self._check_shape(B, Hp, Wp)
+            self._stage_sizes(k, il.image_sizes)
+            self.up_done[k].record(cs)
+        return (B, Hp, Wp), il.image_sizes, orig
+
+    # -- one forward (main stream) ---------------------------------------------------------------------------------------
+    def _graph_input(self, key):
+        B, Hp, Wp = key
+        return self.g_in[:B * 3 * Hp * Wp].view(B, 3, Hp, Wp), self.g_wh[:B]
+
+    def _capture(self, key, image_sizes):
+        x, wh = self._graph_input(key)
+        il = ImageList(x, image_sizes)
+        t0 = time.perf_counter()
+        for i in range(self.warmup):
+            self.forward(il, wh)
+            if i == 0:   # the first forward draws what an eager forward of this batch draws (vision-only masks, query picks);
+                rstate = random.getstate()   # the further warm-ups and the capture must not advance Python's random
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, pool=self.pool):
+            self.g_res[:key[0]].copy_(self.forward(il, wh))
+        state = self.model.graph_state()
+        random.setstate(rstate)
+        e = self.graphs[key] = _Graph(g, state)
+        while len(self.graphs) > self.max_graphs:   # evicted after the capture: the shared pool must stay in use meanwhile
+            _, old = self.graphs.popitem(last=False)
+            old.graph.reset()
+            self.evictions += 1
+        torch.cuda.synchronize(self.dev)
+        self.capture_s += time.perf_counter() - t0
+        self.captures += 1
+        return e
+
+    def _launch(self, k, key, image_sizes):
+        main = torch.cuda.current_stream(self.dev)
+        main.wait_event(self.up_done[k])
+        main.wait_event(self.d2h_done[k])                       # slot k's host buffer has been read by the previous batch
+        B, Hp, Wp = key
+        n = B * 3 * Hp * Wp
+        self.g_in[:n].copy_(self.slot_in[k][:n], non_blocking=True)
+        self.g_wh[:B].copy_(self.slot_wh[k][:B], non_blocking=True)
+        self.fw_done[k].record(main)
+        self.keys.add(key)
+        if self.use_graph:
+            e = self.graphs.get(key)
+            fresh = e is None
+            if fresh:
+                e = self._capture(key, image_sizes)
+            else:
+                self.graphs.move_to_end(key)
+            e.graph.replay()
+            if self.after_replay is not None and not fresh:   # a new shape's first warm-up forward did this batch's host work
+                self.after_replay(e.state)
+        else:
+            x, wh = self._graph_input(key)
+            self.g_res[:B].copy_(self.forward(ImageList(x, image_sizes), wh))
+        self.host[k][:B].copy_(self.g_res[:B], non_blocking=True)
+        self.d2h_done[k].record(main)
+
+    def _results(self, k, B, image_sizes):
+        self.d2h_done[k].synchronize()
+        return self.to_boxlists(self.host[k][:B], image_sizes)
+
+    def _run(self, items, stage):
+        """Two batches in flight: batch s+1 is staged and its forward queued before the host turns batch s into BoxLists."""
+        it = iter(items)
+        first = next(it, None)
+        if first is None:
+            return
+        k = 0
+        cur = stage(k, first)
+        self._launch(k, cur[0], cur[1])
+        while True:
+            item = next(it, None)
+            nxt = None
+            if item is not None:
+                nxt = stage(k ^ 1, item)
+                self._launch(k ^ 1, nxt[0], nxt[1])
+            key, sizes, orig = cur
+            res = self._results(k, key[0], sizes)
+            yield res if orig is None else [bl.resize(o) for bl, o in zip(res, orig)]
+            if nxt is None:
+                return
+            k ^= 1
+            cur = nxt
+
+    @torch.no_grad()
+    def run_batches(self, batches):
+        yield from self._run(batches, self._stage_batch)
+
+    @torch.no_grad()
+    def run_images(self, images_u8, index_batches):
+        from .transforms import TestTransform
+        tf = TestTransform(self.model.cfg)
+        yield from self._run(index_batches, lambda k, idx: self._stage_images(k, tf, images_u8, idx))

@@ -109,7 +109,7 @@ class TestTransform:
     def target_size(self, h, w):
         return get_size((w, h), self.size, self.max_size)
 
-    def __call__(self, images, device, pad=True, want_resized=False, mixed_sizes=False):
+    def __call__(self, images, device, pad=True, want_resized=False, mixed_sizes=False, out=None):
         """images: uint8 HWC RGB numpy arrays or tensors (host or ``device``) -> (ImageList, orig_sizes [(w, h)]).  By default all
         images must resize to one size, so that a batch holds no padding beyond SIZE_DIVISIBILITY and ``want_resized`` has one
         shape.  ``pad=False`` leaves the batch at the resized size; ``want_resized`` adds the resized uint8 images [B, oh, ow, 3]
@@ -117,7 +117,10 @@ class TestTransform:
 
         ``mixed_sizes=True`` takes images that resize to different sizes, as the reference's test loader batches them: each is
         resized to its own target size and the batch is zero-padded to the largest, rounded up to SIZE_DIVISIBILITY (its
-        ``to_image_list``); ``image_sizes`` holds every image's own target size.  ``want_resized`` is then refused."""
+        ``to_image_list``); ``image_sizes`` holds every image's own target size.  ``want_resized`` is then refused.
+
+        ``out``: a flat fp32 buffer on ``device`` to write the batch into (its leading B * 3 * Hp * Wp elements, which the returned
+        ImageList's tensor views), e.g. a staging buffer a captured graph reads."""
         if len(images) == 0:
             raise MqdetError("TestTransform: no images")
         device = _cuda_device(device)
@@ -133,6 +136,13 @@ class TestTransform:
         oh, ow = max(h for h, _ in per_image), max(w for _, w in per_image)
         div = self.div if pad else 0
         Hp, Wp = (-(-oh // div) * div, -(-ow // div) * div) if div > 0 else (oh, ow)
+        dst = None
+        if out is not None:
+            need = len(dev_images) * 3 * Hp * Wp
+            if out.dtype != torch.float32 or out.dim() != 1 or out.numel() < need or out.device != device:
+                raise MqdetError(f"TestTransform: out must be a flat fp32 buffer on {device} of at least {need} elements for a "
+                                 f"[{len(dev_images)}, 3, {Hp}, {Wp}] batch (got {out.dtype} {tuple(out.shape)} on {out.device})")
+            dst = out[:need].view(len(dev_images), 3, Hp, Wp)
         tables = {}
 
         def table(n_in, n_out):
@@ -143,10 +153,11 @@ class TestTransform:
         if mixed_sizes:
             res = ops.test_transform(dev_images, [table(w, t[1]) for (_, w), t in zip(sizes, per_image)],
                                      [table(h, t[0]) for (h, _), t in zip(sizes, per_image)], per_image, (Hp, Wp), self.mean, self.std,
-                                     bgr=self.bgr, times255=self.times255)
+                                     bgr=self.bgr, times255=self.times255, out=dst)
         else:
             res = ops.test_transform(dev_images, [table(w, ow) for _, w in sizes], [table(h, oh) for h, _ in sizes], (oh, ow),
-                                     (Hp, Wp), self.mean, self.std, bgr=self.bgr, times255=self.times255, want_resized=want_resized)
+                                     (Hp, Wp), self.mean, self.std, bgr=self.bgr, times255=self.times255, want_resized=want_resized,
+                                     out=dst)
         batch, resized = res if want_resized else (res, None)
         il = ImageList(batch, list(per_image))
         orig = [(w, h) for h, w in sizes]

@@ -147,6 +147,13 @@ class GeneralizedVLRCNN_New(nn.Module):
         assert len(labels) == len(query_feats)
         return append_to_bank(query_images, labels, query_feats, self.cfg, exclude_similar, max_query_number)
 
+    def graph_state(self):
+        """The cached tensors a forward just read (prompt state, the head's token map, the GCP index and padded-query tables):
+        whoever captures that forward in a CUDA graph keeps this object as long as the graph, because the next prompt or batch
+        size replaces these single-entry caches and would free memory the graph still reads."""
+        from ..language_backbone import modeling_bert_new
+        return (self._prompt, self.rpn._tokmap) + modeling_bert_new.cache_entries()
+
     def invalidate_prompt_cache(self):
         """Drop everything cached per prompt (token ids, selected queries, masks, the head's token map)."""
         self._prompt = None
@@ -286,9 +293,11 @@ class GeneralizedVLRCNN_New(nn.Module):
         return ops.mask_prompt_tokens(st["ids"], st["tok_cat"], flags, self.mask_token_id())
 
     @torch.no_grad()
-    def forward_device(self, images, captions, positive_map, max_out=None):
+    def forward_device(self, images, captions, positive_map, max_out=None, img_wh=None):
         """Everything up to (and excluding) the device->host copy: returns the device-resident result dict.
-        ``max_out`` (rows of the fixed-shape detections) defaults to ``self.max_out()`` (from DETECTIONS_PER_IMG)."""
+        ``max_out`` (rows of the fixed-shape detections) defaults to ``self.max_out()`` (from DETECTIONS_PER_IMG).
+        ``img_wh``: optional fp32 [B, 2] device table of the images' (w, h); the clip then reads it instead of
+        ``images.image_sizes``, so a captured graph serves any image sizes at its padded shape."""
         max_out = self.max_out() if max_out is None else int(max_out)
         if self.training:
             raise NotImplementedError("training is SURVEY.md §8f")
@@ -320,7 +329,8 @@ class GeneralizedVLRCNN_New(nn.Module):
                                             "vision_inputs": {"vision": st["vision"], "images": pooled,
                                                               "vision_attention_mask": st["vmask"],
                                                               "batched_pos_category_map": None}})
-        out = self.rpn.forward_flat(pyr16, levels, images.image_sizes, lang["hidden"], lang["masks"], positive_map, max_out)
+        out = self.rpn.forward_flat(pyr16, levels, images.image_sizes, lang["hidden"], lang["masks"], positive_map, max_out,
+                                    img_wh=img_wh)
         out["image_sizes"], out["levels"] = images.image_sizes, levels
         out["pyramid16"], out["lang_hidden"] = pyr16, lang["hidden"]  # inputs of the fusion tower (parity tests read them)
         out["vision_query_gates"] = lang["vision_query_gates"]

@@ -227,26 +227,50 @@ class GroundingDINO(nn.Module):
             vision, vmask, _ = self.query_selector([labels] * B, [all_map] * B, None)
             vision, vmask = vision.float().to(dev).contiguous(), vmask.float().to(dev).contiguous()
         C = self.cfg.MODEL.DYHEAD.NUM_CLASSES - 1
-        self._prompt = dict(key=key, ids=ids.to(dev), token_mask=am.bool().to(dev), self_mask=sam.to(dev), position_ids=pid.to(dev),
-                            bert_mask=sam.float().to(dev).contiguous(), vision=vision, vmask=vmask,
-                            tokmap=ops.make_tokmap(positive_map, C, dev))
+        st = dict(key=key, ids=ids.to(dev), token_mask=am.bool().to(dev), self_mask=sam.to(dev), position_ids=pid.to(dev),
+                  bert_mask=sam.float().to(dev).contiguous(), vision=vision, vmask=vmask, tokmap=ops.make_tokmap(positive_map, C, dev))
+        st["text_geo"] = self.transformer.prepare_text(st["token_mask"], st["position_ids"], st["self_mask"])
+        self._prompt = st
         self._geo = None
-        return self._prompt
+        return st
+
+    def graph_state(self):
+        """The cached tensors a forward with a device size table just read (prompt state with its text geometry, the GCP index
+        and padded-query tables): whoever captures that forward in a CUDA graph keeps this object as long as the graph, because
+        the next prompt or batch size replaces these single-entry caches and would free memory the graph still reads."""
+        from ..language_backbone import modeling_bert_new
+        return (self._prompt,) + modeling_bert_new.cache_entries()
 
     def _image_key(self, image_sizes, padded_hw, level_hw):
         le = self.transformer.level_embed   # folded into the cached level position embeddings: a reloaded checkpoint invalidates them
         return (tuple(tuple(int(v) for v in s) for s in image_sizes), tuple(padded_hw), tuple(level_hw), le.data_ptr(), le._version)
 
+    @staticmethod
+    def _size_table(image_sizes, dev):
+        """[(h, w)] -> fp32 [B, 2] device table of (w, h) rows, uploaded without waiting for the stream."""
+        return ops.upload_async(torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32), dev)
+
     @torch.no_grad()
-    def _level_masks(self, image_sizes, padded_hw, level_hw, B, dev):
-        """Padding masks per level (backbone.py:103-111, groundingdino.py:513-516) and their position embeddings."""
+    def _level_masks(self, img_wh, padded_hw, level_hw):
+        """Padding masks per level (backbone.py:103-111, groundingdino.py:513-516) and their position embeddings, from the
+        fp32 [B, 2] (w, h) device table: the padded-input mask is 1 at rows >= h or columns >= w, built by comparisons on the
+        device, so it reads nothing on the host and a captured graph follows the table."""
         Hp, Wp = padded_hw
-        m = torch.zeros((B, Hp, Wp), dtype=torch.float32, device=dev)
-        for b, (h, w) in enumerate(image_sizes):
-            m[b, int(h):, :] = 1
-            m[b, :, int(w):] = 1
+        dev = img_wh.device
+        rows = torch.arange(Hp, dtype=torch.float32, device=dev).view(1, Hp, 1)
+        cols = torch.arange(Wp, dtype=torch.float32, device=dev).view(1, 1, Wp)
+        m = ((rows >= img_wh[:, 1].view(-1, 1, 1)) | (cols >= img_wh[:, 0].view(-1, 1, 1))).float()
         masks = [torch.nn.functional.interpolate(m[None], size=hw).to(torch.bool)[0] for hw in level_hw]
         return masks, [self.backbone[1](mk) for mk in masks]
+
+    def _image_geometry(self, img_wh, padded_hw, level_hw, st):
+        """The geometry of one forward from the device size table: ``Transformer.prepare_image`` on the level masks, the prompt's
+        cached text half, the level table and the table itself as the detections' (w, h)."""
+        masks, poss = self._level_masks(img_wh, padded_hw, level_hw)
+        geo = {**self.transformer.prepare_image(masks, poss), **st["text_geo"]}
+        geo["levels"] = ops.get_levels(list(level_hw), img_wh.device)
+        geo["img_wh"] = img_wh
+        return geo
 
     @torch.no_grad()
     def _geometry(self, image_sizes, padded_hw, level_hw, B, dev, st):
@@ -255,11 +279,8 @@ class GroundingDINO(nn.Module):
         key = self._image_key(image_sizes, padded_hw, level_hw) + (st["key"],)
         if self._geo is not None and self._geo["key"] == key:
             return self._geo
-        masks, poss = self._level_masks(image_sizes, padded_hw, level_hw, B, dev)
-        geo = self.transformer.prepare(masks, poss, st["token_mask"], st["position_ids"], st["self_mask"])
+        geo = self._image_geometry(self._size_table(image_sizes, dev), padded_hw, level_hw, st)
         geo["key"] = key
-        geo["levels"] = ops.get_levels(list(level_hw), dev)
-        geo["img_wh"] = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32, device=dev)
         self._geo = geo
         return geo
 
@@ -291,8 +312,11 @@ class GroundingDINO(nn.Module):
         return src32, ops.cast_f16(src32), sizes
 
     @torch.no_grad()
-    def forward_device(self, samples, captions, positive_map, all_layers=False, proposals=None):
-        """-> dict(det_packed [B, nq+1, 6] on the device, pred_logits (raw) [B,nq,T], pred_boxes [B,nq,4], ...)."""
+    def forward_device(self, samples, captions, positive_map, all_layers=False, proposals=None, img_wh=None):
+        """-> dict(det_packed [B, nq+1, 6] on the device, pred_logits (raw) [B,nq,T], pred_boxes [B,nq,4], ...).
+        ``img_wh``: optional fp32 [B, 2] device table of the images' (w, h).  When given, the padding masks and the image geometry
+        are computed from it inside the forward (nothing about the sizes is read on the host or cached), so a captured graph
+        serves any image sizes at its padded shape; otherwise the geometry of ``image_sizes`` is cached."""
         if self.training:
             raise NotImplementedError("training is SURVEY.md §8(f2)")
         images = to_image_list(samples, self.cfg.DATALOADER.SIZE_DIVISIBILITY)
@@ -302,7 +326,10 @@ class GroundingDINO(nn.Module):
         B, dev = x.shape[0], x.device
         st = self._prompt_state(captions, positive_map, B, dev)
         src32, src16, sizes = self.visual_features(x)
-        geo = self._geometry(images.image_sizes, tuple(x.shape[-2:]), tuple(sizes), B, dev, st)
+        if img_wh is not None:
+            geo = self._image_geometry(img_wh, tuple(x.shape[-2:]), tuple(sizes), st)
+        else:
+            geo = self._geometry(images.image_sizes, tuple(x.shape[-2:]), tuple(sizes), B, dev, st)
         pooled = ops.avgpool2_levels(src16, geo["levels"]) if st["vision"] is not None else None   # flatten_fpn_features (:432-434)
         bert = self.bert(input_ids=st["ids"], attention_mask=st["bert_mask"], position_ids=st["position_ids"], vision=st["vision"],
                          images=pooled, vision_attention_mask=st["vmask"], batched_pos_category_map=None)
@@ -374,11 +401,11 @@ class GroundingDINO(nn.Module):
         ikey = self._image_key(image_sizes, padded_hw, level_hw)
         cache = self.__dict__.get("_chunk_pass_cache")
         if cache is None or cache["ikey"] != ikey:
-            masks, poss = self._level_masks(image_sizes, padded_hw, level_hw, B, dev)
+            wh = self._size_table(image_sizes, dev)
+            masks, poss = self._level_masks(wh, padded_hw, level_hw)
             img_geo = self.transformer.prepare_image(masks, poss)
             img_geo["levels"] = ops.get_levels(list(level_hw), dev)
-            wh = torch.tensor([[float(w), float(h)] for h, w in image_sizes], dtype=torch.float32)
-            img_geo["img_wh"] = ops.upload_async(wh, dev)
+            img_geo["img_wh"] = wh
             cache = self._chunk_pass_cache = dict(ikey=ikey, img_geo=img_geo, passes={})
         gkey = tuple(st["key"] for st in sts)
         ps = cache["passes"].get(gkey)

@@ -48,6 +48,11 @@ _idx_cache = {}
 _pad_cache = {}
 
 
+def cache_entries():
+    """The current entries of the two caches, for a holder that must keep them alive (a captured CUDA graph reads them)."""
+    return (_idx_cache.get("e"), _pad_cache.get("e"))
+
+
 def sparse_index(attention_mask):
     """[B,V,T] 0/1 mask -> int32 [B,T,S] ascending query indices padded with V (get_index_with_padding_batch :40-63).
     S = the global max count; computing it needs one device->host read, done once per distinct mask tensor.

@@ -375,12 +375,13 @@ class VLDyHeadModule(nn.Module):
 
     @torch.no_grad()
     def forward_flat(self, pyr16, levels, image_sizes, lang_hidden, lang_masks, positive_map, max_out=None, tokmap=None,
-                     class_labels=None):
+                     class_labels=None, img_wh=None):
         """pyr16 [B,N,256] fp16 -> device-resident detections: dict(det [B,max_out,6], num [B], ...).
         ``image_sizes``: the (h, w) of every element, or of the B images when the elements are chunks of them (e = chunk * B + image);
         each element's boxes are clipped to its own image, as the reference's post-processor clips each BoxList.
         ``tokmap`` int32 [B,C,max_tok] (+ ``class_labels`` int32 [B,C]): explicit per-element positive maps (batched prompt
-        chunks) instead of the one ``positive_map`` dict shared by the batch."""
+        chunks) instead of the one ``positive_map`` dict shared by the batch.  ``img_wh``: fp32 [B, 2] device table of (w, h) per
+        image; when given, the clip reads it and ``image_sizes`` is not read."""
         cfg = self.cfg
         if max_out is None:
             max_out = (int(cfg.MODEL.ATSS.DETECTIONS_PER_IMG) + 28 + 31) // 32 * 32
@@ -390,9 +391,12 @@ class VLDyHeadModule(nn.Module):
             if self._tokmap is None or self._tokmap[0] != pkey:
                 self._tokmap = (pkey, ops.make_tokmap(positive_map, cfg.MODEL.DYHEAD.NUM_CLASSES - 1, pyr16.device))
             tokmap = self._tokmap[1]
-        ih, iw = image_sizes[0]
-        if any(tuple(s) != (ih, iw) for s in image_sizes):   # a padded batch: each element clips to its own image size
-            ih, iw = [float(h) for h, _ in image_sizes], [float(w) for _, w in image_sizes]
+        if img_wh is not None:
+            iw, ih = img_wh, None
+        else:
+            ih, iw = image_sizes[0]
+            if any(tuple(s) != (ih, iw) for s in image_sizes):   # a padded batch: each element clips to its own image size
+                ih, iw = [float(h) for h, _ in image_sizes], [float(w) for _, w in image_sizes]
         out = ops.atss_postprocess(r["dot_product_logits"], r["reg_ctr"], tokmap, levels, cfg.MODEL.RPN.ANCHOR_STRIDE,
                                    cfg.MODEL.RPN.ANCHOR_SIZES, self._reg_scales()[:levels.n], iw, ih,
                                    pre_nms_thresh=cfg.MODEL.ATSS.INFERENCE_TH, pre_nms_top_n=cfg.MODEL.ATSS.PRE_NMS_TOP_N,

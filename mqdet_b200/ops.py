@@ -710,12 +710,13 @@ def resize_coeffs(n_in, n_out, device):
     return table
 
 
-def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False, times255=False, want_resized=False):
+def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False, times255=False, want_resized=False, out=None):
     """uint8 [h_i, w_i, 3] CUDA images (RGB) -> fp32 [B, 3, Hp, Wp]: each image resized to ``out_hw`` = (oh, ow) with
     ``xtabs[i]`` = resize_coeffs(w_i, ow) and ``ytabs[i]`` = resize_coeffs(h_i, oh), then / 255, channels reversed (``bgr``),
     x 255 (``times255``), (x - mean) / std, zero beyond (oh, ow) up to ``pad_hw``.  With ``want_resized`` also returns the
     resized uint8 images [B, oh, ow, 3].  ``out_hw`` may also be B per-image sizes [(oh_i, ow_i)] (a padded batch of differently
-    sized images, the tables built for each image's own size); ``want_resized`` then needs them all equal."""
+    sized images, the tables built for each image's own size); ``want_resized`` then needs them all equal.  ``out``: a contiguous
+    fp32 [B, 3, Hp, Wp] tensor on the images' device to write instead of a new one (every element is written)."""
     global launch_count
     B = len(images)
     if B == 0 or len(xtabs) != B or len(ytabs) != B:
@@ -737,7 +738,10 @@ def test_transform(images, xtabs, ytabs, out_hw, pad_hw, mean, std, *, bgr=False
     if want_resized and len(set(sizes)) != 1:
         raise _lib.MqdetError("test_transform: want_resized needs one output size for every image")
     dev = images[0].device
-    out = torch.empty((B, 3, Hp, Wp), dtype=torch.float32, device=dev)
+    if out is None:
+        out = torch.empty((B, 3, Hp, Wp), dtype=torch.float32, device=dev)
+    elif out.dtype != torch.float32 or tuple(out.shape) != (B, 3, Hp, Wp) or not out.is_contiguous() or out.device != dev:
+        raise _lib.MqdetError(f"test_transform: out must be a contiguous fp32 [{B}, 3, {Hp}, {Wp}] tensor on {dev}")
     oh, ow = sizes[0]
     resized = torch.empty((B, oh, ow, 3), dtype=torch.uint8, device=dev) if want_resized else None
     src = (ctypes.c_void_p * B)(*[im.data_ptr() for im in images])
@@ -1090,7 +1094,9 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
     tokmap int32 [C, max_tok] (shared) or [B, C, max_tok] (one positive map per image: batched prompt chunks);
     class_labels int32 [C] / [B, C] or None (label of score column c = c + 1).
     ``img_w`` / ``img_h``: the clip size of every element, or sequences of n per-image sizes (a padded batch of differently sized
-    images); element e clips to size e % n, so a chunked pass (e = chunk * B + image) passes its B image sizes."""
+    images); element e clips to size e % n, so a chunked pass (e = chunk * B + image) passes its B image sizes.  ``img_w`` may
+    also be a CUDA fp32 tensor [n, 2] of (w, h) rows, with ``img_h`` None: the kernel reads the sizes from device memory, so a
+    captured graph clips each replay to what the table holds then."""
     import numpy as np
     global launch_count
     _need_cuda(logits, reg_ctr, tokmap)
@@ -1109,8 +1115,17 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
     stride_h = np.asarray(strides, dtype=np.float32)
     base_h = np.asarray([base_anchor(s, a) for s, a in zip(strides, anchor_sizes)], dtype=np.float32)
     scale_h = np.asarray(reg_scales, dtype=np.float32)
-    wh_h = np.ascontiguousarray(np.stack(np.broadcast_arrays(np.asarray(img_w, dtype=np.float32).reshape(-1),
-                                                             np.asarray(img_h, dtype=np.float32).reshape(-1)), 1))
+    wh_dev = img_w if torch.is_tensor(img_w) and img_w.is_cuda else None
+    if wh_dev is not None:
+        if img_h is not None or wh_dev.dtype != torch.float32 or wh_dev.dim() != 2 or wh_dev.shape[1] != 2 or \
+                not wh_dev.is_contiguous() or wh_dev.device != dev:
+            raise _lib.MqdetError("atss_postprocess: a device size table must be a contiguous fp32 [n, 2] (w, h) tensor on the "
+                                  "logits' device, with img_h None")
+        n_sizes = wh_dev.shape[0]
+    else:
+        wh_h = np.ascontiguousarray(np.stack(np.broadcast_arrays(np.asarray(img_w, dtype=np.float32).reshape(-1),
+                                                                 np.asarray(img_h, dtype=np.float32).reshape(-1)), 1))
+        n_sizes = wh_h.shape[0]
     S = (L * pre_nms_top_n + 255) // 256 * 256
     ws = torch.empty((int(load().mqdet_atss_workspace_bytes(levels.hw_ptr, L, C, B)),), dtype=torch.uint8, device=dev)
     lvl_counts = torch.empty((B, L), dtype=torch.int32, device=dev)
@@ -1120,12 +1135,12 @@ def atss_postprocess(logits, reg_ctr, tokmap, levels, strides, anchor_sizes, reg
     okey = torch.empty((B, S), dtype=torch.int64, device=dev) if want_keys else None
     cb, csc, cl = torch.empty_like(ob), torch.empty_like(osc), torch.empty_like(ol)
     totals = torch.empty((B,), dtype=torch.int32, device=dev)
-    check(load().mqdet_atss_candidates(_ptr(logits), _dt(logits), _ptr(reg_ctr), _ptr(tokmap), tm_stride, _ptr(class_labels),
-                                       lab_stride, C, max_tok, T, levels.hw_ptr, L,
-                                       stride_h.ctypes.data_as(ctypes.c_void_p), base_h.ctypes.data_as(ctypes.c_void_p),
-                                       scale_h.ctypes.data_as(ctypes.c_void_p), B, float(pre_nms_thresh), int(pre_nms_top_n),
-                                       S, wh_h.ctypes.data_as(ctypes.c_void_p), wh_h.shape[0], _ptr(ws), _ptr(lvl_counts), _ptr(ob), _ptr(osc),
-                                       _ptr(ol), _ptr(okey), _ptr(cb), _ptr(csc), _ptr(cl), _ptr(totals), _stream()),
+    entry = load().mqdet_atss_candidates if wh_dev is None else load().mqdet_atss_candidates_sizes_dev
+    wh_ptr = wh_h.ctypes.data_as(ctypes.c_void_p) if wh_dev is None else _ptr(wh_dev)
+    check(entry(_ptr(logits), _dt(logits), _ptr(reg_ctr), _ptr(tokmap), tm_stride, _ptr(class_labels), lab_stride, C, max_tok, T,
+                levels.hw_ptr, L, stride_h.ctypes.data_as(ctypes.c_void_p), base_h.ctypes.data_as(ctypes.c_void_p),
+                scale_h.ctypes.data_as(ctypes.c_void_p), B, float(pre_nms_thresh), int(pre_nms_top_n), S, wh_ptr, n_sizes, _ptr(ws),
+                _ptr(lvl_counts), _ptr(ob), _ptr(osc), _ptr(ol), _ptr(okey), _ptr(cb), _ptr(csc), _ptr(cl), _ptr(totals), _stream()),
           "atss_candidates")
     nws = torch.empty((int(load().mqdet_ml_nms_batched_workspace_bytes(B, S)),), dtype=torch.uint8, device=dev)
     keep = torch.empty((B, S), dtype=torch.int64, device=dev)
