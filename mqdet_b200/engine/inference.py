@@ -23,7 +23,7 @@ Nothing here computes: it is stream / graph / buffer plumbing around ``Generaliz
 ``run_batches`` / ``run_images`` of both engines take the reference's test-loader batches instead: padded batches of differently
 sized images, whose batch size and padded shape change from batch to batch (``engine/batches.py::reference_test_batches``).  They
 keep one CUDA graph per padded batch shape (B, Hp, Wp) in ``ShapeGraphs``; the image sizes are not part of a graph, they travel in a
-device table the forward reads.
+device table the forward reads.  ``ChunkedEngine`` does the same for the chunked many-category forward (LVIS) of either detector.
 """
 import random
 import time
@@ -364,6 +364,125 @@ class GroundingDINOEngine:
         if self.batches is not None:
             self.batches.close()
             self.batches = None
+
+
+class ChunkedEngine:
+    """Chunked evaluation of a many-category vocabulary (LVIS: TEST.CHUNKED_EVALUATION 40 turns 1203 classes into 31 prompts) through
+    CUDA graphs, for either detector (``GeneralizedVLRCNN_New`` or ``GroundingDINO``; dispatched on its ``forward_chunked_device``).
+    The reference evaluates LVIS at TEST.IMS_PER_BATCH 1, every image its own batch at its own padded size; here one graph per
+    padded batch shape holds every pass of every chunk, so an image costs one replay instead of ~780 launches per pass.
+
+        eng = ChunkedEngine(model, chunk_captions, chunk_positive_maps, chunks_per_pass=8)
+        for boxlists in eng.run_batches(image_lists): ...             # padded ImageLists, e.g. one image each
+        for boxlists in eng.run_images(images_u8, index_batches): ... # decoded uint8 + reference_test_batches index lists
+        eng.stats(); eng.close()
+
+    Each BoxList holds an image's per-chunk detections concatenated in chunk order with their global labels: what
+    ``forward_chunked`` returns and the reference's ``concate_box_list`` makes (engine/inference.py:704-706), bit for bit."""
+
+    # Live graphs by default.  A COCO-like set at 800 / 1333 has 43 padded shapes: one side at 800 and the other in 32-pixel steps
+    # up to 1344, both orientations (35), plus the shapes whose long side is capped at 1333 (8).  Measured over all 43 at 31 chunks
+    # of 40 classes, 8 per pass, one image per batch (tools/prof_chunked_engine.py --all-shapes, H100 80GB HBM3, 700 W; DESIGN.md
+    # section 5): 43 captures, no eviction; per graph 8.3 MB allocated and 16-19 MB reserved beyond the staging buffers (the first
+    # few graphs of a run reserve ~110 MB each, later ones reuse the shared pool); peak max_memory_allocated 6.7 GB for
+    # MQ-GroundingDINO-T, 4.0 GB for MQ-GLIP-T.  48 leaves room for a few more shapes at well under 1 GB.
+    MAX_GRAPHS = 48
+
+    def __init__(self, model, chunk_captions, chunk_positive_maps, chunks_per_pass=8, max_graphs=None, *, use_graph=True, warmup=2):
+        if not hasattr(model, "forward_chunked_device"):
+            raise TypeError(f"ChunkedEngine: {type(model).__name__} has no forward_chunked_device")
+        rate = model.text_mask_rate() if hasattr(model, "text_mask_rate") else 0.0
+        if 0 < rate < 1:
+            raise NotImplementedError("VISION_QUERY.TEXT_DROPOUT < 1 with VISION_QUERY.MASK_DURING_INFERENCE: every forward draws new "
+                                      "token masks, which a replayed graph cannot do; use forward_chunked_device")
+        _refuse_multi_gpu("ChunkedEngine")
+        self._refuse_uncached(model)
+        if len(chunk_captions) != len(chunk_positive_maps) or not chunk_captions:
+            raise ValueError("ChunkedEngine: one positive map per chunk caption, at least one chunk")
+        if int(chunks_per_pass) < 1:
+            raise ValueError(f"chunks_per_pass must be >= 1, got {chunks_per_pass}")
+        self.model, self.captions, self.positive_maps = model, list(chunk_captions), list(chunk_positive_maps)
+        self.chunks_per_pass, self.mask_rate = int(chunks_per_pass), rate
+        self.dev = next(model.parameters()).device
+        if self.dev.type != "cuda":
+            raise MqdetError("ChunkedEngine: the model must live on a CUDA device (no CPU fallback)")
+        self.n_chunks = len(self.captions)
+        self.chunk_rows = model.max_out() + 1 if hasattr(model, "max_out") else int(model.num_queries) + 1
+        self.use_graph, self.warmup = bool(use_graph), max(1, int(warmup))
+        self.max_graphs = self.MAX_GRAPHS if max_graphs is None else max_graphs
+        self.batches = None
+
+    @staticmethod
+    def _refuse_uncached(model):
+        # a capture must find every chunk group cached: rebuilding one reads a count on the host and uploads small tables
+        if not getattr(model, "cache_chunk_groups", True):
+            raise NotImplementedError("ChunkedEngine needs model.cache_chunk_groups = True: a graph can only replay chunk-group "
+                                      "state built before its capture")
+
+    def _forward(self, il, wh):
+        pk = self.model.forward_chunked_device(il, self.captions, self.positive_maps, self.chunks_per_pass, img_wh=wh)["det_packed"]
+        return pk.transpose(0, 1).reshape(pk.shape[1], -1, 6)      # [B, n_chunks * rows, 6]
+
+    def _after_replay(self, state):
+        """The draws of the eager chunked forward at TEXT_DROPOUT >= 1, so that Python's random advances as in the reference."""
+        if self.mask_rate > 0:
+            read = state[-1]
+            self.model.draw_chunk_text_masks(read["states"], read["B"], self.mask_rate)
+
+    def _shape_graphs(self):
+        if self.batches is None:
+            self.batches = ShapeGraphs(self.model, self._forward, self.n_chunks * self.chunk_rows,
+                                       lambda packed, sizes: chunked_to_boxlists(packed, sizes, self.n_chunks),
+                                       use_graph=self.use_graph, warmup=self.warmup, max_graphs=self.max_graphs,
+                                       after_replay=self._after_replay)
+        return self.batches
+
+    def run_batches(self, batches):
+        """batches: iterable of ``ImageList`` (pinned-host or device fp32 [B, 3, Hp, Wp] + ``image_sizes``) -> yields list[BoxList] per
+        batch, each equal bit for bit to ``model.forward_chunked(il, ...)``.  One graph per (B, Hp, Wp) (see ``ShapeGraphs``)."""
+        _refuse_multi_gpu("run_batches")
+        self._refuse_uncached(self.model)
+        return self._shape_graphs().run_batches(batches)
+
+    def run_images(self, images_u8, index_batches):
+        """Decoded uint8 HWC RGB images + the index lists of ``reference_test_batches`` -> yields list[BoxList] per index list, resized
+        to the original image sizes; the upload and the test transform run on the copy stream."""
+        _refuse_multi_gpu("run_images")
+        self._refuse_uncached(self.model)
+        return self._shape_graphs().run_images(images_u8, index_batches)
+
+    def stats(self):
+        """Captures, seconds spent in warm-ups and captures, distinct shapes seen, evictions, graphs live."""
+        return self._shape_graphs().stats()
+
+    def close(self):
+        """Drop the graphs."""
+        if self.batches is not None:
+            self.batches.close()
+            self.batches = None
+
+
+def chunked_to_boxlists(packed, image_sizes, n_chunks):
+    """Host packed rows [B, n_chunks * rows, 6] (per image, chunk c's rows at c * rows, its count row last) -> BoxList (mode xyxy,
+    fields labels / scores) per image at its (h, w): the chunks' detections concatenated in chunk order."""
+    from ..structures.bounding_box import BoxList
+    B = packed.shape[0]
+    pk = packed.reshape(B, n_chunks, -1, 6) if n_chunks else None
+    max_out = pk.shape[2] - 1 if n_chunks else 0
+    res = []
+    for b, (h, w) in enumerate(image_sizes):
+        parts = []
+        for c in range(n_chunks):
+            n = int(round(float(pk[b, c, max_out, 0])))
+            if n > max_out:
+                raise MqdetError(f"image {b}, chunk {c}: {n} detections exceed the {max_out}-row result buffer")
+            parts.append(pk[b, c, :n])
+        d = torch.cat(parts) if parts else torch.zeros((0, 6))
+        bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
+        bl.add_field("labels", d[:, 5].long())
+        bl.add_field("scores", d[:, 4].clone())
+        res.append(bl)
+    return res
 
 
 def packed_to_boxlists(packed, image_sizes, max_out):

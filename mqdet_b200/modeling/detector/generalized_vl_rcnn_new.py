@@ -21,6 +21,7 @@ from torch import nn
 from ... import ops
 from ..._lib import MqdetError
 from ...structures.image_list import to_image_list
+from ...utils import reserve_entries
 from ..backbone.fpn import FPN, LastLevelP6P7
 from ..backbone.swint import SwinTransformer
 from ..language_backbone.bert_model_new import BertEncoder
@@ -82,6 +83,8 @@ class GeneralizedVLRCNN_New(nn.Module):
         self.DEBUG = False
         self._prompt = None
         self.overlap_text_prefix = True   # image-independent BERT layers on a second stream next to the visual backbone
+        self.cache_chunk_groups = True    # keep the prompt side of each chunked pass, BERT prefix included (False: rebuild per pass)
+        self._chunk_read = None
         self._side = {}
 
     def _side_stream(self, device):
@@ -148,11 +151,12 @@ class GeneralizedVLRCNN_New(nn.Module):
         return append_to_bank(query_images, labels, query_feats, self.cfg, exclude_similar, max_query_number)
 
     def graph_state(self):
-        """The cached tensors a forward just read (prompt state, the head's token map, the GCP index and padded-query tables):
-        whoever captures that forward in a CUDA graph keeps this object as long as the graph, because the next prompt or batch
-        size replaces these single-entry caches and would free memory the graph still reads."""
+        """The cached tensors a forward just read (prompt state, the head's token map, the GCP index and padded-query tables, and
+        the chunk and chunk-group states of the last chunked forward): whoever captures that forward in a CUDA graph keeps this
+        object as long as the graph, because the next prompt, batch size or chunk grouping replaces or clears these caches and
+        would free memory the graph still reads."""
         from ..language_backbone import modeling_bert_new
-        return (self._prompt, self.rpn._tokmap) + modeling_bert_new.cache_entries()
+        return (self._prompt, self.rpn._tokmap) + modeling_bert_new.cache_entries() + (self._chunk_read,)
 
     def invalidate_prompt_cache(self):
         """Drop everything cached per prompt (token ids, selected queries, masks, the head's token map)."""
@@ -219,6 +223,12 @@ class GeneralizedVLRCNN_New(nn.Module):
         """:402-406 for the images of ``has`` (one has-query list per image) in order: one ``random.random()`` per category,
         drawn for every category -> [len(has)][C] flags, 1 = mask the category's tokens."""
         return [[int(random.random() < rate and h == 1) for h in row] for row in has]
+
+    @classmethod
+    def draw_chunk_text_masks(cls, states, B, rate):
+        """The draws of a chunked forward over B images: the reference's forwards run images outer, chunks inner
+        (inference.py:600-625) -> [B][chunk][C] flags."""
+        return [[cls.draw_text_masks(st["has"], rate)[0] for st in states] for _ in range(B)]
 
     def max_out(self):
         """Rows of the fixed-shape per-image result: DETECTIONS_PER_IMG plus head-room for the reference's `>= kth score`
@@ -362,11 +372,71 @@ class GeneralizedVLRCNN_New(nn.Module):
         toks = [([positive_map[c]] if isinstance(positive_map[c], int) else list(positive_map[c])) for c in cols]
         if len(cache) > 4096:
             cache.clear()
-        st = cache[key] = dict(ids=ids, am=am, vision=vision, vmask=vmask, cols=cols, toks=toks, **tab)
+        st = cache[key] = dict(key=key, ids=ids, am=am, vision=vision, vmask=vmask, cols=cols, toks=toks, **tab)
         return st
 
+    CHUNK_GROUP_CAPACITY = 16      # chunk groups x batch sizes kept (LVIS at 8 chunks per pass: 4 per batch size); more when one
+                                   # forward has more groups (``reserve_entries``)
+
+    def _chunk_group_key(self, sts, B, wkey):
+        return (tuple(st["key"] for st in sts), int(B), wkey)
+
     @torch.no_grad()
-    def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
+    def _chunk_group_state(self, sts, B, dev, key):
+        """The prompt side of one pass of ``forward_chunked_device`` over elements e = chunk * B + image, a function of the chunk
+        group and the batch size only, built once on the device and cached by (chunk keys, B): token ids and attention mask, the
+        vision queries and their token mask zero-padded to the group's largest count (the pad_sequence padding of
+        QuerySelector.forward, query_selector.py:112-116) with the GCP index table of that mask, the head's token map and class
+        labels, and the embeddings + BERT layers before the first GCP block (they read the token ids only), computed at the pass's
+        own element count.  At 0 < TEXT_DROPOUT < 1 every forward masks other ids, so that path has no prefix.  ``key`` (from
+        ``_chunk_group_key``) carries the (data_ptr, _version) of the prefix's weights, so reloaded weights rebuild it; the
+        forward makes room for all its groups before the first (``reserve_entries``), so nothing is evicted here."""
+        from ..language_backbone import modeling_bert_new
+        cache = self.__dict__.setdefault("_chunk_group_cache", {})
+        gs = cache.get(key)
+        if gs is not None and self.cache_chunk_groups:
+            return gs
+        G = len(sts)
+        T = self.cfg.MODEL.LANGUAGE_BACKBONE.MAX_QUERY_LEN
+        rate = sts[0]["mask_rate"]
+
+        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...]
+            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
+
+        gs = dict(ids=per_element([st["ids_masked" if rate >= 1.0 else "ids"] for st in sts]), am=per_element([st["am"] for st in sts]),
+                  vision=None, vmask=None, vidx=None, prefix=None)
+        if 0 < rate < 1.0:
+            gs["tok_cat"] = per_element([st["tok_cat"] for st in sts])
+            gs["n_cats"] = max(len(st["has"][0]) for st in sts)
+        if sts[0]["vision"] is not None:
+            Vmax = max(st["vision"].shape[0] for st in sts)
+            vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
+            vmask = torch.zeros((G, Vmax, T), dtype=torch.float32, device=dev)
+            for g, st in enumerate(sts):
+                vision[g, :st["vision"].shape[0]] = st["vision"]
+                vmask[g, :st["vmask"].shape[0]] = st["vmask"]
+            gs["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
+            gs["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
+            gs["vidx"] = modeling_bert_new.sparse_index(gs["vmask"])
+        Cmax = max(len(st["cols"]) for st in sts)
+        mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
+        tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
+        lab_h = torch.zeros((G, Cmax), dtype=torch.int32)
+        for g, st in enumerate(sts):
+            for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
+                tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
+                lab_h[g, j] = c
+        gs["tokmap"] = ops.upload_async(tok_h, dev).repeat_interleave(B, dim=0).contiguous()
+        gs["class_labels"] = ops.upload_async(lab_h, dev).repeat_interleave(B, dim=0).contiguous()
+        if not self.cache_chunk_groups:
+            return gs
+        if not 0 < rate < 1.0:
+            gs["prefix"] = self.language_backbone.body.model.text_prefix(gs["ids"], gs["am"], output_hidden_states=False)
+        cache[key] = gs
+        return gs
+
+    @torch.no_grad()
+    def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None, img_wh=None):
         """Chunked evaluation of a many-category vocabulary (LVIS: 1203 classes as 31 prompts of 40 classes,
         maskrcnn_benchmark/engine/inference.py:165-283,605-625).  The reference runs the WHOLE model once per chunk and
         concatenates the per-chunk detections; here Swin + FPN run ONCE per image and the chunks travel as extra batch
@@ -374,7 +444,10 @@ class GeneralizedVLRCNN_New(nn.Module):
         ``chunks_per_pass`` chunks at a time.  Score columns of a chunk are its classes in ascending label order and carry
         their own label table (convert_grounding_to_od_logits_v2 semantics, rpn/inference.py:793-824).
         ``chunk_ids``: the subset of chunks THIS rank evaluates (text-column sharding over ranks), default all.
+        ``img_wh``: optional fp32 [B, 2] device table of the images' (w, h); the clip then reads it instead of
+        ``images.image_sizes``, so a captured graph serves any image sizes at its padded shape.
         Returns {"det_packed": [n_chunks_local, B, max_out + 1, 6] device tensor, "chunks": [chunk index ...], ...}."""
+        from ..language_backbone import modeling_bert_new
         if self.training:
             raise NotImplementedError("training is SURVEY.md §8f")
         images = to_image_list(images, self.cfg.DATALOADER.SIZE_DIVISIBILITY)
@@ -383,7 +456,6 @@ class GeneralizedVLRCNN_New(nn.Module):
             raise MqdetError("GeneralizedVLRCNN_New: CUDA images required (no CPU fallback)")
         dev = x.device
         B = x.shape[0]
-        T = self.cfg.MODEL.LANGUAGE_BACKBONE.MAX_QUERY_LEN
         chunk_ids = list(range(len(chunk_captions))) if chunk_ids is None else list(chunk_ids)
         feats = self.backbone.body.forward_flat(x)
         pyr16, levels = self.backbone.fpn.forward_flat([feats[i] for i in (1, 2, 3)])   # ONCE per image, shared by all chunks
@@ -392,72 +464,45 @@ class GeneralizedVLRCNN_New(nn.Module):
         pooled = None
         states = [self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in chunk_ids]
         rate = states[0]["mask_rate"] if states else 0.0
-        if rate > 0:   # vision-only evaluation: the draws of the reference's forwards, images outer, chunks inner (inference.py:600-625)
-            flags = [[self.draw_text_masks(st["has"], rate)[0] for st in states] for _ in range(B)]
-        for p0 in range(0, len(chunk_ids), chunks_per_pass):
+        if rate > 0:   # vision-only evaluation: the draws of the reference's forwards
+            flags = self.draw_chunk_text_masks(states, B, rate)
+        wkey = self.language_backbone.body.model.prefix_weights_key()
+        keys = [self._chunk_group_key(states[p0:p0 + chunks_per_pass], B, wkey) for p0 in range(0, len(chunk_ids), chunks_per_pass)]
+        reserve_entries(self.__dict__.setdefault("_chunk_group_cache", {}), keys, self.CHUNK_GROUP_CAPACITY)
+        groups = []
+        for p0, key in zip(range(0, len(chunk_ids), chunks_per_pass), keys):
             sts = states[p0:p0 + chunks_per_pass]
             G = len(sts)
-            ids = torch.cat([st["ids_masked" if rate >= 1.0 else "ids"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
+            gs = self._chunk_group_state(sts, B, dev, key)
+            groups.append(gs)
+            ids = gs["ids"]
             if 0 < rate < 1.0:
-                Cmax = max(len(st["has"][0]) for st in sts)
-                fl = torch.tensor([flags[b][p0 + g] + [0] * (Cmax - len(flags[b][p0 + g])) for g in range(G) for b in range(B)],
+                C = gs["n_cats"]
+                fl = torch.tensor([flags[b][p0 + g] + [0] * (C - len(flags[b][p0 + g])) for g in range(G) for b in range(B)],
                                   dtype=torch.uint8)
-                tok_cat = torch.cat([st["tok_cat"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
-                ids = ops.mask_prompt_tokens(ids, tok_cat, ops.upload_async(fl, dev), self.mask_token_id())
-            am = torch.cat([st["am"] for st in sts]).repeat_interleave(B, dim=0).contiguous()
-            vision = vmask = None
-            if sts[0]["vision"] is not None:
-                Vmax = max(st["vision"].shape[0] for st in sts)
-                vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
-                vmask = torch.zeros((G, Vmax, T), dtype=torch.float32, device=dev)
-                for g, st in enumerate(sts):   # zero rows = pad_sequence padding of QuerySelector.forward (:112-116)
-                    vision[g, :st["vision"].shape[0]] = st["vision"]
-                    vmask[g, :st["vmask"].shape[0]] = st["vmask"]
-                vision = vision.repeat_interleave(B, dim=0).contiguous()
-                vmask = vmask.repeat_interleave(B, dim=0).contiguous()
+                ids = ops.mask_prompt_tokens(ids, gs["tok_cat"], ops.upload_async(fl, dev), self.mask_token_id())
+            if gs["vision"] is not None:
+                modeling_bert_new.use_sparse_index(gs["vmask"], gs["vidx"])
                 if pooled is None:
                     pooled = ops.avgpool2_levels(pyr16, levels)
-            Cmax = max(len(st["cols"]) for st in sts)
-            mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
-            tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
-            lab_h = torch.zeros((G, Cmax), dtype=torch.int32)
-            for g, st in enumerate(sts):
-                for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
-                    tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
-                    lab_h[g, j] = c
-            tokmap = tok_h.to(dev).repeat_interleave(B, dim=0).contiguous()
-            labels = lab_h.to(dev).repeat_interleave(B, dim=0).contiguous()
-            lang = self.language_backbone.body({"input_ids": ids, "attention_mask": am,
-                                                "vision_inputs": {"vision": vision,
-                                                                  "images": pooled.repeat(G, 1, 1) if vision is not None else None,
-                                                                  "vision_attention_mask": vmask,
+            lang = self.language_backbone.body({"input_ids": ids, "attention_mask": gs["am"], "text_prefix": gs["prefix"],
+                                                "vision_inputs": {"vision": gs["vision"],
+                                                                  "images": pooled.repeat(G, 1, 1) if gs["vision"] is not None else None,
+                                                                  "vision_attention_mask": gs["vmask"],
                                                                   "batched_pos_category_map": None}})
             out = self.rpn.forward_flat(pyr16.repeat(G, 1, 1), levels, images.image_sizes, lang["hidden"], lang["masks"],
-                                        None, max_out, tokmap=tokmap, class_labels=labels)
+                                        None, max_out, tokmap=gs["tokmap"], class_labels=gs["class_labels"], img_wh=img_wh)
             packed[p0:p0 + G] = out["det_packed"].view(G, B, max_out + 1, 6)
+        self._chunk_read = dict(states=states, groups=groups, B=B)
         return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "pyramid16": pyr16}
 
     def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8):
         """-> list[BoxList]: per image, the per-chunk detections concatenated (``BoxList.concate_box_list``,
         structures/bounding_box.py:273-285; engine/inference.py:704-706), chunk order preserved."""
-        from ...structures.bounding_box import BoxList
+        from ...engine.inference import chunked_to_boxlists
         out = self.forward_chunked_device(images, chunk_captions, chunk_positive_maps, chunks_per_pass)
         pk = out["det_packed"].cpu()
-        max_out = pk.shape[2] - 1
-        res = []
-        for b, (h, w) in enumerate(out["image_sizes"]):
-            parts = []
-            for g in range(pk.shape[0]):
-                n = int(round(float(pk[g, b, max_out, 0])))
-                if n > max_out:
-                    raise MqdetError(f"image {b}, chunk {g}: {n} detections exceed the {max_out}-row result buffer")
-                parts.append(pk[g, b, :n])
-            d = torch.cat(parts) if parts else torch.zeros((0, 6))
-            bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
-            bl.add_field("labels", d[:, 5].long())
-            bl.add_field("scores", d[:, 4].clone())
-            res.append(bl)
-        return res
+        return chunked_to_boxlists(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
 
     def forward(self, images, targets=None, captions=None, positive_map=None, greenlight_map=None,
                 return_backbone_features=False):

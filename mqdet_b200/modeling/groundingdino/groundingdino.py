@@ -24,6 +24,7 @@ from torch import nn
 from ... import ops
 from ..._lib import MqdetError
 from ...structures.image_list import to_image_list
+from ...utils import reserve_entries
 from ...utils.weights import f32, w16
 from ..backbone.swint import SwinTransformer
 from ..language_backbone.bert_model_new import bert_base_config
@@ -138,6 +139,8 @@ class GroundingDINO(nn.Module):
                                  sampling_ratio=rb.POOLER_SAMPLING_RATIO, use_v2=True)
         self._prompt = None
         self._geo = None
+        self.cache_chunk_groups = True    # keep the text side of each chunked pass, BERT prefix included (False: rebuild per pass)
+        self._chunk_read = None
         # loss criterion (groundingdino.py:152); no parameters, so the state_dict keys are unchanged
         self.loss_evaluator = SetCriterion(build_matcher(g.matcher), cfg)
 
@@ -236,10 +239,11 @@ class GroundingDINO(nn.Module):
 
     def graph_state(self):
         """The cached tensors a forward with a device size table just read (prompt state with its text geometry, the GCP index
-        and padded-query tables): whoever captures that forward in a CUDA graph keeps this object as long as the graph, because
-        the next prompt or batch size replaces these single-entry caches and would free memory the graph still reads."""
+        and padded-query tables, and the chunk and chunk-group states of the last chunked forward): whoever captures that forward
+        in a CUDA graph keeps this object as long as the graph, because the next prompt, batch size or chunk grouping replaces or
+        clears these caches and would free memory the graph still reads."""
         from ..language_backbone import modeling_bert_new
-        return (self._prompt,) + modeling_bert_new.cache_entries()
+        return (self._prompt,) + modeling_bert_new.cache_entries() + (self._chunk_read,)
 
     def _image_key(self, image_sizes, padded_hw, level_hw):
         le = self.transformer.level_embed   # folded into the cached level position embeddings: a reloaded checkpoint invalidates them
@@ -361,7 +365,8 @@ class GroundingDINO(nn.Module):
 
     # ---- many-category prompts: chunked evaluation (LVIS) --------------------------------------------------------------
     CHUNK_STATE_CAPACITY = 4096    # distinct chunk prompts kept (LVIS: 31)
-    CHUNK_GROUP_CAPACITY = 16      # passes of one image geometry kept (LVIS at 8 chunks per pass: 4)
+    CHUNK_GROUP_CAPACITY = 16      # passes of one image geometry / text groups kept (LVIS at 8 chunks per pass: 4); the text
+                                   # groups grow to one forward's when it has more (``reserve_entries``)
 
     @torch.no_grad()
     def _chunk_state(self, captions, positive_map, dev):
@@ -391,47 +396,61 @@ class GroundingDINO(nn.Module):
                                vision=vision, vmask=vmask, cols=cols, toks=toks)
         return st
 
+    def _chunk_image_geometry(self, img_wh, padded_hw, level_hw):
+        """The image half of a pass's geometry from the fp32 [B, 2] (w, h) device table, for the B images of the batch."""
+        img_geo = self.transformer.prepare_image(*self._level_masks(img_wh, padded_hw, level_hw))
+        img_geo["levels"] = ops.get_levels(list(level_hw), img_wh.device)
+        img_geo["img_wh"] = img_wh
+        return img_geo
+
+    @staticmethod
+    def _repeat_pass_geometry(img_geo, G):
+        """The image half of a pass of G chunks: element e = chunk * B + image."""
+        ps = Transformer.repeat_image_geometry(img_geo, G)
+        ps["levels"] = img_geo["levels"]
+        ps["img_wh"] = img_geo["img_wh"].repeat(G, 1).contiguous()
+        return ps
+
     @torch.no_grad()
-    def _chunk_pass_state(self, image_sizes, padded_hw, level_hw, B, dev, sts):
+    def _chunk_pass_state(self, image_sizes, padded_hw, level_hw, dev, sts, ts):
         """Everything one pass of ``forward_chunked_device`` needs besides the image features, for elements e = chunk * B + image:
-        the image half of the geometry (computed once per image geometry, repeated per chunk) and the text half of
+        the image half of the geometry (computed once per image geometry, repeated per chunk) and the text half ``ts`` of
         ``_chunk_text_state``.  Cached per (image geometry, chunk group); the cache holds the passes of the current image geometry
         only.  Building it uploads nothing that waits for the stream, so a new geometry (the next scale of test-time
         augmentation) does not stall the host."""
         ikey = self._image_key(image_sizes, padded_hw, level_hw)
         cache = self.__dict__.get("_chunk_pass_cache")
         if cache is None or cache["ikey"] != ikey:
-            wh = self._size_table(image_sizes, dev)
-            masks, poss = self._level_masks(wh, padded_hw, level_hw)
-            img_geo = self.transformer.prepare_image(masks, poss)
-            img_geo["levels"] = ops.get_levels(list(level_hw), dev)
-            img_geo["img_wh"] = wh
+            img_geo = self._chunk_image_geometry(self._size_table(image_sizes, dev), padded_hw, level_hw)
             cache = self._chunk_pass_cache = dict(ikey=ikey, img_geo=img_geo, passes={})
         gkey = tuple(st["key"] for st in sts)
         ps = cache["passes"].get(gkey)
-        if ps is not None:
+        if ps is not None and ps["text"] is ts:
             return ps
-        G = len(sts)
-        img_geo = cache["img_geo"]
-        ps = Transformer.repeat_image_geometry(img_geo, G)
-        ps["levels"] = img_geo["levels"]
-        ps["img_wh"] = img_geo["img_wh"].repeat(G, 1).contiguous()
-        ps.update(self._chunk_text_state(sts, B, dev))
+        ps = self._repeat_pass_geometry(cache["img_geo"], len(sts))
+        ps.update(ts)
+        ps["text"] = ts
         if len(cache["passes"]) >= self.CHUNK_GROUP_CAPACITY:
             cache["passes"].clear()
         cache["passes"][gkey] = ps
         return ps
 
+    def _chunk_text_key(self, sts, B, wkey):
+        return (tuple(st["key"] for st in sts), int(B), wkey)
+
     @torch.no_grad()
-    def _chunk_text_state(self, sts, B, dev):
+    def _chunk_text_state(self, sts, B, dev, key):
         """The text half of a pass, a function of the chunk group and the batch size only: the text half of the geometry and the
         BERT inputs of the chunks, the vision queries zero-padded to the group's largest count (the pad_sequence padding of
-        QuerySelector.forward, query_selector.py:112-116), and the per-element class tables.  Cached apart from the image
-        geometry, so every geometry's pass shares these tensors (the GCP index table is built once per vision mask tensor)."""
-        key = (tuple(st["key"] for st in sts), B)
+        QuerySelector.forward, query_selector.py:112-116) with the GCP index table of their mask, the per-element class tables,
+        and the embeddings + BERT layers before the first GCP block (they read the token ids only), computed at the pass's own
+        element count.  Cached apart from the image geometry, so every geometry's pass shares these tensors.  ``key`` (from
+        ``_chunk_text_key``) carries the (data_ptr, _version) of the prefix's weights, so reloaded weights rebuild it; the
+        forward makes room for all its groups before the first (``reserve_entries``), so nothing is evicted here."""
+        from ..language_backbone import modeling_bert_new
         cache = self.__dict__.setdefault("_chunk_text_cache", {})
         ts = cache.get(key)
-        if ts is not None:
+        if ts is not None and self.cache_chunk_groups:
             return ts
         G = len(sts)
 
@@ -443,7 +462,7 @@ class GroundingDINO(nn.Module):
         ts = dict(self.transformer.prepare_text(token_mask, position_ids, self_mask))
         ts["per_element_max"] = True   # each chunk's fusion scores are shifted by their own maximum (one chunk per reference forward)
         ts["ids"], ts["bert_mask"], ts["position_ids"] = per_element([st["ids"] for st in sts]), self_mask.float().contiguous(), position_ids
-        ts["vision"] = ts["vmask"] = None
+        ts["vision"] = ts["vmask"] = ts["vidx"] = ts["prefix"] = None
         if sts[0]["vision"] is not None:
             Vmax = max(st["vision"].shape[0] for st in sts)
             vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
@@ -453,6 +472,7 @@ class GroundingDINO(nn.Module):
                 vmask[g, :st["vmask"].shape[0]] = st["vmask"]
             ts["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
             ts["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
+            ts["vidx"] = modeling_bert_new.sparse_index(ts["vmask"])
         Cmax = max(max(len(st["cols"]) for st in sts), 1)
         mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
         tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
@@ -463,13 +483,14 @@ class GroundingDINO(nn.Module):
                 lab_h[g, j] = c
         ts["tokmap"] = ops.upload_async(tok_h, dev).repeat_interleave(B, dim=0).contiguous()
         ts["class_labels"] = ops.upload_async(lab_h, dev).repeat_interleave(B, dim=0).contiguous()
-        if len(cache) >= self.CHUNK_GROUP_CAPACITY:
-            cache.clear()
+        if not self.cache_chunk_groups:
+            return ts
+        ts["prefix"] = self.bert.text_prefix(ts["ids"], ts["bert_mask"], position_ids=ts["position_ids"], output_hidden_states=False)
         cache[key] = ts
         return ts
 
     @torch.no_grad()
-    def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
+    def forward_chunked_device(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None, img_wh=None):
         """Chunked evaluation of a many-category vocabulary (LVIS: 1203 classes as 31 prompts of 40 classes,
         maskrcnn_benchmark/engine/inference.py:600-660 with TEST.CHUNKED_EVALUATION).  The reference runs the WHOLE model once per
         chunk and image; here Swin-T + ``input_proj`` run ONCE per image batch and the chunks travel as extra batch elements
@@ -478,7 +499,11 @@ class GroundingDINO(nn.Module):
         detections do not depend on which chunks share its pass.  Score columns of a chunk are its classes in ascending label
         order; the emitted labels are the global class ids (ties to the lowest label, as the reference's ``topk(1)`` over the
         zero-filled full-vocabulary scores).  ``chunk_ids``: the subset of chunks THIS rank evaluates, default all.
+        ``img_wh``: optional fp32 [B, 2] device table of the images' (w, h).  When given, the padding masks and the image half of
+        the geometry are computed from it inside the forward (not cached by host sizes), so a captured graph serves any image
+        sizes at its padded shape.
         Returns {"det_packed": [n_chunks_local, B, num_queries + 1, 6] device tensor, "chunks": [chunk index ...], ...}."""
+        from ..language_backbone import modeling_bert_new
         if self.training:
             raise NotImplementedError("training is SURVEY.md §8(f2)")
         if int(chunks_per_pass) < 1:
@@ -496,16 +521,32 @@ class GroundingDINO(nn.Module):
         nq = self.num_queries
         packed = torch.empty((len(chunk_ids), B, nq + 1, 6), dtype=torch.float32, device=dev)
         pooled = None
-        for p0 in range(0, len(chunk_ids), chunks_per_pass):
-            group = chunk_ids[p0:p0 + chunks_per_pass]
-            G = len(group)
-            sts = [self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in group]
-            ps = self._chunk_pass_state(images.image_sizes, tuple(x.shape[-2:]), tuple(sizes), B, dev, sts)
-            if ps["vision"] is not None and pooled is None:
-                pooled = ops.avgpool2_levels(src16, ps["levels"])   # flatten_fpn_features (:432-434)
+        padded_hw = tuple(x.shape[-2:])
+        img_geo = self._chunk_image_geometry(img_wh, padded_hw, tuple(sizes)) if img_wh is not None else None
+        repeated = {}                                     # G -> image half of a pass, with img_wh
+        read = []
+        groups = [[self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in chunk_ids[p0:p0 + chunks_per_pass]]
+                  for p0 in range(0, len(chunk_ids), chunks_per_pass)]
+        wkey = self.bert.prefix_weights_key()
+        keys = [self._chunk_text_key(sts, B, wkey) for sts in groups]
+        reserve_entries(self.__dict__.setdefault("_chunk_text_cache", {}), keys, self.CHUNK_GROUP_CAPACITY)
+        for p0, sts, key in zip(range(0, len(chunk_ids), chunks_per_pass), groups, keys):
+            G = len(sts)
+            ts = self._chunk_text_state(sts, B, dev, key)
+            if img_geo is None:
+                ps = self._chunk_pass_state(images.image_sizes, padded_hw, tuple(sizes), dev, sts, ts)
+            else:
+                if G not in repeated:
+                    repeated[G] = self._repeat_pass_geometry(img_geo, G)
+                ps = {**repeated[G], **ts}
+            read.append((sts, ts))
+            if ps["vision"] is not None:
+                modeling_bert_new.use_sparse_index(ps["vmask"], ps["vidx"])
+                if pooled is None:
+                    pooled = ops.avgpool2_levels(src16, ps["levels"])   # flatten_fpn_features (:432-434)
             bert = self.bert(input_ids=ps["ids"], attention_mask=ps["bert_mask"], position_ids=ps["position_ids"], vision=ps["vision"],
                              images=pooled.repeat(G, 1, 1) if ps["vision"] is not None else None,
-                             vision_attention_mask=ps["vmask"], batched_pos_category_map=None)
+                             vision_attention_mask=ps["vmask"], batched_pos_category_map=None, text_prefix=ps["prefix"])
             h = bert["last_hidden_state"]
             E, T = h.shape[:2]
             enc_text = ops.gemm(ops.cast_f16(h).view(E * T, -1), w16(self.feat_map.weight), bias=f32(self.feat_map.bias),
@@ -514,25 +555,17 @@ class GroundingDINO(nn.Module):
             logits, boxes = self._last_layer_heads(tr, ps["valid_ratios"], ps["text_token_mask"])
             det = ops.gdino_detections(logits, boxes, ps["tokmap"], ps["img_wh"], self.box_threshold, class_labels=ps["class_labels"])
             packed[p0:p0 + G] = det.view(G, B, nq + 1, 6)
+        self._chunk_read = read
         return {"det_packed": packed, "chunks": chunk_ids, "image_sizes": images.image_sizes, "srcs": src32, "pyramid16": src16,
                 "levels": ops.get_levels(sizes, dev)}
 
     def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
         """-> list[BoxList] (mode xyxy, fields labels / scores): per image, the per-chunk detections concatenated in chunk order
         with their global labels (``BoxList.concate_box_list``, engine/inference.py:704-706)."""
-        from ...structures.bounding_box import BoxList
+        from ...engine.inference import chunked_to_boxlists
         out = self.forward_chunked_device(images, chunk_captions, chunk_positive_maps, chunks_per_pass, chunk_ids)
         pk = out["det_packed"].cpu()
-        nq = pk.shape[2] - 1
-        res = []
-        for b, (h, w) in enumerate(out["image_sizes"]):
-            parts = [pk[g, b, :int(pk[g, b, nq, 0])] for g in range(pk.shape[0])]
-            d = torch.cat(parts) if parts else torch.zeros((0, 6))
-            bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
-            bl.add_field("labels", d[:, 5].long())
-            bl.add_field("scores", d[:, 4].clone())
-            res.append(bl)
-        return res
+        return chunked_to_boxlists(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
 
     @torch.no_grad()
     def decoder_outputs_flat(self, out):

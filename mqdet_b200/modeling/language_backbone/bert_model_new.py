@@ -34,10 +34,11 @@ class BertEncoder(nn.Module):
     @torch.no_grad()
     def forward(self, x):
         ids, mask, vi = x["input_ids"], x["attention_mask"], x["vision_inputs"]
-        out = self.model(input_ids=ids, attention_mask=mask, output_hidden_states=True, vision=vi["vision"],
+        # only the last hidden state is read, so a cached prompt prefix needs no per-layer states
+        out = self.model(input_ids=ids, attention_mask=mask, output_hidden_states=False, vision=vi["vision"],
                          images=vi["images"], vision_attention_mask=vi["vision_attention_mask"],
                          batched_pos_category_map=vi.get("batched_pos_category_map"), text_prefix=x.get("text_prefix"))
-        hidden = out.hidden_states[-1]
+        hidden = out.last_hidden_state
         # features = mean of the last N_LAYERS(=1) states / 1; embedded/aggregate are unused by the MHA-B fusion path
         # (bert_model_new.py:61-69) but part of the returned dict — a masked row-scale and a masked mean.
         m = mask.unsqueeze(-1).float()

@@ -68,6 +68,12 @@ def sparse_index(attention_mask):
     return idx
 
 
+def use_sparse_index(attention_mask, idx):
+    """Make ``idx`` (``sparse_index(attention_mask)``, kept by the caller) the current entry: a forward that alternates between
+    several masks (one per pass of a chunked forward) then reads no count on the host, and can be captured in a CUDA graph."""
+    _idx_cache["e"] = (attention_mask, attention_mask._version, idx)
+
+
 def padded_vision(vision):
     """cat(vision, zero row) -> fp32 [B, V+1, D] (modeling_bert_new.py:176-177); cached per vision tensor object."""
     ent = _pad_cache.get("e")
@@ -465,6 +471,12 @@ class QVBertModel(nn.Module):
                 attn_gates.append(blk.attn_gate_value)
             ff_gates.append(blk.ff_gate)
         return {"attn_gates": attn_gates, "ffn_gates": ff_gates}
+
+    def prefix_weights_key(self):
+        """(data_ptr, _version) of every parameter ``text_prefix`` reads: a cached prefix is valid while this is unchanged
+        (``load_state_dict`` and in-place updates bump the versions)."""
+        mods = [self.embeddings] + [self.encoder.layer[i] for i in range(self.encoder.start_qv_layer_index)]
+        return tuple((p.data_ptr(), p._version) for m in mods for p in m.parameters())
 
     @torch.no_grad()
     def text_prefix(self, input_ids, attention_mask=None, token_type_ids=None, position_ids=None, output_hidden_states=True):
