@@ -34,10 +34,72 @@ import torch.distributed as dist
 
 from .. import parallel
 from .._lib import MqdetError
+from ..structures.bounding_box import boxlists_from_packed
 from ..structures.image_list import ImageList
 
 
-class InferenceEngine:
+class _ShapeGraphEngine:
+    """What the three engines share: the checks of the model, and ``run_batches`` / ``run_images`` / ``close`` over the
+    ``ShapeGraphs`` of the engine's forward, built on first use.  The forward is the single-prompt ``forward_device`` of either
+    detector; ``ChunkedEngine`` replaces it with its chunked forward."""
+    n_chunks = 1
+
+    def __init__(self, model, *, use_graph, warmup, max_graphs):
+        # vision-only evaluation: at TEXT_DROPOUT >= 1 the masked ids are part of the captured prompt state
+        self.mask_rate = model.text_mask_rate()
+        if 0 < self.mask_rate < 1:
+            raise NotImplementedError("VISION_QUERY.TEXT_DROPOUT < 1 with VISION_QUERY.MASK_DURING_INFERENCE: every forward draws new "
+                                      "token masks, which a replayed graph cannot do; use the eager forward")
+        self.dev = next(model.parameters()).device
+        if self.dev.type != "cuda":
+            raise MqdetError(f"{type(self).__name__}: the model must live on a CUDA device (no CPU fallback)")
+        self.model = model
+        self.use_graph, self.warmup, self.max_graphs = bool(use_graph), max(1, int(warmup)), max_graphs
+        self.batches = None                     # ShapeGraphs of run_batches / run_images, built on first use
+
+    def _refuse(self, what):
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise NotImplementedError(f"{what} runs on one GPU: under GroupedBatchSampler the ranks' batch counts and tail sizes "
+                                      "differ, so the ranks would not reach the same steps; run it per rank without a process group, "
+                                      "or use run() with one batch shape")
+
+    def _graph_forward(self, il, wh):
+        return self.model.forward_device(il, self.captions, self.positive_map, img_wh=wh)["det_packed"]
+
+    def _after_replay(self, state):
+        """The draws of the eager forward at TEXT_DROPOUT >= 1, so that Python's random advances as in the reference (MQ-GLIP only:
+        MQ-GroundingDINO's rate is 0)."""
+        self.model.draw_text_masks(state[0]["has"], self.mask_rate)
+
+    def _shape_graphs(self):
+        if self.batches is None:
+            self.batches = ShapeGraphs(self.model, self._graph_forward, self.n_chunks, use_graph=self.use_graph, warmup=self.warmup,
+                                       max_graphs=self.max_graphs, after_replay=self._after_replay if self.mask_rate > 0 else None)
+        return self.batches
+
+    def run_batches(self, batches):
+        """batches: iterable of ``ImageList`` (a pinned-host or device fp32 tensor [B, 3, Hp, Wp] + ``image_sizes``), e.g. the
+        reference's test-loader batches -> yields list[BoxList] per batch, each at its image's own size, equal bit for bit to the
+        eager forward (``model(il, ...)`` / ``model.forward_chunked(il, ...)``).  One graph per (B, Hp, Wp), captured the first time
+        that shape comes (see ``ShapeGraphs``); the upload of batch s+1 overlaps the forward of batch s."""
+        self._refuse("run_batches")
+        return self._shape_graphs().run_batches(batches)
+
+    def run_images(self, images_u8, index_batches):
+        """Decoded uint8 HWC RGB images + the index lists of ``reference_test_batches`` -> yields list[BoxList] per index list in
+        original-image coordinates, equal to the test transform followed by the eager forward.  The upload and the test transform run
+        on the copy stream, straight into the staging buffer the next forward reads."""
+        self._refuse("run_images")
+        return self._shape_graphs().run_images(images_u8, index_batches)
+
+    def close(self):
+        """Drop the graphs of ``run_batches`` / ``run_images``."""
+        if self.batches is not None:
+            self.batches.close()
+            self.batches = None
+
+
+class InferenceEngine(_ShapeGraphEngine):
     def __init__(self, model, captions, positive_map, batch_shape=None, image_sizes=None, *, use_graph=True, gather=True, warmup=2,
                  gather_every=8, max_graphs=None):
         """model: GeneralizedVLRCNN_New (eval, on its CUDA device); captions / positive_map: the prompt of the run;
@@ -45,20 +107,9 @@ class InferenceEngine:
         gather_every: steps whose packed results are exchanged by one all-gather (N > 1).
         Without ``batch_shape`` / ``image_sizes`` nothing is captured up front and only ``run_batches`` / ``run_images`` serve;
         ``max_graphs`` bounds their live graphs (default ``ShapeGraphs.MAX_GRAPHS``)."""
-        # vision-only evaluation: at TEXT_DROPOUT >= 1 the masked ids are part of the captured prompt state
-        self.mask_rate = model.text_mask_rate()
-        if 0 < self.mask_rate < 1:
-            raise NotImplementedError("VISION_QUERY.TEXT_DROPOUT < 1 with VISION_QUERY.MASK_DURING_INFERENCE: every forward draws new "
-                                      "token masks, which a replayed graph cannot do; use forward_device")
-        self.model = model
+        super().__init__(model, use_graph=use_graph, warmup=warmup, max_graphs=max_graphs)
         self.captions, self.positive_map = captions, positive_map
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise MqdetError("InferenceEngine: the model must live on a CUDA device (no CPU fallback)")
-        self.warmup, self.max_graphs = max(1, warmup), max_graphs
-        self.batches = None                     # ShapeGraphs of run_batches / run_images, built on first use
         self.graphs, self.outs = [None, None], [None, None]
-        self.use_graph = bool(use_graph)
         self.max_out = model.max_out()
         if batch_shape is None or image_sizes is None:
             if batch_shape is not None or image_sizes is not None:
@@ -197,45 +248,8 @@ class InferenceEngine:
         self.graphs = [None, None]
         self.outs = [None, None]
         self.use_graph = False
-        if self.batches is not None:
-            self.batches.close()
-            self.batches = None
+        super().close()
         torch.cuda.synchronize(self.dev)
-
-    def to_boxlists(self, k=0):
-        """BoxLists of the LOCAL images from pinned host buffer k (waits for that step's device->host copy only)."""
-        self.d2h_done[k].synchronize()
-        return packed_to_boxlists(self.host[k], self.image_sizes, self.max_out)
-
-    def _shape_graphs(self):
-        if self.batches is None:
-            model, caps, pmap = self.model, self.captions, self.positive_map
-            mask_rate = self.mask_rate
-
-            def after_replay(state):   # the draws of the eager forward, so that Python's random advances as in the reference
-                if mask_rate > 0:
-                    model.draw_text_masks(state[0]["has"], mask_rate)
-
-            self.batches = ShapeGraphs(model, lambda il, wh: model.forward_device(il, caps, pmap, img_wh=wh)["det_packed"],
-                                       self.max_out + 1, lambda packed, sizes: packed_to_boxlists(packed, sizes, self.max_out),
-                                       use_graph=self.use_graph, warmup=self.warmup, max_graphs=self.max_graphs,
-                                       after_replay=after_replay)
-        return self.batches
-
-    def run_batches(self, batches):
-        """batches: iterable of ``ImageList`` (a pinned-host or device fp32 tensor [B, 3, Hp, Wp] + ``image_sizes``), e.g. the
-        reference's test-loader batches -> yields list[BoxList] per batch, each at its image's own size, equal bit for bit to
-        ``model(il, ...)``.  One graph per (B, Hp, Wp), captured the first time that shape comes (see ``ShapeGraphs``); the
-        upload of batch s+1 overlaps the forward of batch s."""
-        _refuse_multi_gpu("run_batches")
-        return self._shape_graphs().run_batches(batches)
-
-    def run_images(self, images_u8, index_batches):
-        """Decoded uint8 HWC RGB images + the index lists of ``reference_test_batches`` -> yields list[BoxList] per index list in
-        original-image coordinates, equal to ``predict(model, [images_u8[i] for i in idx], ..., mixed_sizes=True)``.  The upload and
-        the test transform run on the copy stream, straight into the staging buffer the next forward reads."""
-        _refuse_multi_gpu("run_images")
-        return self._shape_graphs().run_images(images_u8, index_batches)
 
     def run(self, batches):
         """batches: iterable of pinned (or pageable) HOST tensors [B, 3, H, W] -> yields list[BoxList] per batch, in order.
@@ -259,13 +273,14 @@ class InferenceEngine:
                 self._launch(k ^ 1)
             if nxt is None:
                 self.flush()  # the tail of the run reaches the other ranks
-            yield self.to_boxlists(k)
+            self.d2h_done[k].synchronize()   # the LOCAL images' packed result is in pinned host buffer k
+            yield boxlists_from_packed(self.host[k], self.image_sizes)
             if nxt is None:
                 return
             k ^= 1
 
 
-class GroundingDINOEngine:
+class GroundingDINOEngine(_ShapeGraphEngine):
     """The same idea for ``mqdet_b200.modeling.groundingdino.groundingdino.GroundingDINO`` (BASELINE config 4): the whole forward
     (≈ 780 kernels at 2 images) recorded once as a CUDA graph over a static input buffer and replayed per batch; pinned host images in,
     ``list[BoxList]`` out, and — with ``torch.distributed`` initialised — ONE all-gather of the packed ``[B, num_queries + 1, 6]`` result
@@ -279,12 +294,8 @@ class GroundingDINOEngine:
                  max_graphs=None):
         """Without ``batch_shape`` / ``image_sizes`` nothing is captured up front and only ``run_batches`` / ``run_images`` serve
         (one graph per padded shape, at most ``max_graphs`` live, default ``ShapeGraphs.MAX_GRAPHS``)."""
-        self.model, self.captions, self.positive_map = model, captions, positive_map
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise MqdetError("GroundingDINOEngine: the model must live on a CUDA device (no CPU fallback)")
-        self.use_graph, self.warmup, self.max_graphs = bool(use_graph), max(1, warmup), max_graphs
-        self.batches = None                     # ShapeGraphs of run_batches / run_images, built on first use
+        super().__init__(model, use_graph=use_graph, warmup=warmup, max_graphs=max_graphs)
+        self.captions, self.positive_map = captions, positive_map
         self.graph, self.static_out, self.note = None, None, "eager launches"
         if batch_shape is None or image_sizes is None:
             if batch_shape is not None or image_sizes is not None:
@@ -329,44 +340,16 @@ class GroundingDINOEngine:
     @torch.no_grad()
     def run(self, host_batches):
         """host_batches: iterable of pinned fp32 [B,3,H,W] tensors -> yields ``list[BoxList]`` of the LOCAL images per batch."""
-        from ..modeling.groundingdino.groundingdino import GroundingDINO
         rank = dist.get_rank() if self.world > 1 else 0
         for hb in host_batches:
             det = self.step_device(hb)
             local = det[rank * self.B:(rank + 1) * self.B] if self.world > 1 else det
             self.host.copy_(local, non_blocking=True)
             torch.cuda.current_stream(self.dev).synchronize()
-            yield GroundingDINO.to_boxlists(self.host, self.image_sizes)
-
-    def _shape_graphs(self):
-        if self.batches is None:
-            from ..modeling.groundingdino.groundingdino import GroundingDINO
-            model, caps, pmap = self.model, self.captions, self.positive_map
-            self.batches = ShapeGraphs(model, lambda il, wh: model.forward_device(il, caps, pmap, img_wh=wh)["det_packed"],
-                                       int(model.num_queries) + 1, GroundingDINO.to_boxlists, use_graph=self.use_graph,
-                                       warmup=self.warmup, max_graphs=self.max_graphs)
-        return self.batches
-
-    def run_batches(self, batches):
-        """``InferenceEngine.run_batches`` for MQ-GroundingDINO: ImageLists in, list[BoxList] per batch out, each equal bit for bit
-        to ``model(il, ...)``; one graph per padded shape, so a dataset of differently sized images (the reference's one image per
-        test batch) replays a graph per shape instead of launching every kernel from the host."""
-        _refuse_multi_gpu("run_batches")
-        return self._shape_graphs().run_batches(batches)
-
-    def run_images(self, images_u8, index_batches):
-        """``InferenceEngine.run_images`` for MQ-GroundingDINO."""
-        _refuse_multi_gpu("run_images")
-        return self._shape_graphs().run_images(images_u8, index_batches)
-
-    def close(self):
-        """Drop the graphs of ``run_batches`` / ``run_images``."""
-        if self.batches is not None:
-            self.batches.close()
-            self.batches = None
+            yield boxlists_from_packed(self.host, self.image_sizes)
 
 
-class ChunkedEngine:
+class ChunkedEngine(_ShapeGraphEngine):
     """Chunked evaluation of a many-category vocabulary (LVIS: TEST.CHUNKED_EVALUATION 40 turns 1203 classes into 31 prompts) through
     CUDA graphs, for either detector (``GeneralizedVLRCNN_New`` or ``GroundingDINO``; dispatched on its ``forward_chunked_device``).
     The reference evaluates LVIS at TEST.IMS_PER_BATCH 1, every image its own batch at its own padded size; here one graph per
@@ -391,121 +374,34 @@ class ChunkedEngine:
     def __init__(self, model, chunk_captions, chunk_positive_maps, chunks_per_pass=8, max_graphs=None, *, use_graph=True, warmup=2):
         if not hasattr(model, "forward_chunked_device"):
             raise TypeError(f"ChunkedEngine: {type(model).__name__} has no forward_chunked_device")
-        rate = model.text_mask_rate() if hasattr(model, "text_mask_rate") else 0.0
-        if 0 < rate < 1:
-            raise NotImplementedError("VISION_QUERY.TEXT_DROPOUT < 1 with VISION_QUERY.MASK_DURING_INFERENCE: every forward draws new "
-                                      "token masks, which a replayed graph cannot do; use forward_chunked_device")
-        _refuse_multi_gpu("ChunkedEngine")
-        self._refuse_uncached(model)
         if len(chunk_captions) != len(chunk_positive_maps) or not chunk_captions:
             raise ValueError("ChunkedEngine: one positive map per chunk caption, at least one chunk")
         if int(chunks_per_pass) < 1:
             raise ValueError(f"chunks_per_pass must be >= 1, got {chunks_per_pass}")
-        self.model, self.captions, self.positive_maps = model, list(chunk_captions), list(chunk_positive_maps)
-        self.chunks_per_pass, self.mask_rate = int(chunks_per_pass), rate
-        self.dev = next(model.parameters()).device
-        if self.dev.type != "cuda":
-            raise MqdetError("ChunkedEngine: the model must live on a CUDA device (no CPU fallback)")
-        self.n_chunks = len(self.captions)
-        self.chunk_rows = model.max_out() + 1 if hasattr(model, "max_out") else int(model.num_queries) + 1
-        self.use_graph, self.warmup = bool(use_graph), max(1, int(warmup))
-        self.max_graphs = self.MAX_GRAPHS if max_graphs is None else max_graphs
-        self.batches = None
+        self.model = model
+        self._refuse("ChunkedEngine")
+        super().__init__(model, use_graph=use_graph, warmup=warmup, max_graphs=self.MAX_GRAPHS if max_graphs is None else max_graphs)
+        self.captions, self.positive_maps = list(chunk_captions), list(chunk_positive_maps)
+        self.chunks_per_pass, self.n_chunks = int(chunks_per_pass), len(self.captions)
 
-    @staticmethod
-    def _refuse_uncached(model):
+    def _refuse(self, what):
+        super()._refuse(what)
         # a capture must find every chunk group cached: rebuilding one reads a count on the host and uploads small tables
-        if not getattr(model, "cache_chunk_groups", True):
+        if not self.model.cache_chunk_groups:
             raise NotImplementedError("ChunkedEngine needs model.cache_chunk_groups = True: a graph can only replay chunk-group "
                                       "state built before its capture")
 
-    def _forward(self, il, wh):
+    def _graph_forward(self, il, wh):
         pk = self.model.forward_chunked_device(il, self.captions, self.positive_maps, self.chunks_per_pass, img_wh=wh)["det_packed"]
         return pk.transpose(0, 1).reshape(pk.shape[1], -1, 6)      # [B, n_chunks * rows, 6]
 
     def _after_replay(self, state):
-        """The draws of the eager chunked forward at TEXT_DROPOUT >= 1, so that Python's random advances as in the reference."""
-        if self.mask_rate > 0:
-            read = state[-1]
-            self.model.draw_chunk_text_masks(read["states"], read["B"], self.mask_rate)
-
-    def _shape_graphs(self):
-        if self.batches is None:
-            self.batches = ShapeGraphs(self.model, self._forward, self.n_chunks * self.chunk_rows,
-                                       lambda packed, sizes: chunked_to_boxlists(packed, sizes, self.n_chunks),
-                                       use_graph=self.use_graph, warmup=self.warmup, max_graphs=self.max_graphs,
-                                       after_replay=self._after_replay)
-        return self.batches
-
-    def run_batches(self, batches):
-        """batches: iterable of ``ImageList`` (pinned-host or device fp32 [B, 3, Hp, Wp] + ``image_sizes``) -> yields list[BoxList] per
-        batch, each equal bit for bit to ``model.forward_chunked(il, ...)``.  One graph per (B, Hp, Wp) (see ``ShapeGraphs``)."""
-        _refuse_multi_gpu("run_batches")
-        self._refuse_uncached(self.model)
-        return self._shape_graphs().run_batches(batches)
-
-    def run_images(self, images_u8, index_batches):
-        """Decoded uint8 HWC RGB images + the index lists of ``reference_test_batches`` -> yields list[BoxList] per index list, resized
-        to the original image sizes; the upload and the test transform run on the copy stream."""
-        _refuse_multi_gpu("run_images")
-        self._refuse_uncached(self.model)
-        return self._shape_graphs().run_images(images_u8, index_batches)
+        read = state[-1]
+        self.model.draw_chunk_text_masks(read["states"], read["B"], self.mask_rate)
 
     def stats(self):
         """Captures, seconds spent in warm-ups and captures, distinct shapes seen, evictions, graphs live."""
         return self._shape_graphs().stats()
-
-    def close(self):
-        """Drop the graphs."""
-        if self.batches is not None:
-            self.batches.close()
-            self.batches = None
-
-
-def chunked_to_boxlists(packed, image_sizes, n_chunks):
-    """Host packed rows [B, n_chunks * rows, 6] (per image, chunk c's rows at c * rows, its count row last) -> BoxList (mode xyxy,
-    fields labels / scores) per image at its (h, w): the chunks' detections concatenated in chunk order."""
-    from ..structures.bounding_box import BoxList
-    B = packed.shape[0]
-    pk = packed.reshape(B, n_chunks, -1, 6) if n_chunks else None
-    max_out = pk.shape[2] - 1 if n_chunks else 0
-    res = []
-    for b, (h, w) in enumerate(image_sizes):
-        parts = []
-        for c in range(n_chunks):
-            n = int(round(float(pk[b, c, max_out, 0])))
-            if n > max_out:
-                raise MqdetError(f"image {b}, chunk {c}: {n} detections exceed the {max_out}-row result buffer")
-            parts.append(pk[b, c, :n])
-        d = torch.cat(parts) if parts else torch.zeros((0, 6))
-        bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
-        bl.add_field("labels", d[:, 5].long())
-        bl.add_field("scores", d[:, 4].clone())
-        res.append(bl)
-    return res
-
-
-def packed_to_boxlists(packed, image_sizes, max_out):
-    """Pinned-host packed rows [B, max_out + 1, 6] (row max_out = (count, ...)) -> BoxList (mode xyxy, fields labels / scores)
-    per image at its (h, w) of ``image_sizes``."""
-    from ..structures.bounding_box import BoxList
-    res = []
-    for b, (h, w) in enumerate(image_sizes):
-        n = int(round(float(packed[b, max_out, 0])))
-        if n > max_out:
-            raise MqdetError(f"image {b}: {n} detections exceed the {max_out}-row result buffer")
-        bl = BoxList(packed[b, :n, :4].clone(), (w, h), mode="xyxy")
-        bl.add_field("labels", packed[b, :n, 5].long())
-        bl.add_field("scores", packed[b, :n, 4].clone())
-        res.append(bl)
-    return res
-
-
-def _refuse_multi_gpu(what):
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        raise NotImplementedError(f"{what} runs on one GPU: under GroupedBatchSampler the ranks' batch counts and tail sizes differ, "
-                                  "so the ranks would not reach the same steps; run it per rank without a process group, or "
-                                  "use run() with one batch shape")
 
 
 class _Graph:
@@ -543,11 +439,12 @@ class ShapeGraphs:
     # the padded shapes of a COCO-sized set at 800 / 1333 (one side at 800, the other in 32-pixel steps, per orientation).
     MAX_GRAPHS = 32
 
-    def __init__(self, model, forward, rows, to_boxlists, *, use_graph=True, warmup=1, max_graphs=None, after_replay=None):
-        """forward(ImageList, img_wh fp32 [B, 2] device) -> packed fp32 [B, rows, 6] device result; to_boxlists(pinned packed
-        [B, rows, 6], image_sizes) -> list[BoxList]; after_replay(graph state): host work an eager forward would also do."""
+    def __init__(self, model, forward, n_chunks=1, *, use_graph=True, warmup=1, max_graphs=None, after_replay=None):
+        """forward(ImageList, img_wh fp32 [B, 2] device) -> packed fp32 [B, n_chunks * (model.max_out() + 1), 6] device result
+        (``boxlists_from_packed`` turns it into BoxLists); after_replay(graph state): host work an eager forward would also do."""
         cfg = model.cfg
-        self.model, self.forward, self.rows, self.to_boxlists = model, forward, int(rows), to_boxlists
+        self.model, self.forward, self.n_chunks = model, forward, int(n_chunks)
+        self.rows = self.n_chunks * (model.max_out() + 1)
         self.after_replay = after_replay
         self.use_graph, self.warmup = bool(use_graph), max(1, int(warmup))
         self.max_graphs = self.MAX_GRAPHS if max_graphs is None else int(max_graphs)
@@ -691,7 +588,7 @@ class ShapeGraphs:
 
     def _results(self, k, B, image_sizes):
         self.d2h_done[k].synchronize()
-        return self.to_boxlists(self.host[k][:B], image_sizes)
+        return boxlists_from_packed(self.host[k][:B], image_sizes, self.n_chunks)
 
     def _run(self, items, stage):
         """Two batches in flight: batch s+1 is staged and its forward queued before the host turns batch s into BoxLists."""

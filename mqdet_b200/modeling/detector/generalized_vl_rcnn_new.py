@@ -20,10 +20,12 @@ from torch import nn
 
 from ... import ops
 from ..._lib import MqdetError
+from ...structures.bounding_box import boxlists_from_packed
 from ...structures.image_list import to_image_list
 from ...utils import reserve_entries
 from ..backbone.fpn import FPN, LastLevelP6P7
 from ..backbone.swint import SwinTransformer
+from ..chunk_prompts import cached_chunk_state, chunk_columns, chunk_group_tables, group_key, per_element, prompt_key
 from ..language_backbone.bert_model_new import BertEncoder
 from ..poolers import Pooler
 from ..query_selector.query_selector import QuerySelector
@@ -163,22 +165,6 @@ class GeneralizedVLRCNN_New(nn.Module):
         self._prompt = None
         self.rpn._tokmap = None
 
-    @staticmethod
-    def _prompt_key(captions, positive_map, B, bank_version):
-        """Content key of a prompt: token ids / caption strings, the positive map's entries, batch size and the query
-        bank version — an in-place edit of ``positive_map`` or a swapped bank is a different prompt."""
-        if isinstance(captions, dict):
-            ids = captions["input_ids"]
-            am = captions["attention_mask"]
-            if ids.is_cuda:  # no device->host sync on the hot path: storage identity + version counters
-                ck = (tuple(ids.shape), ids.data_ptr(), ids._version, am.data_ptr(), am._version)
-            else:
-                ck = (tuple(ids.shape), ids.detach().numpy().tobytes(), am.detach().numpy().tobytes())
-        else:
-            ck = tuple(captions) if isinstance(captions, (list, tuple)) else captions
-        pk = tuple((int(k), tuple(int(t) for t in (v if not isinstance(v, int) else [v]))) for k, v in sorted(positive_map.items()))
-        return (ck, pk, int(B), int(bank_version))
-
     def text_mask_rate(self):
         """Vision-only evaluation (generalized_vl_rcnn_new.py:397-407): VISION_QUERY.TEXT_DROPOUT when MASK_DURING_INFERENCE
         masks prompt tokens at inference, else 0.  Each forward draws one ``random.random()`` per category per image; the
@@ -268,7 +254,7 @@ class GeneralizedVLRCNN_New(nn.Module):
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
         same_objects = st is not None and st["captions"] is captions and st["positive_map"] is positive_map
         rate = self.text_mask_rate()
-        key = self._prompt_key(captions, positive_map, B, bank_version) + (rate,)
+        key = prompt_key(captions, positive_map, B, bank_version) + (rate,)
         if st is not None and st["key"] == key:
             if not same_objects:
                 st["captions"], st["positive_map"] = captions, positive_map
@@ -353,81 +339,46 @@ class GeneralizedVLRCNN_New(nn.Module):
         the token masking tables of vision-only evaluation), cached by content like ``_prompt_state``."""
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
         rate = self.text_mask_rate()
-        key = self._prompt_key(captions, positive_map, 1, bank_version) + (rate,)
-        cache = self.__dict__.setdefault("_chunk_cache", {})
-        st = cache.get(key)
-        if st is not None:
-            return st
-        ids, am = self._tokenize(captions, dev)
-        ids, am = ids[:1], am[:1]
-        vision = vmask = None
-        tab = dict(mask_rate=0.0)
-        if self.query_selector is not None and self.query_selector.query_bank is not None:
-            labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
-            vision, vmask, has = self.query_selector([labels], [all_map], None)
-            vision, vmask = vision[0].float().contiguous(), vmask[0].float().contiguous()
-            if rate > 0:
-                tab = self._mask_tables(ids.contiguous(), all_map, has, rate)
-        cols = sorted(int(k) for k in positive_map)
-        toks = [([positive_map[c]] if isinstance(positive_map[c], int) else list(positive_map[c])) for c in cols]
-        if len(cache) > 4096:
-            cache.clear()
-        st = cache[key] = dict(key=key, ids=ids, am=am, vision=vision, vmask=vmask, cols=cols, toks=toks, **tab)
-        return st
+
+        def build():
+            ids, am = self._tokenize(captions, dev)
+            ids, am = ids[:1], am[:1]
+            vision = vmask = None
+            tab = dict(mask_rate=0.0)
+            if self.query_selector is not None and self.query_selector.query_bank is not None:
+                labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
+                vision, vmask, has = self.query_selector([labels], [all_map], None)
+                vision, vmask = vision[0].float().contiguous(), vmask[0].float().contiguous()
+                if rate > 0:
+                    tab = self._mask_tables(ids.contiguous(), all_map, has, rate)
+            cols, toks = chunk_columns(positive_map)
+            return dict(ids=ids, am=am, vision=vision, vmask=vmask, cols=cols, toks=toks, **tab)
+
+        return cached_chunk_state(self, prompt_key(captions, positive_map, 1, bank_version) + (rate,), build)
 
     CHUNK_GROUP_CAPACITY = 16      # chunk groups x batch sizes kept (LVIS at 8 chunks per pass: 4 per batch size); more when one
                                    # forward has more groups (``reserve_entries``)
-
-    def _chunk_group_key(self, sts, B, wkey):
-        return (tuple(st["key"] for st in sts), int(B), wkey)
 
     @torch.no_grad()
     def _chunk_group_state(self, sts, B, dev, key):
         """The prompt side of one pass of ``forward_chunked_device`` over elements e = chunk * B + image, a function of the chunk
         group and the batch size only, built once on the device and cached by (chunk keys, B): token ids and attention mask, the
-        vision queries and their token mask zero-padded to the group's largest count (the pad_sequence padding of
-        QuerySelector.forward, query_selector.py:112-116) with the GCP index table of that mask, the head's token map and class
-        labels, and the embeddings + BERT layers before the first GCP block (they read the token ids only), computed at the pass's
-        own element count.  At 0 < TEXT_DROPOUT < 1 every forward masks other ids, so that path has no prefix.  ``key`` (from
-        ``_chunk_group_key``) carries the (data_ptr, _version) of the prefix's weights, so reloaded weights rebuild it; the
-        forward makes room for all its groups before the first (``reserve_entries``), so nothing is evicted here."""
-        from ..language_backbone import modeling_bert_new
+        padded vision queries, GCP index and class tables of ``chunk_group_tables``, and the embeddings + BERT layers before the
+        first GCP block (they read the token ids only), computed at the pass's own element count.  At 0 < TEXT_DROPOUT < 1 every
+        forward masks other ids, so that path has no prefix.  ``key`` (``chunk_prompts.group_key``) carries the (data_ptr,
+        _version) of the prefix's weights, so reloaded weights rebuild it; the forward makes room for all its groups before the
+        first (``reserve_entries``), so nothing is evicted here."""
         cache = self.__dict__.setdefault("_chunk_group_cache", {})
         gs = cache.get(key)
         if gs is not None and self.cache_chunk_groups:
             return gs
-        G = len(sts)
-        T = self.cfg.MODEL.LANGUAGE_BACKBONE.MAX_QUERY_LEN
         rate = sts[0]["mask_rate"]
-
-        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...]
-            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
-
-        gs = dict(ids=per_element([st["ids_masked" if rate >= 1.0 else "ids"] for st in sts]), am=per_element([st["am"] for st in sts]),
-                  vision=None, vmask=None, vidx=None, prefix=None)
+        gs = dict(ids=per_element([st["ids_masked" if rate >= 1.0 else "ids"] for st in sts], B),
+                  am=per_element([st["am"] for st in sts], B), prefix=None)
         if 0 < rate < 1.0:
-            gs["tok_cat"] = per_element([st["tok_cat"] for st in sts])
+            gs["tok_cat"] = per_element([st["tok_cat"] for st in sts], B)
             gs["n_cats"] = max(len(st["has"][0]) for st in sts)
-        if sts[0]["vision"] is not None:
-            Vmax = max(st["vision"].shape[0] for st in sts)
-            vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
-            vmask = torch.zeros((G, Vmax, T), dtype=torch.float32, device=dev)
-            for g, st in enumerate(sts):
-                vision[g, :st["vision"].shape[0]] = st["vision"]
-                vmask[g, :st["vmask"].shape[0]] = st["vmask"]
-            gs["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
-            gs["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
-            gs["vidx"] = modeling_bert_new.sparse_index(gs["vmask"])
-        Cmax = max(len(st["cols"]) for st in sts)
-        mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
-        tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
-        lab_h = torch.zeros((G, Cmax), dtype=torch.int32)
-        for g, st in enumerate(sts):
-            for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
-                tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
-                lab_h[g, j] = c
-        gs["tokmap"] = ops.upload_async(tok_h, dev).repeat_interleave(B, dim=0).contiguous()
-        gs["class_labels"] = ops.upload_async(lab_h, dev).repeat_interleave(B, dim=0).contiguous()
+        gs.update(chunk_group_tables(sts, B, dev))
         if not self.cache_chunk_groups:
             return gs
         if not 0 < rate < 1.0:
@@ -467,7 +418,7 @@ class GeneralizedVLRCNN_New(nn.Module):
         if rate > 0:   # vision-only evaluation: the draws of the reference's forwards
             flags = self.draw_chunk_text_masks(states, B, rate)
         wkey = self.language_backbone.body.model.prefix_weights_key()
-        keys = [self._chunk_group_key(states[p0:p0 + chunks_per_pass], B, wkey) for p0 in range(0, len(chunk_ids), chunks_per_pass)]
+        keys = [group_key(states[p0:p0 + chunks_per_pass], B, wkey) for p0 in range(0, len(chunk_ids), chunks_per_pass)]
         reserve_entries(self.__dict__.setdefault("_chunk_group_cache", {}), keys, self.CHUNK_GROUP_CAPACITY)
         groups = []
         for p0, key in zip(range(0, len(chunk_ids), chunks_per_pass), keys):
@@ -499,13 +450,12 @@ class GeneralizedVLRCNN_New(nn.Module):
     def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8):
         """-> list[BoxList]: per image, the per-chunk detections concatenated (``BoxList.concate_box_list``,
         structures/bounding_box.py:273-285; engine/inference.py:704-706), chunk order preserved."""
-        from ...engine.inference import chunked_to_boxlists
         out = self.forward_chunked_device(images, chunk_captions, chunk_positive_maps, chunks_per_pass)
         pk = out["det_packed"].cpu()
-        return chunked_to_boxlists(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
+        return boxlists_from_packed(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
 
     def forward(self, images, targets=None, captions=None, positive_map=None, greenlight_map=None,
                 return_backbone_features=False):
         """Reference signature (:307-314), eval: returns list[BoxList] (fields ``labels``, ``scores``; mode xyxy)."""
         out = self.forward_device(images, captions, positive_map)
-        return self.rpn.to_boxlists(out["det"], out["num"], out["image_sizes"])
+        return boxlists_from_packed(out["det_packed"], out["image_sizes"])

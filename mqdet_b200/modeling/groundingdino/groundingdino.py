@@ -23,10 +23,12 @@ from torch import nn
 
 from ... import ops
 from ..._lib import MqdetError
+from ...structures.bounding_box import boxlists_from_packed
 from ...structures.image_list import to_image_list
 from ...utils import reserve_entries
 from ...utils.weights import f32, w16
 from ..backbone.swint import SwinTransformer
+from ..chunk_prompts import cached_chunk_state, chunk_columns, chunk_group_tables, group_key, per_element, prompt_key
 from ..language_backbone.bert_model_new import bert_base_config
 from ..language_backbone.modeling_bert_new import QVBertModel
 from ..query_selector.query_selector import QuerySelector
@@ -179,6 +181,15 @@ class GroundingDINO(nn.Module):
         torch.save({int(k): v.detach().cpu() for k, v in query_images.items()}, path)
 
     # ---- prompt / geometry state ------------------------------------------------------------------------------------
+    def max_out(self):
+        """Rows of the fixed-shape per-image result: one per decoder query."""
+        return int(self.num_queries)
+
+    def text_mask_rate(self):
+        """0: MQ-GroundingDINO masks no prompt tokens at inference; like the reference it ignores VISION_QUERY.MASK_DURING_INFERENCE
+        (DESIGN.md row f8)."""
+        return 0.0
+
     def load_query_bank(self, query_path):
         self.query_selector.load_query_bank(query_path)
         self._prompt = None
@@ -211,11 +222,8 @@ class GroundingDINO(nn.Module):
     def _prompt_state(self, captions, positive_map, B, dev):
         """Token ids, per-category text masks / position ids (bertwarper.py:271-320), selected vision queries and the class ->
         token table: everything that depends on the prompt only, rebuilt when its CONTENT (or the query bank) changes."""
-        from ..detector.generalized_vl_rcnn_new import GeneralizedVLRCNN_New
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
-        # content key (token ids / strings, positive map entries, batch size, bank version); device-resident ids are keyed by storage
-        # identity + version counter, so the hot path never synchronises to compare prompts
-        key = GeneralizedVLRCNN_New._prompt_key(captions, positive_map, B, bank_version)
+        key = prompt_key(captions, positive_map, B, bank_version)
         st = self._prompt
         if st is not None and st["key"] == key:
             return st
@@ -364,7 +372,6 @@ class GroundingDINO(nn.Module):
         return self.class_embed[-1](hs16, text_dict), boxes
 
     # ---- many-category prompts: chunked evaluation (LVIS) --------------------------------------------------------------
-    CHUNK_STATE_CAPACITY = 4096    # distinct chunk prompts kept (LVIS: 31)
     CHUNK_GROUP_CAPACITY = 16      # passes of one image geometry / text groups kept (LVIS at 8 chunks per pass: 4); the text
                                    # groups grow to one forward's when it has more (``reserve_entries``)
 
@@ -373,28 +380,22 @@ class GroundingDINO(nn.Module):
         """Per-chunk prompt state, cached by content like ``_prompt_state``: token ids, attention mask, per-category self-attention
         mask and restarted position ids (bertwarper.py:271-320), selected vision queries + their token mask, and the chunk's
         classes in ascending label order with their token lists (its score columns)."""
-        from ..detector.generalized_vl_rcnn_new import GeneralizedVLRCNN_New
         bank_version = self.query_selector.bank_version if self.query_selector is not None else 0
-        key = GeneralizedVLRCNN_New._prompt_key(captions, positive_map, 1, bank_version)
-        cache = self.__dict__.setdefault("_chunk_cache", {})
-        st = cache.get(key)
-        if st is not None:
-            return st
-        ids, am = self._tokenize(captions)
-        ids, am = ids[:1, : self.max_text_len].cpu(), am[:1, : self.max_text_len].cpu()
-        sam, pid, _ = generate_masks_with_special_tokens_and_transfer_map({"input_ids": ids}, self.specical_tokens, self.tokenizer)
-        vision = vmask = None
-        if self.cfg.VISION_QUERY.ENABLED and self.query_selector is not None and self.query_selector.query_bank is not None:
-            labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
-            vision, vmask, _ = self.query_selector([labels], [all_map], None)
-            vision, vmask = vision[0].float().to(dev).contiguous(), vmask[0].float().to(dev).contiguous()
-        cols = sorted(int(k) for k in positive_map)
-        toks = [([positive_map[c]] if isinstance(positive_map[c], int) else list(positive_map[c])) for c in cols]
-        if len(cache) >= self.CHUNK_STATE_CAPACITY:
-            cache.clear()
-        st = cache[key] = dict(key=key, ids=ids.to(dev), token_mask=am.bool().to(dev), self_mask=sam.to(dev), position_ids=pid.to(dev),
-                               vision=vision, vmask=vmask, cols=cols, toks=toks)
-        return st
+
+        def build():
+            ids, am = self._tokenize(captions)
+            ids, am = ids[:1, : self.max_text_len].cpu(), am[:1, : self.max_text_len].cpu()
+            sam, pid, _ = generate_masks_with_special_tokens_and_transfer_map({"input_ids": ids}, self.specical_tokens, self.tokenizer)
+            vision = vmask = None
+            if self.cfg.VISION_QUERY.ENABLED and self.query_selector is not None and self.query_selector.query_bank is not None:
+                labels, all_map = self.get_labels_and_maps_from_positive_map(positive_map)
+                vision, vmask, _ = self.query_selector([labels], [all_map], None)
+                vision, vmask = vision[0].float().to(dev).contiguous(), vmask[0].float().to(dev).contiguous()
+            cols, toks = chunk_columns(positive_map)
+            return dict(ids=ids.to(dev), token_mask=am.bool().to(dev), self_mask=sam.to(dev), position_ids=pid.to(dev),
+                        vision=vision, vmask=vmask, cols=cols, toks=toks)
+
+        return cached_chunk_state(self, prompt_key(captions, positive_map, 1, bank_version), build)
 
     def _chunk_image_geometry(self, img_wh, padded_hw, level_hw):
         """The image half of a pass's geometry from the fp32 [B, 2] (w, h) device table, for the B images of the batch."""
@@ -435,54 +436,25 @@ class GroundingDINO(nn.Module):
         cache["passes"][gkey] = ps
         return ps
 
-    def _chunk_text_key(self, sts, B, wkey):
-        return (tuple(st["key"] for st in sts), int(B), wkey)
-
     @torch.no_grad()
     def _chunk_text_state(self, sts, B, dev, key):
         """The text half of a pass, a function of the chunk group and the batch size only: the text half of the geometry and the
-        BERT inputs of the chunks, the vision queries zero-padded to the group's largest count (the pad_sequence padding of
-        QuerySelector.forward, query_selector.py:112-116) with the GCP index table of their mask, the per-element class tables,
-        and the embeddings + BERT layers before the first GCP block (they read the token ids only), computed at the pass's own
-        element count.  Cached apart from the image geometry, so every geometry's pass shares these tensors.  ``key`` (from
-        ``_chunk_text_key``) carries the (data_ptr, _version) of the prefix's weights, so reloaded weights rebuild it; the
+        BERT inputs of the chunks, the padded vision queries, GCP index and class tables of ``chunk_group_tables``, and the
+        embeddings + BERT layers before the first GCP block (they read the token ids only), computed at the pass's own element
+        count.  Cached apart from the image geometry, so every geometry's pass shares these tensors.  ``key``
+        (``chunk_prompts.group_key``) carries the (data_ptr, _version) of the prefix's weights, so reloaded weights rebuild it; the
         forward makes room for all its groups before the first (``reserve_entries``), so nothing is evicted here."""
-        from ..language_backbone import modeling_bert_new
         cache = self.__dict__.setdefault("_chunk_text_cache", {})
         ts = cache.get(key)
         if ts is not None and self.cache_chunk_groups:
             return ts
-        G = len(sts)
-
-        def per_element(ts):   # [1, ...] per chunk -> [G * B, ...], element e = chunk * B + image
-            return torch.cat(ts).repeat_interleave(B, dim=0).contiguous()
-
-        token_mask = per_element([st["token_mask"] for st in sts])
-        self_mask, position_ids = per_element([st["self_mask"] for st in sts]), per_element([st["position_ids"] for st in sts])
+        token_mask = per_element([st["token_mask"] for st in sts], B)
+        self_mask, position_ids = per_element([st["self_mask"] for st in sts], B), per_element([st["position_ids"] for st in sts], B)
         ts = dict(self.transformer.prepare_text(token_mask, position_ids, self_mask))
         ts["per_element_max"] = True   # each chunk's fusion scores are shifted by their own maximum (one chunk per reference forward)
-        ts["ids"], ts["bert_mask"], ts["position_ids"] = per_element([st["ids"] for st in sts]), self_mask.float().contiguous(), position_ids
-        ts["vision"] = ts["vmask"] = ts["vidx"] = ts["prefix"] = None
-        if sts[0]["vision"] is not None:
-            Vmax = max(st["vision"].shape[0] for st in sts)
-            vision = torch.zeros((G, Vmax, sts[0]["vision"].shape[1]), dtype=torch.float32, device=dev)
-            vmask = torch.zeros((G, Vmax, sts[0]["vmask"].shape[1]), dtype=torch.float32, device=dev)
-            for g, st in enumerate(sts):
-                vision[g, :st["vision"].shape[0]] = st["vision"]
-                vmask[g, :st["vmask"].shape[0]] = st["vmask"]
-            ts["vision"] = vision.repeat_interleave(B, dim=0).contiguous()
-            ts["vmask"] = vmask.repeat_interleave(B, dim=0).contiguous()
-            ts["vidx"] = modeling_bert_new.sparse_index(ts["vmask"])
-        Cmax = max(max(len(st["cols"]) for st in sts), 1)
-        mt = max(max((len(t) for t in st["toks"]), default=1) for st in sts)
-        tok_h = torch.full((G, Cmax, mt), -1, dtype=torch.int32)
-        lab_h = torch.zeros((G, Cmax), dtype=torch.int32)
-        for g, st in enumerate(sts):
-            for j, (c, tk) in enumerate(zip(st["cols"], st["toks"])):
-                tok_h[g, j, :len(tk)] = torch.tensor(tk, dtype=torch.int32)
-                lab_h[g, j] = c
-        ts["tokmap"] = ops.upload_async(tok_h, dev).repeat_interleave(B, dim=0).contiguous()
-        ts["class_labels"] = ops.upload_async(lab_h, dev).repeat_interleave(B, dim=0).contiguous()
+        ts["ids"], ts["bert_mask"], ts["position_ids"] = per_element([st["ids"] for st in sts], B), self_mask.float().contiguous(), position_ids
+        ts["prefix"] = None
+        ts.update(chunk_group_tables(sts, B, dev))
         if not self.cache_chunk_groups:
             return ts
         ts["prefix"] = self.bert.text_prefix(ts["ids"], ts["bert_mask"], position_ids=ts["position_ids"], output_hidden_states=False)
@@ -528,7 +500,7 @@ class GroundingDINO(nn.Module):
         groups = [[self._chunk_state(chunk_captions[c], chunk_positive_maps[c], dev) for c in chunk_ids[p0:p0 + chunks_per_pass]]
                   for p0 in range(0, len(chunk_ids), chunks_per_pass)]
         wkey = self.bert.prefix_weights_key()
-        keys = [self._chunk_text_key(sts, B, wkey) for sts in groups]
+        keys = [group_key(sts, B, wkey) for sts in groups]
         reserve_entries(self.__dict__.setdefault("_chunk_text_cache", {}), keys, self.CHUNK_GROUP_CAPACITY)
         for p0, sts, key in zip(range(0, len(chunk_ids), chunks_per_pass), groups, keys):
             G = len(sts)
@@ -562,10 +534,9 @@ class GroundingDINO(nn.Module):
     def forward_chunked(self, images, chunk_captions, chunk_positive_maps, chunks_per_pass=8, chunk_ids=None):
         """-> list[BoxList] (mode xyxy, fields labels / scores): per image, the per-chunk detections concatenated in chunk order
         with their global labels (``BoxList.concate_box_list``, engine/inference.py:704-706)."""
-        from ...engine.inference import chunked_to_boxlists
         out = self.forward_chunked_device(images, chunk_captions, chunk_positive_maps, chunks_per_pass, chunk_ids)
         pk = out["det_packed"].cpu()
-        return chunked_to_boxlists(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
+        return boxlists_from_packed(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), out["image_sizes"], pk.shape[0])
 
     @torch.no_grad()
     def decoder_outputs_flat(self, out):
@@ -600,25 +571,10 @@ class GroundingDINO(nn.Module):
         return {"pred_logits": logits[L - 1], "pred_boxes": boxes[L - 1],
                 "aux_outputs": [{"pred_logits": logits[k], "pred_boxes": boxes[k]} for k in range(L - 1)]}
 
-    @staticmethod
-    def to_boxlists(packed, image_sizes):
-        """One device->host copy of the packed result, then BoxList(mode xyxy, fields labels / scores) per image."""
-        from ...structures.bounding_box import BoxList
-        h = packed.cpu()
-        nq = h.shape[1] - 1
-        res = []
-        for b, (ih, iw) in enumerate(image_sizes):
-            k = int(h[b, nq, 0])
-            bl = BoxList(h[b, :k, :4].clone(), (iw, ih), mode="xyxy")
-            bl.add_field("labels", h[b, :k, 5].long())
-            bl.add_field("scores", h[b, :k, 4].clone())
-            res.append(bl)
-        return res
-
     def forward(self, samples, targets=None, **kw):
         """Reference signature (groundingdino.py:447): eval -> list[BoxList] (or (result, srcs) with return_backbone_features)."""
         out = self.forward_device(samples, kw["captions"], kw["positive_map"])
-        res = self.to_boxlists(out["det_packed"], out["image_sizes"])
+        res = boxlists_from_packed(out["det_packed"], out["image_sizes"])
         if kw.get("return_backbone_features", False):
             B = out["srcs"].shape[0]
             off, maps = 0, []

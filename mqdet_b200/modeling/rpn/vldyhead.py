@@ -17,6 +17,7 @@ from torch import nn
 
 from ... import ops
 from ..._lib import MqdetError
+from ...structures.bounding_box import boxlists_from_packed
 from ...utils.fuse_helper import BiAttentionBlockForCheckpoint, _flatten_levels, _split_levels
 from ...utils.weights import f32, w16
 from ..language_backbone.modeling_bert_new import BertLayer
@@ -450,24 +451,6 @@ class VLDyHeadModule(nn.Module):
             raise ValueError(f"positive_map has {positive_map.shape[0]} rows for {off} GT boxes")
         return {"boxes": boxes, "labels": labels, "count": torch.tensor(counts, dtype=torch.int32).to(device), "tokens": tokens}
 
-    @staticmethod
-    def to_boxlists(det, num, image_sizes):
-        """One device->host copy of the fixed-shape result, then BoxList(mode xyxy, fields labels/scores) per image."""
-        from ...structures.bounding_box import BoxList
-        det_h = det.cpu()
-        num_h = num.cpu()
-        res = []
-        for b, (h, w) in enumerate(image_sizes):
-            k = int(num_h[b])
-            if k > det_h.shape[1]:  # never clip silently: kept rows are in candidate (level-major) order, not score order
-                raise MqdetError(f"image {b}: {k} detections kept (score ties at the DETECTIONS_PER_IMG cut) exceed the "
-                                 f"{det_h.shape[1]}-row result buffer; pass a larger max_out")
-            bl = BoxList(det_h[b, :k, :4].clone(), (w, h), mode="xyxy")
-            bl.add_field("labels", det_h[b, :k, 5].long())
-            bl.add_field("scores", det_h[b, :k, 4].clone())
-            res.append(bl)
-        return res
-
     @torch.no_grad()
     def forward(self, images, features, targets=None, language_dict_features=None, positive_map=None, captions=None,
                 swint_feature_c4=None):
@@ -489,4 +472,4 @@ class VLDyHeadModule(nn.Module):
         out = self.forward_flat(v16, levels, sizes, language_dict_features["hidden"], language_dict_features["masks"],
                                 positive_map)
         language_dict_features["hidden"] = out["head"]["hidden"]
-        return self.to_boxlists(out["det"], out["num"], sizes), {}, None
+        return boxlists_from_packed(out["det_packed"], sizes), {}, None

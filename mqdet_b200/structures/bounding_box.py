@@ -2,7 +2,8 @@
 
 Only the part of the interface that crosses the hot-path boundary: construction, per-box fields, indexing, device moves,
 xyxy <-> xywh with the reference's inclusive-pixel (+1) convention, resizing, clipping, area.  The reference's class is a superset
-and can be passed wherever this one is accepted; tests/test_host_cpu.py pins the shared behaviour against it.
+and can be passed wherever this one is accepted; tests/test_host_cpu.py pins the shared behaviour against it.  ``boxlists_from_packed``
+turns the detectors' packed fixed-shape results into BoxLists.
 """
 import torch
 
@@ -108,3 +109,30 @@ class BoxList(object):
     def __repr__(self):
         return "BoxList(num_boxes={}, image_width={}, image_height={}, mode={})".format(len(self), self.size[0],
                                                                                          self.size[1], self.mode)
+
+
+def boxlists_from_packed(packed, image_sizes, n_chunks=1):
+    """Packed detections fp32 [B, n_chunks * rows, 6], on the host or the device -> one BoxList per image at its (h, w) of
+    ``image_sizes``, mode xyxy, fields ``labels`` then ``scores``.  Per image, chunk c holds rows c * rows .. (c + 1) * rows - 1:
+    its detections (x1, y1, x2, y2, score, label), then a count row (count, ...); the chunks' detections are concatenated in chunk
+    order.  One device->host copy.  A count above its chunk's rows - 1 is an error, never a silent truncation: the rows kept are
+    in candidate order, not score order."""
+    from .._lib import MqdetError
+    pk = packed.cpu()
+    pk = pk.reshape(pk.shape[0], n_chunks, -1, 6)
+    n_rows = pk.shape[2] - 1
+    res = []
+    for b, (h, w) in enumerate(image_sizes):
+        parts = []
+        for c in range(n_chunks):
+            n = int(round(float(pk[b, c, n_rows, 0])))
+            if n > n_rows:
+                where = f"image {b}, chunk {c}" if n_chunks > 1 else f"image {b}"
+                raise MqdetError(f"{where}: {n} detections exceed the {n_rows}-row result buffer")
+            parts.append(pk[b, c, :n])
+        d = torch.cat(parts) if n_chunks > 1 else parts[0]
+        bl = BoxList(d[:, :4].clone(), (w, h), mode="xyxy")
+        bl.add_field("labels", d[:, 5].long())
+        bl.add_field("scores", d[:, 4].clone())
+        res.append(bl)
+    return res

@@ -1,8 +1,15 @@
 """CPU: the host side of ``ChunkedEngine`` — the per-image concatenation of the packed chunk rows (what ``forward_chunked`` and the
-reference's ``concate_box_list`` return) and the refusals made before anything touches a device."""
+reference's ``concate_box_list`` return), the decoding of single-prompt results, the per-pass tables of a chunk group
+(tests/hostlogic/chunk_tables_case.py) and the refusals made before anything touches a device."""
+import os
+import subprocess
+import sys
+
 import pytest
 import torch
 import torch.distributed as dist
+
+from util import ROOT
 
 
 def _packed(counts, rows=5, seed=0):
@@ -18,12 +25,12 @@ def _packed(counts, rows=5, seed=0):
     return pk.view(B, n * rows, 6)
 
 
-def test_chunked_to_boxlists_concatenates_in_chunk_order():
-    from mqdet_b200.engine.inference import chunked_to_boxlists
+def test_boxlists_from_packed_concatenates_in_chunk_order():
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
     counts = [[2, 0, 4], [0, 0, 1]]
     pk = _packed(counts)
     sizes = [(120, 200), (90, 64)]
-    res = chunked_to_boxlists(pk, sizes, 3)
+    res = boxlists_from_packed(pk, sizes, 3)
     full = pk.view(2, 3, 5, 6)
     for b, bl in enumerate(res):
         want = torch.cat([full[b, c, :counts[b][c]] for c in range(3)])
@@ -33,11 +40,40 @@ def test_chunked_to_boxlists_concatenates_in_chunk_order():
     assert res[0].get_field("labels").tolist() == [1, 2, 21, 22, 23, 24]
 
 
-def test_chunked_to_boxlists_refuses_an_overfull_chunk():
+@pytest.mark.parametrize("rows", [5, 101], ids=["one_chunk", "gdino_num_queries_plus_one"])
+def test_boxlists_from_packed_one_chunk(rows):
+    """A single-prompt result [B, rows, 6], MQ-GLIP's max_out + 1 or MQ-GroundingDINO's num_queries + 1 rows: each image's first
+    count rows, fields labels then scores, each a copy rather than a view of the (reused) packed buffer."""
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
+    counts = [[3], [0], [rows - 1]]
+    pk = _packed(counts, rows=rows, seed=1)
+    sizes = [(120, 200), (90, 64), (33, 47)]
+    res = boxlists_from_packed(pk, sizes)
+    for b, bl in enumerate(res):
+        n = counts[b][0]
+        assert bl.size == (sizes[b][1], sizes[b][0]) and bl.mode == "xyxy" and len(bl) == n
+        assert bl.fields() == ["labels", "scores"]
+        assert torch.equal(bl.bbox, pk[b, :n, :4]) and torch.equal(bl.get_field("scores"), pk[b, :n, 4])
+        assert torch.equal(bl.get_field("labels"), pk[b, :n, 5].long())
+    kept = [bl.bbox.clone() for bl in res]
+    pk.zero_()
+    assert all(torch.equal(bl.bbox, k) for bl, k in zip(res, kept))
+
+
+def test_boxlists_from_packed_refuses_an_overfull_result():
     from mqdet_b200._lib import MqdetError
-    from mqdet_b200.engine.inference import chunked_to_boxlists
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
     with pytest.raises(MqdetError, match="chunk 1: 5 detections exceed the 4-row"):
-        chunked_to_boxlists(_packed([[1, 5]]), [(10, 10)], 2)
+        boxlists_from_packed(_packed([[1, 5]]), [(10, 10)], 2)
+    with pytest.raises(MqdetError, match="image 1: 5 detections exceed the 4-row"):
+        boxlists_from_packed(_packed([[1], [5]]), [(10, 10), (10, 10)])
+
+
+def test_chunk_group_tables_host_logic():
+    env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "hostlogic", "chunk_tables_case.py")], capture_output=True,
+                       text=True, timeout=600, env=env, cwd=ROOT)
+    assert r.returncode == 0 and "PASS chunk_tables" in r.stdout, (r.stdout[-1500:], r.stderr[-3000:])
 
 
 class _Stub(torch.nn.Module):

@@ -98,6 +98,32 @@ def test_cached_group_state_and_prefix_equal_a_rebuild_per_pass(case, dev):
     assert int(want[:, :, -1, 0].min()) > 0
 
 
+def test_an_empty_chunk_detects_nothing(case, dev):
+    """A chunk with an empty positive map gets one score column without tokens, so it detects nothing, in a pass of its own or
+    next to another chunk, and the other chunks' rows do not change; the engine replays such a pass as eager runs it.  Without a
+    query bank, since the query selector has no class to pick queries for."""
+    from mqdet_b200.engine.inference import ChunkedEngine
+    kind, model, caps, pmaps = case
+    il = _one_image_batches(kind, dev, [(150, 203)])[0]
+    qs = model.query_selector
+    bank = qs.query_bank
+    qs.query_bank, qs.bank_version = None, qs.bank_version + 1
+    try:
+        want = model.forward_chunked_device(il, caps[:2], pmaps[:2], 1)["det_packed"].clone()
+        assert int(want[:, :, -1, 0].sum()) > 0
+        caps3, pmaps3 = [caps[0], caps[0], caps[1]], [pmaps[0], {}, pmaps[1]]
+        for cpp in (1, 2):
+            got = model.forward_chunked_device(il, caps3, pmaps3, cpp)["det_packed"]
+            assert int(got[1, 0, -1, 0]) == 0, cpp
+            if cpp == 1:
+                assert torch.equal(got[[0, 2]], want)
+        eng = ChunkedEngine(model, caps3, pmaps3, chunks_per_pass=1)
+        _same(list(eng.run_batches([il]))[0], model.forward_chunked(il, caps3, pmaps3, 1), f"{kind} with an empty chunk")
+        eng.close()
+    finally:
+        qs.set_query_bank(bank)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # 3-7, 9. ChunkedEngine
 # ---------------------------------------------------------------------------------------------------------------------

@@ -283,7 +283,8 @@ def test_groundingdino_forward_vs_oracle(dev):
     assert torch.equal(torch.isfinite(f["pred_logits"]).cpu(), fin)
     assert_close(torch.where(fin, f["pred_logits"].cpu(), torch.zeros(())), torch.where(fin, ref["pred_logits"], torch.zeros(())), 1e-2,
                  "gdino: class logits (oracle's selection)", defer=errs)
-    res = model.to_boxlists(out["det_packed"], out["image_sizes"])
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
+    res = boxlists_from_packed(out["det_packed"], out["image_sizes"])
     n, n_ref = [len(r) for r in res], [d[0].shape[0] for d in ref["detections"]]
     _record("forward_small", {"errors": errs, "detections": n, "oracle_detections": n_ref, "selection_overlap": overlap})
     assert not errs, errs
@@ -394,6 +395,7 @@ def test_groundingdino_engine_graph_replay_equals_eager(dev):
     """GroundingDINOEngine (CUDA-graph replay over a static input buffer, pinned host batches in, list[BoxList] out) returns exactly
     what the eager forward returns, for two different batches through the same captured graph."""
     from mqdet_b200.engine.inference import GroundingDINOEngine
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
     from mqdet_b200.structures.image_list import ImageList
     from oracle import synth
     B, h, w, el, dl, nq = 2, 150, 203, 1, 1, 50
@@ -406,7 +408,7 @@ def test_groundingdino_engine_graph_replay_equals_eager(dev):
     assert eng.graph is not None, eng.note
     got = list(eng.run([img.pin_memory(), img2.pin_memory(), img.pin_memory()]))
     for x, res in zip((img, img2, img), got):
-        ref = model.to_boxlists(model.forward_device(ImageList(x.to(dev), [(h, w)] * B), caps, pmap)["det_packed"], [(h, w)] * B)
+        ref = boxlists_from_packed(model.forward_device(ImageList(x.to(dev), [(h, w)] * B), caps, pmap)["det_packed"], [(h, w)] * B)
         for a, b in zip(res, ref):
             assert len(a) == len(b) and torch.equal(a.bbox, b.bbox) and torch.equal(a.get_field("scores"), b.get_field("scores"))
             assert torch.equal(a.get_field("labels"), b.get_field("labels"))

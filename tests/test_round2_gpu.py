@@ -259,8 +259,9 @@ def test_detections_per_img_300_and_packed_result(dev):
     # a too-small result buffer is an error, never a silent truncation
     from mqdet_b200._lib import MqdetError
     small = model.forward_device(il, caps, pmap, max_out=64)
-    with pytest.raises(MqdetError):
-        model.rpn.to_boxlists(small["det"], small["num"], [(h, w)] * B)
+    from mqdet_b200.structures.bounding_box import boxlists_from_packed
+    with pytest.raises(MqdetError, match="exceed the 64-row result buffer"):
+        boxlists_from_packed(small["det_packed"], [(h, w)] * B)
 
 
 def test_prompt_cache_invalidation(dev):

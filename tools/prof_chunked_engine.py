@@ -8,7 +8,7 @@ other from 800 to 1333 in 32-pixel steps, both orientations, plus originals whos
 the capture pass shows whether the default graph limit holds them all, and what they hold in memory.
 Per model, alternating within every round and each timed over the whole set (host clock around work that ends in a device
 synchronise, after a warm-up pass that also captures the engine's graphs):
-  * ``eager``: eager ``forward_chunked_device`` of the transformed image plus one device-to-host copy of its packed detections;
+  * ``eager``: eager ``forward_chunked`` of the transformed image (one device-to-host copy of its packed detections, then BoxLists);
   * ``run_batches``: ``ChunkedEngine.run_batches`` over the same transformed images (device ImageLists);
   * ``run_images``: ``ChunkedEngine.run_images`` over the decoded uint8 images (upload and transform on its copy stream).
 Reports images/s and chunk-forwards/s per round, the engine's capture pass apart (captures, seconds, evictions, device memory per
@@ -27,7 +27,7 @@ import numpy as np
 import torch
 
 from mqdet_b200 import _lib
-from mqdet_b200.engine.inference import ChunkedEngine, chunked_to_boxlists
+from mqdet_b200.engine.inference import ChunkedEngine
 from mqdet_b200.engine.transforms import TestTransform, upload
 from tools import synth
 from tools.prof_gcp_queries import card
@@ -99,8 +99,7 @@ def profile(name, args, dev):
     def eager():
         res = []
         for il in pre:
-            pk = model.forward_chunked_device(il, caps, pmaps, cpp)["det_packed"].cpu()
-            res.append(chunked_to_boxlists(pk.transpose(0, 1).reshape(pk.shape[1], -1, 6), il.image_sizes, n)[0])
+            res.append(model.forward_chunked(il, caps, pmaps, cpp)[0])
         return res
 
     want = eager()
