@@ -6,9 +6,11 @@ from util import ROOT
 
 
 def _declared():
+    """name -> parameter count of every declaration, read with a regex of its own (not the loader's parser)."""
     src = open(os.path.join(ROOT, "include", "mqdet_b200.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(mqdet_[a-z0-9_]+)\s*\(", src)))
+    return {name: 0 if params.strip() in ("", "void") else params.count(",") + 1
+            for name, params in re.findall(r"\b(mqdet_[a-z0-9_]+)\s*\(([^)]*)\)", src)}
 
 
 def test_library_loads_and_exports_every_declared_symbol():
@@ -16,27 +18,44 @@ def test_library_loads_and_exports_every_declared_symbol():
     lib = _lib.load()  # binds every name in SIGNATURES; AttributeError if one is missing
     declared = _declared()
     assert declared, "no declarations parsed"
-    assert sorted(_lib.SIGNATURES) == declared, (sorted(set(declared) ^ set(_lib.SIGNATURES)))
+    assert sorted(_lib.SIGNATURES) == sorted(declared), (sorted(set(declared) ^ set(_lib.SIGNATURES)))
+    assert {k: len(v[1]) for k, v in _lib.SIGNATURES.items()} == declared
     for name in declared:
         assert hasattr(lib, name)
     assert lib.mqdet_version() >= 100
     assert lib.mqdet_ml_nms_workspace_bytes(5000) > 5000 * 79 * 8
 
 
+def test_header_types_without_a_binding_raise():
+    import ctypes
+    import pytest
+    from mqdet_b200 import _lib
+    sigs = _lib.parse_header("const char* mqdet_a(void);\nvoid mqdet_b(const float* x, int64_t n,\n    int k, void* stream);")
+    assert sigs == {"mqdet_a": (ctypes.c_char_p, []),
+                    "mqdet_b": (None, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_void_p])}
+    with pytest.raises(_lib.MqdetError, match=r"mqdet_c.*double"):
+        _lib.parse_header("int mqdet_c(const float* x, double scale, void* stream);")
+    with pytest.raises(_lib.MqdetError, match=r"mqdet_d.*size_t"):
+        _lib.parse_header("size_t mqdet_d(void);")
+
+
 def test_gemm_args_struct_matches_header_field_order():
+    import ctypes
     from mqdet_b200 import _lib
     src = open(os.path.join(ROOT, "include", "mqdet_b200.h")).read()
     body = src[src.index("typedef struct mqdet_gemm_args {"):src.index("} mqdet_gemm_args;")]
     body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    names = []
+    scalar = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "float": ctypes.c_float}
+    fields = []
     for decl in body.split("{", 1)[1].split(";"):
         decl = decl.strip()
         if not decl:
             continue
+        ctype = ctypes.c_void_p if "*" in decl else scalar[decl.split()[0]]
         parts = decl.replace("*", " ").split(",")
-        names.append(parts[0].split()[-1])
-        names.extend(p.strip() for p in parts[1:])
-    assert names == [f[0] for f in _lib.GemmArgs._fields_]
+        fields.append((parts[0].split()[-1], ctype))
+        fields.extend((p.strip(), ctype) for p in parts[1:])
+    assert fields == list(_lib.GemmArgs._fields_)
 
 
 def test_product_path_never_imports_the_oracle():
