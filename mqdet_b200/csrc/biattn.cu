@@ -5,11 +5,13 @@
 //                         column-max partials (for the text side) -> masked row softmax over the T tokens in the accumulator
 //                         fragments -> P (fp16, registers: the A operand of the next wgmma) -> P . mT_h, summed over the heads
 //                         -> v' = residual + gamma * (acc + bias).  Neither the scores nor the per-head context reach HBM.
-//   biattn_text_kernel  : text -> image side (one CTA per (image, head, 64 text tokens), streams all image tokens):
+//   biattn_text_kernel  : text -> image side (one CTA per (image, head, 128 text tokens): a TMA producer warpgroup streams all
+//                         image tokens through a ring to two consumer warpgroups of 64 text tokens each):
 //                         S^T recomputed on the tensor cores, exp(S^T - column max), P . V accumulated in registers, with
-//                         V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile): the value
-//                         projection is applied AFTER the token reduction (sum_n p[n] = 1), and the column sums are
-//                         accumulated in-kernel, so the [B, E, N] value tensor of the image side is never built.
+//                         V = the layer-normed image tokens themselves (read MN-major from the same [n x c] tile, loaded once
+//                         when q is those tokens): the value projection is applied AFTER the token reduction (sum_n p[n] = 1),
+//                         and the column sums are accumulated in-kernel, so the [B, E, N] value tensor of the image side is
+//                         never built.
 // Each MMA warpgroup keeps a 64 x 256 fp32 accumulator in its registers (128 per thread).  Operands arrive by TMA (128B swizzle);
 // accumulator fragment: row / column of element i of thread t = wg_row / wg_col.
 #include "common.cuh"
@@ -42,98 +44,141 @@ __device__ __forceinline__ float quad_sum(float v) {
 // =====================================================================================================================
 // Fused text -> image side of the bi-directional attention (BiMultiHeadAttention, fuse_helper.py:257-275, 289-291):
 //     out[t, :] = sum_n softmax_n(clamp(k_t . q_n + rowbias_t)) * vn[n, :]   per (image, head), t = text token, n = image token
-// One CTA (one warpgroup, two-stage ring) per (z, 64 text tokens).  The transposed probabilities [T, N] never reach HBM.
-// Per step of 64 image tokens:
+// One CTA per (z, 128 text tokens), 384 threads.  The transposed probabilities [T, N] never reach HBM.
+//   warpgroup 0     : producer.  One thread loads the K tiles once, then streams the image tokens 64 at a time through a ring
+//                     with a full and an empty mbarrier per stage.  When q is vn itself (same memory, the head broadcast - the
+//                     fusion layers pass it so) a stage is ONE [64 n x 256 c] tile that serves as both operands: K-major as the
+//                     B operand of S^T, MN-major as the B operand of P . vn (5 stages).  Otherwise a stage carries the q tile
+//                     next to it (2 stages).
+//   warpgroups 1, 2 : consumers; warpgroup w owns the text tokens 64 w .. 64 w + 63 of the CTA: its resident K tile, its O
+//                     accumulator (64 x 256 fp32 in registers), its column sums and its epilogue.  A consumer whose tokens all
+//                     lie at or beyond T exits at once, and the empty barriers count only the active consumers.
+// Per step of 64 image tokens, per consumer:
 //     S^T   = K_tile (64 x 256, resident) . Q_step^T           16 wgmma 64x64x16
 //     P     = exp(clamp(S^T + rowbias) - colmax_t)             in the accumulator fragments -> fp16 A operand (registers)
 //     O    += P . vn_step                                        4 wgmma 64x256x16, O (64 x 256) in registers
 //     out   = O / colsum_t  -> fp16
+// The products are issued one step apart: S^T of step i + 1 goes to the tensor cores ahead of P . vn of step i, so the exps of
+// step i + 1 can run while P . vn of step i (and the other consumer's products) execute; a stage is released once the P . vn
+// that read it has retired.  Every sum keeps the order of one warpgroup walking the image tokens.
 // colmax comes from biattn_image_kernel (the column maxima of the same clamped fp32 scores), so no online rescaling is needed;
 // colsum is accumulated here from the fp32 scores.
 // =====================================================================================================================
-constexpr int BT_STEP = 64;  // image tokens per step
+constexpr int BT_STEP = 64;     // image tokens per step
+constexpr int BT_ROWS = 2 * BM;  // text tokens per CTA: one 64-token tile per consumer warpgroup
 struct BtCfg {
-  static constexpr int KT_BYTES = 4 * KB_BYTES;       // resident K tile: 4 k-blocks of [64 x 64]
-  static constexpr int Q_BYTES = 4 * KB_BYTES;        // Q step [64 n x 256 d]
-  static constexpr int V_BYTES = 256 * BT_STEP * 2;   // image-token tile [64 n x 256 c]
-  static constexpr int STAGE_BYTES = Q_BYTES + V_BYTES;
-  static constexpr int SMEM_BYTES = KT_BYTES + 2 * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int TILE_BYTES = 4 * KB_BYTES;    // [64 x 256] as four [64 x 64] k-blocks: a K tile or an image-token tile
+  static constexpr int RING_TILES = 5;               // 5 stages of one tile, or 2 stages of [vn tile | q tile]
+  static constexpr int SMEM_BYTES = 2 * TILE_BYTES + RING_TILES * TILE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 static_assert(BtCfg::SMEM_BYTES <= 232448, "biattn_text: dynamic shared memory above the 227 KB per-CTA limit");
+static_assert((1 + 2 * BtCfg::RING_TILES) * 8 <= 256, "biattn_text: barrier space");
 struct BtP {
   const float* stat;  // [Z][T] column max
   float clamp;
   int nb1, T, N, n_steps;
   int k_bc1, k_bc2, q_bc1, q_bc2, v_bc1, v_bc2;  // 1 -> batch coordinate pinned to 0
+  int q_is_vn;                                    // q and vn are the same tokens: one tile per stage serves both operands
   const float* rowbias;                           // optional [Z][T * rb_ld] additive score bias per text token (folded q bias)
   int rb_ld;
   __half* out;                                    // [nb2][nb1][T][256]
   long o_ld, o_b1, o_b2;
 };
 
-__global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_constant__ CUtensorMap tma_k,
+// keeps the compiler from reusing the A-fragment registers of an asynchronous wgmma before it has retired
+__device__ __forceinline__ void keep_a_live(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
+}
+
+__global__ void __launch_bounds__(384, 1) biattn_text_kernel(const __grid_constant__ CUtensorMap tma_k,
                                                              const __grid_constant__ CUtensorMap tma_q,
                                                              const __grid_constant__ CUtensorMap tma_v, const BtP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* kt = smem;
-  uint8_t* ring = kt + BtCfg::KT_BYTES;  // 2 x [Q step | V step]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + 2 * BtCfg::STAGE_BYTES);
+  uint8_t* kt = smem;                         // [2 consumers] K tiles
+  uint8_t* ring = kt + 2 * BtCfg::TILE_BYTES;  // stages of [vn tile] or [vn tile | q tile]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + BtCfg::RING_TILES * BtCfg::TILE_BYTES);
   uint64_t* kt_full = bars;
-  uint64_t* full = bars + 1;  // [2]
+  uint64_t* full = bars + 1;                 // [stages]
+  uint64_t* empty = full + BtCfg::RING_TILES;  // [stages]
 
-  const int tid = threadIdx.x;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int mt = blockIdx.x, z = blockIdx.y;
   const int z1 = z % p.nb1, z2 = z / p.nb1;
   const int NS = p.n_steps;
-  const int qz1 = p.q_bc1 ? 0 : z1, qz2 = p.q_bc2 ? 0 : z2, vz1 = p.v_bc1 ? 0 : z1, vz2 = p.v_bc2 ? 0 : z2;
-
-  auto issue = [&](int i) {  // Q and V of step i into stage i & 1
-    uint8_t* st = ring + (i & 1) * BtCfg::STAGE_BYTES;
-    uint64_t* bar = &full[i & 1];
-    mbar_expect_tx(bar, BtCfg::STAGE_BYTES);
-    for (int kb = 0; kb < 4; ++kb) tma_load_4d(st + kb * KB_BYTES, &tma_q, bar, kb * BK, i * BT_STEP, qz1, qz2);
-    // image tokens themselves, [64 n x 256 c] as four [64 n x 64 c] blocks: the B operand of P.vn is read MN-major
-    for (int cb = 0; cb < 4; ++cb) tma_load_4d(st + BtCfg::Q_BYTES + cb * KB_BYTES, &tma_v, bar, cb * BK, i * BT_STEP, vz1, vz2);
-  };
-  if (tid == 0) {
+  const int nact = p.T - mt * BT_ROWS > BM ? 2 : 1;  // consumers with at least one text token
+  const int stage_bytes = (p.q_is_vn ? 1 : 2) * BtCfg::TILE_BYTES;
+  const int stages = p.q_is_vn ? BtCfg::RING_TILES : BtCfg::RING_TILES / 2;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_k);
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_v);
     mbar_init(kt_full, 1);
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 128 * nact);  // every thread of each active consumer releases every stage
+    }
     fence_mbar_init();
-    mbar_expect_tx(kt_full, BtCfg::KT_BYTES);
-    for (int kb = 0; kb < 4; ++kb)
-      tma_load_4d(kt + kb * KB_BYTES, &tma_k, kt_full, kb * BK, mt * BM, p.k_bc1 ? 0 : z1, p.k_bc2 ? 0 : z2);
-    issue(0);
-    if (NS > 1) issue(1);
   }
   __syncthreads();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (tid == 0) {
+      mbar_expect_tx(kt_full, nact * BtCfg::TILE_BYTES);
+      for (int w = 0; w < nact; ++w)
+        for (int kb = 0; kb < 4; ++kb)
+          tma_load_4d(kt + w * BtCfg::TILE_BYTES + kb * KB_BYTES, &tma_k, kt_full, kb * BK, mt * BT_ROWS + w * BM,
+                      p.k_bc1 ? 0 : z1, p.k_bc2 ? 0 : z2);
+      const int qz1 = p.q_bc1 ? 0 : z1, qz2 = p.q_bc2 ? 0 : z2, vz1 = p.v_bc1 ? 0 : z1, vz2 = p.v_bc2 ? 0 : z2;
+      int s = 0;
+      uint32_t ph = 0;
+      for (int i = 0; i < NS; ++i) {
+        mbar_wait(&empty[s], ph ^ 1);
+        uint8_t* st = ring + s * stage_bytes;
+        mbar_expect_tx(&full[s], stage_bytes);
+        // image tokens [64 n x 256 c] as four [64 n x 64 c] blocks
+        for (int cb = 0; cb < 4; ++cb) tma_load_4d(st + cb * KB_BYTES, &tma_v, &full[s], cb * BK, i * BT_STEP, vz1, vz2);
+        if (!p.q_is_vn)
+          for (int kb = 0; kb < 4; ++kb)
+            tma_load_4d(st + BtCfg::TILE_BYTES + kb * KB_BYTES, &tma_q, &full[s], kb * BK, i * BT_STEP, qz1, qz2);
+        if (++s == stages) {
+          s = 0;
+          ph ^= 1;
+        }
+      }
+    }
+    return;
+  }
+  const int w = wg - 1;
+  if (w >= nact) return;
+  setmaxnreg_inc<232>();
+  const int t0 = mt * BT_ROWS + w * BM;  // first text token of this consumer
 
   // the two text tokens (rows) of this thread
   constexpr float L2E = 1.4426950408889634f;
   float m_l2[2] = {0.f, 0.f}, inv[2] = {0.f, 0.f}, gb[2] = {0.f, 0.f}, lsum[2] = {0.f, 0.f};
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int t = mt * BM + wg_row(tid, 2 * h);
+    const int t = t0 + wg_row(tid, 2 * h);
     if (t < p.T) {
       m_l2[h] = -p.stat[(long)z * p.T + t] * L2E;
       if (p.rowbias) gb[h] = p.rowbias[((long)z * p.T + t) * p.rb_ld];
     }
   }
   const float clampv = p.clamp > 0.f ? p.clamp : 3.0e38f;
-  const uint32_t kt_addr = smem_u32(kt);
+  const uint32_t kt_addr = smem_u32(kt + w * BtCfg::TILE_BYTES), ring_addr = smem_u32(ring);
+  const uint32_t q_off = p.q_is_vn ? 0 : BtCfg::TILE_BYTES;
   float o[128];
 #pragma unroll
   for (int i = 0; i < 128; ++i) o[i] = 0.f;
-  mbar_wait(kt_full, 0);
-  for (int i = 0; i < NS; ++i) {
-    const int s = i & 1;
-    mbar_wait(&full[s], (i >> 1) & 1);
-    const uint32_t q0 = smem_u32(ring + s * BtCfg::STAGE_BYTES), v0 = q0 + BtCfg::Q_BYTES;
-    float sc[32];
+  float sc[32];
+  // S^T of the image-token tile in stage s -> sc (committed, not waited for)
+  auto scores = [&](int s) {
+    const uint32_t q0 = ring_addr + s * stage_bytes + q_off;
 #pragma unroll
     for (int j = 0; j < 32; ++j) sc[j] = 0.f;
     wgmma_fence_acc(sc);
@@ -144,7 +189,9 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
       for (int k = 0; k < 4; ++k)
         wgmma_ss_m64n64_kk(sc, wg_desc_k_sw128(kt_addr + kb * KB_BYTES + k * 32), wg_desc_k_sw128(q0 + kb * KB_BYTES + k * 32), 1);
     wgmma_commit();
-    wgmma_wait<0>();
+  };
+  // retired scores of step i -> e = exp(...), column sums, and the fp16 A fragments of P . vn
+  auto probs = [&](int i, uint32_t (&pa)[4][4]) {
     wgmma_fence_acc(sc);
     const int nrem = p.N - i * BT_STEP;  // valid image tokens of this step
 #pragma unroll
@@ -156,9 +203,12 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
       lsum[h] += e;
       sc[j] = e;
     }
-    uint32_t pa[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) acc_to_a(sc, kk, pa[kk]);
+  };
+  // O += P . vn of the tile in stage s (committed, not waited for)
+  auto pv = [&](int s, const uint32_t (&pa)[4][4]) {
+    const uint32_t v0 = ring_addr + s * stage_bytes;
     wgmma_fence_acc(o);
     wgmma_fence();
 #pragma unroll
@@ -168,11 +218,38 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
       wgmma_rs_m64n256_kmn(o, pa[kk], wg_desc_mn_sw128(v0 + kk * 2048, KB_BYTES, 1024), 1);
     }
     wgmma_commit();
+  };
+  uint32_t pa[4][4];
+  mbar_wait(kt_full, 0);
+  mbar_wait(&full[0], 0);
+  scores(0);
+  wgmma_wait<0>();
+  probs(0, pa);
+  int s = 0;
+  uint32_t ph = 0;
+  for (int i = 0; i + 1 < NS; ++i) {
+    const int sn = s + 1 == stages ? 0 : s + 1;
+    const uint32_t phn = sn == 0 ? ph ^ 1 : ph;
+    mbar_wait(&full[sn], phn);
+    scores(sn);
+    pv(s, pa);
+    wgmma_wait<1>();  // S^T of step i + 1 has retired; P . vn of step i may still run
+    uint32_t pn[4][4];
+    probs(i + 1, pn);
     wgmma_wait<0>();
     wgmma_fence_acc(o);
-    __syncthreads();  // every wgmma of the warpgroup has read stage s
-    if (tid == 0 && i + 2 < NS) issue(i + 2);
+    keep_a_live(pa);
+    mbar_arrive(&empty[s]);  // P . vn of step i has read stage s
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) pa[kk][r] = pn[kk][r];
+    s = sn;
+    ph = phn;
   }
+  pv(s, pa);
+  wgmma_wait<0>();
+  wgmma_fence_acc(o);
   // total column sum of this text token: the four threads of a quad hold its columns
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -184,7 +261,7 @@ __global__ void __launch_bounds__(128, 1) biattn_text_kernel(const __grid_consta
 #pragma unroll
   for (int j = 0; j < 128; j += 2) {
     const int h = (j >> 1) & 1;
-    const int t = mt * BM + wg_row(tid, j);
+    const int t = t0 + wg_row(tid, j);
     if (t < p.T)
       *reinterpret_cast<__half2*>(out + (long)t * p.o_ld + wg_col(tid, j)) = __floats2half2_rn(o[j] * inv[h], o[j + 1] * inv[h]);
   }
@@ -513,11 +590,21 @@ extern "C" int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, i
   memset(&p, 0, sizeof(p));
   int rc = make_operand_map(&mk, k, T, 256, k_ld, (int)nb1, k_b1, (int)nb2, k_b2, BM, &p.k_bc1, &p.k_bc2);
   if (rc) return rc;
-  rc = make_operand_map(&mq, q, N, 256, q_ld, (int)nb1, q_b1, (int)nb2, q_b2, BT_STEP, &p.q_bc1, &p.q_bc2);
-  if (rc) return rc;
   // image tokens [N][256 c]: box [64 n x 64 c]
   rc = make_operand_map(&mv, vn, N, 256, vn_ld, (int)nb1, vn_b1, (int)nb2, vn_b2, BT_STEP, &p.v_bc1, &p.v_bc2);
   if (rc) return rc;
+  // q is vn itself when both address the same elements for every (image, head): then the kernel loads one tile per step
+  const bool same_b1 = (q_b1 == 0 || nb1 == 1) ? (vn_b1 == 0 || nb1 == 1) : q_b1 == vn_b1;
+  const bool same_b2 = (q_b2 == 0 || nb2 == 1) ? (vn_b2 == 0 || nb2 == 1) : q_b2 == vn_b2;
+  p.q_is_vn = q == vn && q_ld == vn_ld && same_b1 && same_b2;
+  if (p.q_is_vn) {
+    mq = mv;
+    p.q_bc1 = p.v_bc1;
+    p.q_bc2 = p.v_bc2;
+  } else {
+    rc = make_operand_map(&mq, q, N, 256, q_ld, (int)nb1, q_b1, (int)nb2, q_b2, BT_STEP, &p.q_bc1, &p.q_bc2);
+    if (rc) return rc;
+  }
   MQ_REQUIRE((nb1 == 1 || o_b1 != 0) && (nb2 == 1 || o_b2 != 0), "biattn_text_vn: output batch strides must be non-zero");
   p.out = (__half*)out;
   p.o_ld = o_ld;
@@ -531,10 +618,10 @@ extern "C" int mqdet_biattn_text_vn(const void* k, int64_t k_ld, int64_t k_b1, i
   p.n_steps = (int)((N + BT_STEP - 1) / BT_STEP);
   p.rowbias = rowbias;
   p.rb_ld = (int)(rb_ld > 0 ? rb_ld : 1);
-  dim3 grid((unsigned)((T + BM - 1) / BM), (unsigned)(nb1 * nb2));
+  dim3 grid((unsigned)((T + BT_ROWS - 1) / BT_ROWS), (unsigned)(nb1 * nb2));
   rc = ensure_dyn_smem(reinterpret_cast<const void*>(&biattn_text_kernel), BtCfg::SMEM_BYTES);
   if (rc) return rc;
-  biattn_text_kernel<<<grid, 128, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
+  biattn_text_kernel<<<grid, 384, BtCfg::SMEM_BYTES, (cudaStream_t)stream>>>(mk, mq, mv, p);
   return check_launch("biattn_text_kernel");
 }
 
