@@ -36,6 +36,18 @@ __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
+// one step of a transposing max-butterfly over the lanes that differ in bit `mask`: the lane with that bit set keeps the upper
+// n values, the other the lower n, and each takes the maximum with the half its partner sends; the result is in v[0 .. n)
+template <int n>
+__device__ __forceinline__ void butterfly_max(float (&v)[32], int lane, int mask) {
+  const bool hi = lane & mask;
+#pragma unroll
+  for (int k = 0; k < n; ++k) {
+    const float send = hi ? v[k] : v[k + n];
+    const float keep = hi ? v[k + n] : v[k];
+    v[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, mask));
+  }
+}
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
@@ -426,19 +438,31 @@ __global__ void __launch_bounds__(384, 1) biattn_image_kernel(const __grid_const
     wgmma_wait<0>();
     wgmma_fence_acc(sc);
     mbar_arrive(&empty[(qh + 3) % STAGES]);
+    // rows at or beyond N (in the last tile of an image only) drop out of the column maxima as -inf.  Nothing else reads their
+    // scores: a row's softmax and its P . mT row use only its own scores, and its output is never written
+    if (m0 + BM > p.N) {
+#pragma unroll
+      for (int j = 0; j < 64; ++j)
+        if (!valid[(j >> 1) & 1]) sc[j] = NEG_INF;
+    }
     // ---- column maxima over the tile's valid rows (for the text side): two rows per thread, then the 8 row groups of the warp,
     //      then the 4 warps of the warpgroup through shared memory.  The +-5e4 clamp (fuse_helper.py:245-252) is applied to the
     //      REDUCED values (clamp is monotonic) ----
+    {
+      // cm[k]: column 8 (k >> 1) + 2 (lane & 3) + (k & 1).  The row groups meet in a transposing butterfly: at the xor-(4 << st)
+      // step a lane keeps one half of its columns, sends the other half to its partner and takes the maximum with what the
+      // partner sends, so after three steps it holds the warp's maxima of 4 of the 32 columns (28 shuffles, where reducing each
+      // column on its own takes 96)
+      float cm[32];
 #pragma unroll
-    for (int j = 0; j < 64; j += 4) {
+      for (int k = 0; k < 32; ++k) cm[k] = fmaxf(sc[4 * (k >> 1) + (k & 1)], sc[4 * (k >> 1) + 2 + (k & 1)]);
+      butterfly_max<16>(cm, lane, 4);
+      butterfly_max<8>(cm, lane, 8);
+      butterfly_max<4>(cm, lane, 16);
+      // cm[k] (k < 4) now holds column index k + 4 b2 + 8 b1 + 16 b0 of the 32, b_i = bit i of lane >> 2
+      const int k0 = 16 * ((lane >> 2) & 1) + 8 * ((lane >> 3) & 1) + 4 * ((lane >> 4) & 1);
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        float m = fmaxf(valid[0] ? sc[j + c] : NEG_INF, valid[1] ? sc[j + 2 + c] : NEG_INF);
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-        if (lane < 4) cw[warp * 128 + wg_col(tid, j + c)] = m;
-      }
+      for (int k = 0; k < 4; ++k) cw[warp * 128 + 8 * ((k0 + k) >> 1) + 2 * (lane & 3) + (k & 1)] = cm[k];
     }
     // ---- row softmax over the T tokens; `kk` carries the folded query bias and the token mask as an additive 0 / -inf.
     //      Each warpgroup holds half of a row; the halves meet in xmax / xpart / xsum ----
@@ -474,11 +498,14 @@ __global__ void __launch_bounds__(384, 1) biattn_image_kernel(const __grid_const
 #pragma unroll
     for (int j = 0; j < 64; ++j) {
       const int r = (j >> 1) & 1;
-      float ev = (sc[j] == NEG_INF) ? 0.f : ex2_approx(fmaf(fminf(fmaxf(sc[j], -clampv), clampv), L2E, -ml2[r]));
-      // every token of the image masked (the row maximum is -inf for every row of the tile): the reference's fp32 sum
-      // A + (-9e15) swallows A and the softmax is uniform over the T tokens
-      if (uniform) ev = (t0 + wg_col(tid, j) < p.T) ? 1.f : 0.f;
-      sc[j] = ev;
+      sc[j] = (sc[j] == NEG_INF) ? 0.f : ex2_approx(fmaf(fminf(fmaxf(sc[j], -clampv), clampv), L2E, -ml2[r]));
+    }
+    // every token of the image masked (the row maximum is -inf for every row of the tile): the reference's fp32 sum
+    // A + (-9e15) swallows A and the softmax is uniform over the T tokens
+    if (__any_sync(0xffffffffu, uniform)) {
+#pragma unroll
+      for (int j = 0; j < 64; ++j)
+        if (uniform) sc[j] = (t0 + wg_col(tid, j) < p.T) ? 1.f : 0.f;
     }
     // row sum: the thread of warpgroup 1 continues the sequential sum of the same thread of warpgroup 0 (the same rows, the
     // columns 128 further), then the four threads of a row combine
@@ -540,22 +567,28 @@ __global__ void __launch_bounds__(384, 1) biattn_image_kernel(const __grid_const
     for (int j = 0; j < 64; ++j) dsum[j] = (h == 0 ? 0.f : dsum[j]) + dh[j];
   }
   // ================= epilogue: out = res + gamma * (Dsum + bias) on this warpgroup's 128 columns =================
+  // elements j, j + 1 (row0) and j + 2, j + 3 (row0 + 8) share the columns c, c + 1 and their gamma / bias
+  const __half* res = p.res ? p.res + (long)b * p.res_b : nullptr;
+  __half* out = p.out + (long)b * p.o_b;
 #pragma unroll
-  for (int j = 0; j < 64; j += 2) {
-    const long row = m0 + wg_row(tid, j);
+  for (int j = 0; j < 64; j += 4) {
     const int c = t0 + wg_col(tid, j);
-    if (row >= p.N) continue;
-    float o0 = dsum[j], o1 = dsum[j + 1];
-    const float g0 = p.gamma ? p.gamma[c] : 1.f, g1 = p.gamma ? p.gamma[c + 1] : 1.f;
-    const float b0 = p.bias ? p.bias[c] : 0.f, b1 = p.bias ? p.bias[c + 1] : 0.f;
-    o0 = (o0 + b0) * g0;  // gamma * (D + bias)
-    o1 = (o1 + b1) * g1;
-    if (p.res) {
-      const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.res + (long)b * p.res_b + row * p.res_ld + c));
-      o0 += r.x;
-      o1 += r.y;
+    const float2 g = p.gamma ? *reinterpret_cast<const float2*>(p.gamma + c) : make_float2(1.f, 1.f);
+    const float2 bi = p.bias ? *reinterpret_cast<const float2*>(p.bias + c) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const long row = m0 + row0 + 8 * r;
+      if (row >= p.N) continue;
+      // gamma * (D + bias), then + res, rounded step by step (never contracted into one fma)
+      float o0 = __fmul_rn(dsum[j + 2 * r] + bi.x, g.x);
+      float o1 = __fmul_rn(dsum[j + 2 * r + 1] + bi.y, g.y);
+      if (res) {
+        const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(res + row * p.res_ld + c));
+        o0 = __fadd_rn(o0, rv.x);
+        o1 = __fadd_rn(o1, rv.y);
+      }
+      *reinterpret_cast<__half2*>(out + row * p.o_ld + c) = __floats2half2_rn(o0, o1);
     }
-    *reinterpret_cast<__half2*>(p.out + (long)b * p.o_b + row * p.o_ld + c) = __floats2half2_rn(o0, o1);
   }
 }
 
