@@ -640,6 +640,28 @@ int mqdet_query_bank_update(const float* feats, const int32_t* labels, const int
                             int32_t* bank_count, float* row_norm, int64_t L, int64_t cap, int64_t max_query, float sim_thr,
                             void* stream);
 
+/* ---- vision-query bank extraction over a dataset (tools/train_net.py:256-336, extract_query(exclude_similar=False)) (query_bank.cu)
+ *   mqdet_query_gt_rois     : ground-truth table (device, int32 words): per image b < B 8 words (first box, boxes n_b, arrival number
+ *                             of its first box, 0, then as f32 bits ratio_w, ratio_h, img_w - 1, img_h - 1), then boxes f32 [nbox][4]
+ *                             (x1, y1, x2, y2 in original-image coordinates), then labels i32 [nbox] -> rois f32 [nbox][5] = (image
+ *                             index, x1, y1, x2, y2), labels i32, arrival i32 (arrival of the first box + box index) and *count
+ *                             (device): each box resized (x * ratio_w, y * ratio_h; BoxList.resize), then grown and clipped exactly
+ *                             as mqdet_query_candidates does, the kept ones in image-then-box order.  One CTA.
+ *   mqdet_query_bank_append : mqdet_query_bank_update without the similarity test (a feature is appended whenever its label has fewer
+ *                             than max_query rows), that also stores arrival[i] in bank_arrival i32 [L][cap] beside each appended row.
+ *   mqdet_query_bank_merge  : parts = DEVICE table of G device pointers, part r = rows f32 [part_rows[r]][2 + C] = (label bits, arrival
+ *                             bits, feature), sorted by label then arrival; seg i32 [G][L][2] = (first row, rows) of each label in
+ *                             each part; arrivals distinct across parts.  Writes out f32 [L][max_query][C]: per label the first
+ *                             max_query rows of all parts in arrival order; the rest of out is untouched.  max_rows >= every
+ *                             part_rows[r] (host).  One warp per row. */
+int mqdet_query_gt_rois(const int32_t* table, int64_t B, int64_t nbox, float expand_ratio, float* rois, int32_t* labels,
+                        int32_t* arrival, int32_t* count, void* stream);
+int mqdet_query_bank_append(const float* feats, const int32_t* labels, const int32_t* arrival, const int32_t* count, int64_t C,
+                            float* bank, int32_t* bank_count, float* row_norm, int32_t* bank_arrival, int64_t L, int64_t cap,
+                            int64_t max_query, void* stream);
+int mqdet_query_bank_merge(const float* const* parts, const int32_t* seg, const int32_t* part_rows, int64_t max_rows, int64_t G,
+                           int64_t L, int64_t C, int64_t max_query, float* out, void* stream);
+
 /* ---- Box AP on the device (lvis_eval.cu): LVIS (lvis_eval.py: LvisEvaluatorFixedAP / LVISEval, both protocols) and COCO
  *      (od_eval.py + pycocotools COCOeval, bbox).  Where the protocols differ the rule is an argument, never a protocol switch.
  *   mqdet_lvis_collect : packed f32 [G][B][M + 1][6] detector rows (row M = (count, ...)) -> pool slots base + (b * G + g) * M + r:

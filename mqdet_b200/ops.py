@@ -828,6 +828,102 @@ def query_bank_update(bank, feats, labels, count, max_query, sim_thr):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# Vision-query bank extraction over a dataset: ground-truth boxes, the capped append, the merge of several ranks (csrc/query_bank.cu)
+# ----------------------------------------------------------------------------------------------------------------------
+QG_IMG = 8   # int32 words per image of the ground-truth table
+
+
+def query_gt_rois(images, expand_ratio, device):
+    """Ground-truth boxes of one batch -> (rois fp32 [nbox, 5], labels int32 [nbox], arrival int32 [nbox], count int32 [1]), nbox
+    = the boxes of all images.  ``images``: per image (boxes [n, 4] xyxy in original-image coordinates, labels [n], (w, h) original,
+    (w, h) resized, arrival number of its first box), host tensors.  On the device each box is resized (BoxList.resize: x * fp32(w'
+    / w), y * fp32(h' / h)), grown by ``expand_ratio`` about its centre and clipped to the resized image, the empty ones removed; the
+    kept rows come first, in image-then-box order, and carry arrival = that of the image's first box + the box's index.  The table
+    crosses to the device in one asynchronous copy from pinned memory; nothing is read on the host."""
+    import numpy as np
+    B = len(images)
+    if B == 0:
+        raise _lib.MqdetError("query_gt_rois: no images")
+    ns = [int(bx.shape[0]) for bx, *_ in images]
+    nbox = sum(ns)
+    table = np.zeros((B * QG_IMG + 5 * nbox,), dtype=np.int32)
+    head = table[:B * QG_IMG].reshape(B, QG_IMG)
+    boxes = table[B * QG_IMG:B * QG_IMG + 4 * nbox].view(np.float32).reshape(nbox, 4)
+    labels = table[B * QG_IMG + 4 * nbox:]
+    off = 0
+    for b, ((bx, lab, (w, h), (rw, rh), arr0), n) in enumerate(zip(images, ns)):
+        if tuple(bx.shape) != (n, 4) or tuple(lab.shape) != (n,):
+            raise _lib.MqdetError(f"query_gt_rois: image {b}: boxes [n, 4] and labels [n] required (got {tuple(bx.shape)}, "
+                                  f"{tuple(lab.shape)})")
+        if not (0 < w and 0 < h and 0 < rw < (1 << 24) and 0 < rh < (1 << 24)):
+            raise _lib.MqdetError(f"query_gt_rois: image {b}: bad sizes {w}x{h} -> {rw}x{rh}")
+        if not (0 <= int(arr0) and int(arr0) + n < (1 << 31)):
+            raise _lib.MqdetError(f"query_gt_rois: image {b}: arrival numbers {arr0} + {n} outside int32")
+        ratios = np.array([float(rw) / float(w), float(rh) / float(h), rw - 1, rh - 1], dtype=np.float32)   # fp64 ratio, rounded
+        head[b, :3] = (off, n, int(arr0))
+        head[b, 4:] = ratios.view(np.int32)
+        boxes[off:off + n] = bx.detach().to("cpu", torch.float32).numpy()
+        labels[off:off + n] = lab.detach().to("cpu", torch.int64).numpy()
+        off += n
+    t = upload_async(torch.from_numpy(table), device)
+    cap = max(nbox, 1)                                        # an empty tensor has no storage to point at
+    rois = torch.empty((cap, 5), dtype=torch.float32, device=device)
+    lab_out = torch.empty((cap,), dtype=torch.int32, device=device)
+    arrival = torch.empty((cap,), dtype=torch.int32, device=device)
+    count = torch.empty((1,), dtype=torch.int32, device=device)
+    _launch("mqdet_query_gt_rois", _ptr(t), B, nbox, float(expand_ratio), _ptr(rois), _ptr(lab_out), _ptr(arrival), _ptr(count),
+            what="query_gt_rois")
+    return rois[:nbox], lab_out[:nbox], arrival[:nbox], count
+
+
+def query_bank_append(bank, feats, labels, arrival, count, max_query, bank_arrival):
+    """``query_bank_update`` without the similarity test, as extract_query(exclude_similar=False) appends: each of the first
+    ``count`` features goes to its label's rows unless the label already has ``max_query``.  The feature's arrival number (int32,
+    one per feature) is stored beside its row in ``bank_arrival`` (int32 [L, cap]).  One launch, no host read."""
+    _need_cuda(feats, labels, arrival, count, bank_arrival)
+    if feats.dtype != torch.float32 or not feats.is_contiguous() or feats.dim() != 2 or feats.shape[1] != bank.C:
+        raise _lib.MqdetError(f"query_bank_append: contiguous fp32 features [cap, {bank.C}] required")
+    for t in (labels, arrival):
+        if t.dtype != torch.int32 or t.numel() != feats.shape[0]:
+            raise _lib.MqdetError("query_bank_append: int32 labels and arrival numbers (one per feature) required")
+    if count.dtype != torch.int32 or count.numel() != 1:
+        raise _lib.MqdetError("query_bank_append: an int32 count [1] required")
+    if bank_arrival.dtype != torch.int32 or tuple(bank_arrival.shape) != (bank.L, bank.cap) or not bank_arrival.is_contiguous():
+        raise _lib.MqdetError(f"query_bank_append: contiguous int32 bank_arrival [{bank.L}, {bank.cap}] required")
+    if not 0 <= int(max_query) <= bank.cap:
+        raise _lib.MqdetError(f"query_bank_append: max_query {max_query} outside [0, {bank.cap}]")
+    _launch("mqdet_query_bank_append", _ptr(feats), _ptr(labels), _ptr(arrival), _ptr(count), bank.C, _ptr(bank.rows),
+            _ptr(bank.count), _ptr(bank.norm), _ptr(bank_arrival), bank.L, bank.cap, int(max_query), what="query_bank_append")
+    return bank
+
+
+def query_bank_merge(parts, counts, max_query, C):
+    """Several ranks' capped banks -> the one bank a single rank builds over all their rows: fp32 [L, max_query, C] and the rows in
+    use per label (host int64 [L]).  ``parts``: per rank the rows fp32 [n_r, 2 + C] = (label bits, arrival bits, feature), sorted by
+    label then arrival (device); ``counts``: host int [G, L], rank r's rows of each label.  Per label the rows of all ranks are taken
+    in arrival order and the first ``max_query`` kept; arrivals must be distinct across ranks."""
+    _need_cuda(*parts)
+    counts = torch.as_tensor(counts, dtype=torch.int64)
+    G, L = counts.shape
+    if len(parts) != G or G == 0:
+        raise _lib.MqdetError(f"query_bank_merge: {len(parts)} parts for counts of {G} ranks")
+    for r, p in enumerate(parts):
+        n = int(counts[r].sum())
+        if p.dtype != torch.float32 or not p.is_contiguous() or tuple(p.shape) != (n, 2 + C):
+            raise _lib.MqdetError(f"query_bank_merge: part {r} must be contiguous fp32 [{n}, {2 + C}] (got {p.dtype} {tuple(p.shape)})")
+    dev = parts[0].device
+    first = torch.cumsum(counts, 1) - counts
+    seg = torch.stack([first, counts], 2).to(torch.int32).contiguous()
+    rows = counts.sum(1)
+    ptrs = torch.tensor([p.data_ptr() for p in parts], dtype=torch.int64)
+    out = torch.zeros((L, max_query, C), dtype=torch.float32, device=dev)
+    seg_d, rows_d, ptrs_d = (upload_async(t, dev) for t in (seg, rows.to(torch.int32), ptrs))
+    _launch("mqdet_query_bank_merge", _ptr(ptrs_d), _ptr(seg_d), _ptr(rows_d), int(rows.max()), G, L, C, int(max_query), _ptr(out),
+            what="query_bank_merge")
+    return out, counts.sum(0).clamp(max=int(max_query))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # DyHead vision path
 # ----------------------------------------------------------------------------------------------------------------------
 class Levels:
